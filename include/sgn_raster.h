@@ -248,7 +248,8 @@ typedef struct sgn_blend_fwd_out {
     float* raw;            /* [H,W,4] saved for backward */
     float* final_T;        /* [3,H,W] planar: slot 0 main, 1 object, 2 background */
     int32_t* final_idx;    /* [3,H,W] */
-    int32_t* tile_depth;   /* [3,tiles] entries traversed per tile (main, object, background pass); sizes the backward */
+    int32_t* tile_depth;   /* [3,tiles] entries traversed per tile: main; object entries walked past the main traversal;
+                              background pass.  Sizes the backward */
     int32_t* sched;        /* scratch of sgn_blend_sched_ints(tiles) int32, or NULL: heavy-first work lists (longest tile
                               lists are scheduled first; without it CTAs take the tiles in raster order) */
     float* staged;         /* scratch of 12 * M floats (16-byte aligned) for SGN_TUNE_FWD_TMA, or NULL */

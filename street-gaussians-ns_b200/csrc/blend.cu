@@ -3,10 +3,13 @@
 // One traversal of each tile's depth-sorted list produces what the reference obtains from two gsplat
 // rasterize_gaussians calls (street_gaussians_ns/sgn_splatfacto.py:954-996: rgb+alpha and the depth
 // pass), with gsplat's skip and termination rules (SURVEY.md Appendix A.6).  The objects-only and
-// background-only accumulations (street_gaussians_ns/sgn_splatfacto_scene_graph.py:364-366) are
-// accumulation-only traversals of the compacted per-tile class sub-lists (binning.cu), which is
-// what the reference's subset re-renders see.  The reference's post-ops (:968-975, :995) run in
-// the epilogue.
+// background-only accumulations (street_gaussians_ns/sgn_splatfacto_scene_graph.py:364-366) see the
+// compacted per-tile class sub-lists (binning.cu), which is what the reference's subset re-renders see.
+// The objects-only one rides along in the main traversal (same alphas, a second transmittance advanced
+// by the object entries only) and finishes on the object sub-list where the main streams ended; its
+// gradient is folded into the main backward's reduction.  The background-only one is a separate
+// accumulation-only traversal of the pixels an object entry took part in.  The reference's post-ops
+// (:968-975, :995) run in the epilogue.
 //
 // Execution shape (H100): the loops are FP32/MUFU issue-bound, not HBM-bound, so the
 // design minimises instructions per (pixel, Gaussian) pair:
@@ -25,13 +28,15 @@
 // Sorted payloads carry the Gaussian row in bits 0-30 and the object-class flag in bit 31.
 #include "sgn_common.cuh"
 
+#include <type_traits>
+
 // Resident CTAs per SM the compiler must leave room for (register budget = 65536 / (32 * N) per thread); one warp per CTA, at
 // most 32 CTAs per SM.  -maxrregcount is ignored for kernels with launch bounds, so the occupancy experiments go through these.
 #ifndef BLEND_FWD_MIN_BLOCKS
-#define BLEND_FWD_MIN_BLOCKS 1
+#define BLEND_FWD_MIN_BLOCKS 16  // 128 registers: the objects-only stream would otherwise take the main forward to ~150
 #endif
 #ifndef BLEND_BWD_MIN_BLOCKS
-#define BLEND_BWD_MIN_BLOCKS 1
+#define BLEND_BWD_MIN_BLOCKS 12  // 168 registers: the folded objects-only gradient would otherwise take it to 178 (11 CTAs)
 #endif
 #ifndef BLEND_ACC_MIN_BLOCKS
 #define BLEND_ACC_MIN_BLOCKS 1
@@ -259,11 +264,11 @@ __device__ __forceinline__ int strips_for(int len, int t1) { return len <= t1 ? 
 extern "C" size_t sgn_blend_sched_ints(int tiles) { return 3 * SCHED_STRIDE(tiles > 0 ? tiles : 0); }
 
 __global__ void __launch_bounds__(1024)
-sched_kernel(int tiles, const int2* __restrict__ tile_bins, const int2* __restrict__ cls_bins0, const int2* __restrict__ cls_bins1,
-             const int32_t* __restrict__ tile_depth /* backward: lengths come from here */, int split_main, int split_acc,
-             int32_t* __restrict__ sched) {
-    const int kind = blockIdx.x;  // 0 main, 1 object, 2 background
-    const int2* bins = kind == SLOT_MAIN ? tile_bins : (kind == SLOT_OBJ ? cls_bins1 : cls_bins0);
+sched_kernel(int tiles, const int2* __restrict__ tile_bins, const int2* __restrict__ cls_bins0,
+             const int32_t* __restrict__ tile_depth /* backward: lengths come from here */, int fuse_obj, int split_main,
+             int split_acc, int32_t* __restrict__ sched) {
+    const int kind = blockIdx.x ? SLOT_BG : SLOT_MAIN;  // the objects-only pass is part of the main one
+    const int2* bins = kind == SLOT_MAIN ? tile_bins : cls_bins0;
     const int split = kind == SLOT_MAIN ? split_main : split_acc;
     int32_t* out = sched + kind * SCHED_STRIDE(tiles);
     // per-warp histograms / cursors: the tiles of a frame fall into a handful of length buckets, and 9600 shared-memory
@@ -277,7 +282,10 @@ sched_kernel(int tiles, const int2* __restrict__ tile_bins, const int2* __restri
     // colour, zero accumulation, v_sky); only the accumulation backward has nothing to do there
     const bool visit_empty = !tile_depth || kind == SLOT_MAIN;
     auto length = [&](int t) {
-        if (tile_depth) return tile_depth[(size_t)kind * tiles + t];
+        if (tile_depth) {  // backward: with fuse_obj the main traversal also walks the objects-only streams' residual
+            const int d = tile_depth[(size_t)kind * tiles + t];
+            return kind == SLOT_MAIN && fuse_obj ? d + tile_depth[(size_t)SLOT_OBJ * tiles + t] : d;
+        }
         const int2 r = bins[t];
         return r.y - r.x;
     };
@@ -329,301 +337,20 @@ __device__ __forceinline__ bool take_work(const int32_t* __restrict__ sched, int
     return true;
 }
 
-template <int PPL, bool CLS, bool SKIP, bool PACK, bool TMA = false>
-__device__ __forceinline__ void blend_fwd_strip(const BlendFwdParams& p, int tile, int strip, const int2 range,
-                                                float4 (*sA)[32], float4 (*sB)[32], float4 (*sC)[32],
-                                                float4 (*sE)[96] = nullptr, uint64_t* mbar = nullptr) {
-    const int tx = tile % p.tiles_x, ty = tile / p.tiles_x;
-    const int lane = threadIdx.x;
-    const int j = tx * SGN_TILE + (lane & 15);
-    const int i0 = ty * SGN_TILE + strip * (2 * PPL) + (lane >> 4);
-    const float px = (float)j + 0.5f, py0 = (float)i0 + 0.5f;
-    // The slot loop is bound by the half-rate ALU pipe (compares, selects, min/max, bit logic), not by FMA:
-    // its bookkeeping is therefore arithmetic wherever possible.
-    //   * liveness lives in the slot's row offset: a pixel that has terminated (or lies outside the image)
-    //     gets the offset DEAD, which drives sigma out of range, so there is no per-slot `done` test;
-    //   * validity (0 <= sigma*log2e <= log2(255 o)) is ONE unsigned compare of the float's bits;
-    //   * an invalid slot is masked once (alpha = 0): T and the sums then pass through unchanged;
-    //   * "an object entry took part" is accumulated with an FMA (osum += objflag * alpha).
-    constexpr float DEAD = 1e18f;
-    float T[PPL], pr[PPL], pg[PPL], pb[PPL], pd[PPL], yoff[PPL], osum[PPL];
-    int idx[PPL];
-#pragma unroll
-    for (int s = 0; s < PPL; ++s) {
-        T[s] = 1.f; pr[s] = pg[s] = pb[s] = pd[s] = 0.f; osum[s] = 0.f;
-        idx[s] = -1;
-        const bool inside = (j < p.width) && (i0 + 2 * s < p.height);
-        yoff[s] = inside ? (float)(2 * s) : DEAD;
-    }
-
-    Staged nxt;
-    unsigned parity = 0;    // TMA: phase parity of the two mbarriers (bit b = buffer b)
-    int pending_buf = -1;   // TMA: buffer with a bulk copy in flight that nobody has waited for yet
-    if constexpr (TMA) {
-        if (lane == 0) {
-            mbar_init(&mbar[0], 1);
-            mbar_init(&mbar[1], 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            if (range.x < range.y) {
-                const uint32_t bytes = (uint32_t)min(32, range.y - range.x) * 48u;
-                mbar_expect_tx(&mbar[0], bytes);
-                bulk_g2s(sE[0], p.staged + 3 * (size_t)range.x, bytes, &mbar[0]);
-            }
-        }
-        __syncwarp();
-    } else {
-        if (range.x + lane < range.y) nxt = gather_entry(p.records, p.sorted_ids[range.x + lane]);
-    }
-    int buf = 0;
-    bool finished = false;
-    const float yc0 = (float)((tile / p.tiles_x) * SGN_TILE + strip * (2 * PPL)) + 1.0f;
-    unsigned slot_live = (1u << PPL) - 1u;  // warp-uniform: row pairs that still have an unterminated pixel (refreshed per batch)
-    constexpr bool PK = PACK && PPL >= 2;
-    constexpr int NP = PK ? PPL / 2 : 1;
-    f2 T2[NP], pr2[NP], pg2[NP], pb2[NP], pd2[NP], yoff2[NP], osum2[NP];
-#pragma unroll
-    for (int q = 0; q < NP; ++q) {
-        T2[q] = dup2(1.f); pr2[q] = pg2[q] = pb2[q] = pd2[q] = osum2[q] = dup2(0.f);
-        if (PK) yoff2[q] = f2{yoff[2 * q], yoff[2 * q + 1]};
-    }
-    const float clampf = in_register(p.clamp_fwd), nclamp = in_register(-p.clamp_fwd);
-    for (int base = range.x; base < range.y && !finished; base += 32) {
-        if constexpr (TMA) {
-            __syncwarp();  // every lane has finished reading the other buffer (previous batch)
-            pending_buf = -1;
-            if (base + 32 < range.y) {
-                if (lane == 0) {
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    const uint32_t bytes = (uint32_t)min(32, range.y - base - 32) * 48u;
-                    mbar_expect_tx(&mbar[buf ^ 1], bytes);
-                    bulk_g2s(sE[buf ^ 1], p.staged + 3 * (size_t)(base + 32), bytes, &mbar[buf ^ 1]);
-                }
-                pending_buf = buf ^ 1;
-            }
-            mbar_wait(&mbar[buf], (parity >> buf) & 1u);
-            parity ^= 1u << buf;
-        } else {
-        sA[buf][lane] = nxt.A; sB[buf][lane] = nxt.B;
-        sC[buf][lane] = make_float4(nxt.C.x, nxt.C.y, nxt.C.z, SKIP ? row_reach(nxt) + 0.5f : 0.f);
-        __syncwarp();
-        if (base + 32 + lane < range.y) nxt = gather_entry(p.records, p.sorted_ids[base + 32 + lane]);
-        }
-        if (SKIP) {
-            slot_live = 0;
-#pragma unroll
-            for (int s = 0; s < PPL; ++s) {
-                const float yo = PK ? ((s & 1) ? yoff2[s / 2].y : yoff2[s / 2].x) : yoff[s];
-                slot_live |= __any_sync(FULL, yo < 0.5f * DEAD) ? (1u << s) : 0u;
-            }
-        }
-        const int n = min(32, range.y - base);
-        // strips of long lists (PPL <= 2) are the kernel's critical path, and one entry is a ~70-cycle dependency
-        // chain: unrolled, consecutive entries (independent but for the one-FMA T chain) overlap
-#pragma unroll(PPL <= 2 ? 4 : 1)
-        for (int t = 0; t < n; ++t) {
-            if ((t & 7) == 0) {  // every pixel of the strip terminated: stop traversing (checked every 8 entries)
-                float ymin = DEAD;
-#pragma unroll
-                for (int s = 0; s < PPL; ++s) ymin = fminf(ymin, PK ? ((s & 1) ? yoff2[s / 2].y : yoff2[s / 2].x) : yoff[s]);
-                if (__all_sync(FULL, ymin >= 0.5f * DEAD)) { finished = true; break; }
-            }
-            const float4 A = TMA ? sE[buf][3 * t] : sA[buf][t];
-            const float4 B = TMA ? sE[buf][3 * t + 1] : sB[buf][t];
-            const float4 Cc = TMA ? sE[buf][3 * t + 2] : sC[buf][t];
-            const float objflag = (CLS && (__float_as_int(Cc.z) < 0)) ? 1.f : 0.f;
-            const float dyc = A.y - yc0;
-            const float dx = A.x - px;
-            const float bdx = A.w * dx, ax2 = A.z * dx * dx;
-            const float dy0 = A.y - py0;
-            // valid  <=>  0 <= sg <= log2(255 o)  <=>  bits(sg) < lim1   (sg = sigma*log2e; negative and NaN have huge bits)
-            const float span = LOG2_255 + B.y;
-            const unsigned lim1 = (unsigned)(max(__float_as_int(span), -1) + 1);  // 0 when span < 0 (negative floats are negative ints)
-            const int k = base + t;
-            if constexpr (PK) {
-                // paired row slots (f2); weights and the blended channels are kept negated (nw = -alpha*T)
-                const f2 dyb = dup2(dy0);
-#pragma unroll
-                for (int q = 0; q < NP; ++q) {
-                    if (SKIP) {
-                        if (!((slot_live >> (2 * q)) & 3u) || fabsf(dyc - (float)(4 * q + 1)) > Cc.w + 1.f) continue;
-                    }
-                    const f2 dy = f2{dy0 - yoff2[q].x, dy0 - yoff2[q].y};
-                    const f2 sg = fma2(dy, fma2(dup2(B.x), dy, dup2(bdx)), dup2(ax2));
-                    const bool v0 = __float_as_uint(sg.x) < lim1, v1 = __float_as_uint(sg.y) < lim1;
-                    const f2 nam = f2{v0 ? fmaxf(nclamp, -fast_ex2(B.y - sg.x)) : 0.f, v1 ? fmaxf(nclamp, -fast_ex2(B.y - sg.y)) : 0.f};
-                    const f2 nT = fma2(nam, T2[q], T2[q]);
-                    const bool st0 = nT.x <= T_STOP, st1 = nT.y <= T_STOP;
-                    const f2 nau = f2{st0 ? 0.f : nam.x, st1 ? 0.f : nam.y};
-                    const f2 nw = mul2(nau, T2[q]);
-                    T2[q] = fma2(nau, T2[q], T2[q]);
-                    yoff2[q].x = st0 ? DEAD : yoff2[q].x; yoff2[q].y = st1 ? DEAD : yoff2[q].y;
-                    idx[2 * q] = (nau.x < 0.f) ? k : idx[2 * q];
-                    idx[2 * q + 1] = (nau.y < 0.f) ? k : idx[2 * q + 1];
-                    pr2[q] = fma2(dup2(B.z), nw, pr2[q]); pg2[q] = fma2(dup2(B.w), nw, pg2[q]);
-                    pb2[q] = fma2(dup2(Cc.x), nw, pb2[q]); pd2[q] = fma2(dup2(Cc.y), nw, pd2[q]);
-                    if (CLS) osum2[q] = fma2(dup2(objflag), nam, osum2[q]);
-                    (void)dyb;
-                }
-            } else {
-                // straight-line, predicated: the PPL pixel chains are independent and interleave (ILP)
-#pragma unroll
-                for (int s = 0; s < PPL; ++s) {
-                    if (SKIP) {  // warp-uniform: the entry cannot reach this row pair, or all its pixels terminated
-                        if (!((slot_live >> s) & 1u) || fabsf(dyc - (float)(2 * s)) > Cc.w) continue;
-                    }
-                    const float dy = dy0 - yoff[s];
-                    const float sg = __fmaf_rn(dy, __fmaf_rn(B.x, dy, bdx), ax2);
-                    const bool valid = __float_as_uint(sg) < lim1;
-                    const float am = valid ? fminf(clampf, fast_ex2(B.y - sg)) : 0.f;
-                    const float nT = __fmaf_rn(-am, T[s], T[s]);
-                    const bool stop = nT <= T_STOP;  // only a valid entry can get here: T > T_STOP is invariant
-                    const float au = stop ? 0.f : am;
-                    const float w = au * T[s];
-                    T[s] = __fmaf_rn(-au, T[s], T[s]);
-                    yoff[s] = stop ? DEAD : yoff[s];
-                    idx[s] = (au > 0.f) ? k : idx[s];
-                    pr[s] = __fmaf_rn(B.z, w, pr[s]); pg[s] = __fmaf_rn(B.w, w, pg[s]);
-                    pb[s] = __fmaf_rn(Cc.x, w, pb[s]); pd[s] = __fmaf_rn(Cc.y, w, pd[s]);
-                    if (CLS) osum[s] = __fmaf_rn(objflag, am, osum[s]);
-                }
-            }
-        }
-        buf ^= 1;
-    }
-    if constexpr (TMA) {  // a copy issued for a batch the traversal never reached must land before the CTA may exit
-        if (pending_buf >= 0) mbar_wait(&mbar[pending_buf], (parity >> pending_buf) & 1u);
-    }
-    if constexpr (PK) {
-#pragma unroll
-        for (int q = 0; q < NP; ++q) {
-            T[2 * q] = T2[q].x; T[2 * q + 1] = T2[q].y;
-            pr[2 * q] = -pr2[q].x; pr[2 * q + 1] = -pr2[q].y; pg[2 * q] = -pg2[q].x; pg[2 * q + 1] = -pg2[q].y;
-            pb[2 * q] = -pb2[q].x; pb[2 * q + 1] = -pb2[q].y; pd[2 * q] = -pd2[q].x; pd[2 * q + 1] = -pd2[q].y;
-            osum[2 * q] = -osum2[q].x; osum[2 * q + 1] = -osum2[q].y;
-        }
-    }
-    const size_t P = (size_t)p.width * p.height;
-    {   // how deep this tile was traversed: the backward sizes its strips from it
-        int kdeep = -1;
-#pragma unroll
-        for (int s = 0; s < PPL; ++s) kdeep = max(kdeep, idx[s]);
-        kdeep = warp_max(kdeep);
-        if (lane == 0 && kdeep >= 0) atomicMax(p.tile_depth + tile, kdeep + 1 - range.x);
-    }
-#pragma unroll
-    for (int s = 0; s < PPL; ++s) {
-        const int i = i0 + 2 * s;
-        if (j >= p.width || i >= p.height) continue;
-        const size_t pid = (size_t)i * p.width + j;
-        const float alpha = 1.f - T[s];
-        p.raw[pid] = make_float4(pr[s], pg[s], pb[s], pd[s]);
-        if (p.raw_mode) {  // gsplat rasterize_gaussians: out = blended + T_final * background
-            p.rgb[3 * pid] = pr[s] + T[s] * p.bg[0]; p.rgb[3 * pid + 1] = pg[s] + T[s] * p.bg[1];
-            p.rgb[3 * pid + 2] = pb[s] + T[s] * p.bg[2];
-            p.depth[pid] = pd[s] + T[s] * p.bg[3];
-            p.acc[pid] = alpha;
-            p.final_T[SLOT_MAIN * P + pid] = T[s];
-            p.final_idx[SLOT_MAIN * P + pid] = idx[s];
-            continue;
-        }
-        // post-ops (sgn_splatfacto.py:968-975): clamp(max=1), sky blend (premultiplied rgb times alpha again), eval clamp
-        float r = fminf(pr[s], 1.f), g = fminf(pg[s], 1.f), bl = fminf(pb[s], 1.f);
-        if (p.has_sky) {
-            const float* sk = p.sky + 3 * pid;
-            r = r * alpha + sk[0] * (1.f - alpha);
-            g = g * alpha + sk[1] * (1.f - alpha);
-            bl = bl * alpha + sk[2] * (1.f - alpha);
-        }
-        if (p.eval_clamp) {
-            r = fminf(fmaxf(r, 0.f), 1.f); g = fminf(fmaxf(g, 0.f), 1.f); bl = fminf(fmaxf(bl, 0.f), 1.f);
-        }
-        p.rgb[3 * pid] = r; p.rgb[3 * pid + 1] = g; p.rgb[3 * pid + 2] = bl;
-        p.acc[pid] = alpha;
-        p.depth[pid] = alpha > 1e-3f ? pd[s] / alpha : 10.f;  // sgn_splatfacto.py:995
-        p.final_T[SLOT_MAIN * P + pid] = T[s];
-        p.final_idx[SLOT_MAIN * P + pid] = idx[s];
-        if (CLS) {
-            const bool hit = osum[s] > 0.f;
-            p.final_idx[SLOT_BG * P + pid] = hit ? BG_TODO : BG_SAME_AS_MAIN;
-            if (!hit) { p.final_T[SLOT_BG * P + pid] = T[s]; p.bg_acc[pid] = alpha; }
-        }
-    }
-}
-
-template <bool CLS, bool SKIP, bool PACK>
-__global__ void __launch_bounds__(32, BLEND_FWD_MIN_BLOCKS) blend_fwd_kernel(const BlendFwdParams p) {
-    __shared__ float4 sA[2][32];
-    __shared__ float4 sB[2][32];
-    __shared__ float4 sC[2][32];
-    int tile, strip;
-    if (!take_work(p.sched, SLOT_MAIN, p.tiles, tile, strip)) return;
-    const int2 range = p.tile_bins[tile];
-    const int W = strips_for(range.y - range.x, p.split_main);
-    if (strip >= W) return;
-    switch (W) {
-        case 1: blend_fwd_strip<8, CLS, SKIP, PACK>(p, tile, strip, range, sA, sB, sC); break;
-        case 2: blend_fwd_strip<4, CLS, SKIP, PACK>(p, tile, strip, range, sA, sB, sC); break;
-        case 4: blend_fwd_strip<2, CLS, SKIP, PACK>(p, tile, strip, range, sA, sB, sC); break;
-        default: blend_fwd_strip<1, CLS, SKIP, PACK>(p, tile, strip, range, sA, sB, sC); break;
-    }
-}
-
-template <bool CLS>
-__global__ void __launch_bounds__(32) blend_fwd_tma_kernel(const BlendFwdParams p) {
-    __shared__ __align__(128) float4 sE[2][96];
-    __shared__ __align__(8) uint64_t mbar[2];
-    int tile, strip;
-    if (!take_work(p.sched, SLOT_MAIN, p.tiles, tile, strip)) return;
-    const int2 range = p.tile_bins[tile];
-    const int W = strips_for(range.y - range.x, p.split_main);
-    if (strip >= W) return;
-    switch (W) {
-        case 1: blend_fwd_strip<8, CLS, false, true, true>(p, tile, strip, range, nullptr, nullptr, nullptr, sE, mbar); break;
-        case 2: blend_fwd_strip<4, CLS, false, true, true>(p, tile, strip, range, nullptr, nullptr, nullptr, sE, mbar); break;
-        case 4: blend_fwd_strip<2, CLS, false, true, true>(p, tile, strip, range, nullptr, nullptr, nullptr, sE, mbar); break;
-        default: blend_fwd_strip<1, CLS, false, true, true>(p, tile, strip, range, nullptr, nullptr, nullptr, sE, mbar); break;
-    }
-}
-
-// materialises the per-tile lists as staged entries (the TMA experiment's input): entry k of the sorted list -> 48 bytes
-__global__ void __launch_bounds__(256)
-stage_entries_kernel(long long M, const float4* __restrict__ records, const int32_t* __restrict__ sorted_ids, float4* __restrict__ staged) {
-    const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (k >= M) return;
-    const Staged s = gather_entry(records, sorted_ids[k]);
-    staged[3 * k] = s.A; staged[3 * k + 1] = s.B; staged[3 * k + 2] = s.C;
-}
-
-// accumulation-only pass over one class's per-tile sub-lists (objects-only / background-only render)
+// Accumulation-only traversal of the class sub-list positions [range.x, range.y) (objects-only / background-only render).
+// Carries each pixel's transmittance T and last-entry index idx (a sub-list position); yoff = 2s for a pixel whose stream is
+// still live, DEAD for one that has terminated or is not rendered.
 template <int PPL, bool SKIP>
-__device__ __forceinline__ void acc_fwd_strip(const BlendFwdParams& p, int cls, int tile, int strip, const int2 range,
-                                              float4 (*sA)[32], float4 (*sB)[32]) {
-    const int32_t* __restrict__ ids = p.cls_ids[cls];
-    const int slot = cls ? SLOT_OBJ : SLOT_BG;
-    float* __restrict__ out_acc = cls ? p.obj_acc : p.bg_acc;
+__device__ __forceinline__ void acc_fwd_traverse(const BlendFwdParams& p, const int32_t* __restrict__ ids, int tile, int strip,
+                                                 const int2 range, float (&T)[PPL], int (&idx)[PPL], float (&yoff)[PPL],
+                                                 float4 (*sA)[32], float4 (*sB)[32]) {
     const float yc0 = (float)((tile / p.tiles_x) * SGN_TILE + strip * (2 * PPL)) + 1.0f;
     const int tx = tile % p.tiles_x, ty = tile / p.tiles_x;
     const int lane = threadIdx.x;
     const int j = tx * SGN_TILE + (lane & 15);
     const int i0 = ty * SGN_TILE + strip * (2 * PPL) + (lane >> 4);
     const float px = (float)j + 0.5f, py0 = (float)i0 + 0.5f;
-    constexpr unsigned ALL = (1u << PPL) - 1u;
     constexpr float DEAD = 1e18f;  // row offset of a terminated / skipped pixel (see blend_fwd_strip)
-    float T[PPL], yoff[PPL];
-    int idx[PPL];
-    unsigned skip = 0;
-    const size_t P = (size_t)p.width * p.height;
-#pragma unroll
-    for (int s = 0; s < PPL; ++s) {
-        T[s] = 1.f; idx[s] = -1; yoff[s] = (float)(2 * s);
-        const int i = i0 + 2 * s;
-        if (!((j < p.width) && (i < p.height))) { yoff[s] = DEAD; skip |= 1u << s; }
-        else if (cls == 0 && p.final_idx[SLOT_BG * P + (size_t)i * p.width + j] != BG_TODO) {
-            yoff[s] = DEAD; skip |= 1u << s;  // the main forward already wrote this pixel's background result
-        }
-    }
-    if (__all_sync(FULL, skip == ALL)) return;
     const float clampf = in_register(p.clamp_fwd), nclampf = in_register(-p.clamp_fwd);
     Staged nxt;
     if (range.x + lane < range.y) nxt = gather_entry(p.records, ids[range.x + lane]);
@@ -688,6 +415,322 @@ __device__ __forceinline__ void acc_fwd_strip(const BlendFwdParams& p, int cls, 
         }
         buf ^= 1;
     }
+}
+
+// The main pass.  CLS: the per-tile list carries object entries (payload bit 31), and the strip also renders the
+// objects-only accumulation: a second transmittance To per pixel, advanced with the SAME alpha by the object entries
+// only (a warp-uniform branch), with its last-entry index recorded as a position in the object sub-list -- the object
+// entries of the list in list order.  When every pixel's main stream has terminated, the objects-only streams that are
+// still live continue on the object sub-list from the first object entry not yet passed (acc_fwd_traverse).
+template <int PPL, bool CLS, bool SKIP, bool PACK, bool TMA = false>
+__device__ __forceinline__ void blend_fwd_strip(const BlendFwdParams& p, int tile, int strip, const int2 range,
+                                                float4 (*sA)[32], float4 (*sB)[32], float4 (*sC)[32],
+                                                float4 (*sE)[96] = nullptr, uint64_t* mbar = nullptr) {
+    const int tx = tile % p.tiles_x, ty = tile / p.tiles_x;
+    const int lane = threadIdx.x;
+    const int j = tx * SGN_TILE + (lane & 15);
+    const int i0 = ty * SGN_TILE + strip * (2 * PPL) + (lane >> 4);
+    const float px = (float)j + 0.5f, py0 = (float)i0 + 0.5f;
+    // The slot loop is bound by the half-rate ALU pipe (compares, selects, min/max, bit logic), not by FMA:
+    // its bookkeeping is therefore arithmetic wherever possible.
+    //   * liveness lives in the sign of the stream's transmittance: a stream that has terminated (or a pixel outside
+    //     the image) holds -|T|, for which the next T is never above T_STOP, so nothing more is blended into it and
+    //     there is no per-slot `done` test.  The alpha itself stays live for the other stream of the pixel;
+    //   * validity (0 <= sigma*log2e <= log2(255 o)) is ONE unsigned compare of the float's bits;
+    //   * an invalid slot is masked once (alpha = 0): T and the sums then pass through unchanged.
+    float T[PPL], pr[PPL], pg[PPL], pb[PPL], pd[PPL], osum[PPL], To[PPL];
+    int idx[PPL], idxo[PPL];
+#pragma unroll
+    for (int s = 0; s < PPL; ++s) {
+        pr[s] = pg[s] = pb[s] = pd[s] = 0.f; osum[s] = 0.f;
+        idx[s] = idxo[s] = -1;
+        const bool inside = (j < p.width) && (i0 + 2 * s < p.height);
+        T[s] = To[s] = inside ? 1.f : -1.f;
+    }
+    // object sub-list position of the next object entry of the list (warp-uniform)
+    int orank = CLS ? p.cls_bins[1][tile].x : 0;
+
+    Staged nxt;
+    unsigned parity = 0;    // TMA: phase parity of the two mbarriers (bit b = buffer b)
+    int pending_buf = -1;   // TMA: buffer with a bulk copy in flight that nobody has waited for yet
+    if constexpr (TMA) {
+        if (lane == 0) {
+            mbar_init(&mbar[0], 1);
+            mbar_init(&mbar[1], 1);
+            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            if (range.x < range.y) {
+                const uint32_t bytes = (uint32_t)min(32, range.y - range.x) * 48u;
+                mbar_expect_tx(&mbar[0], bytes);
+                bulk_g2s(sE[0], p.staged + 3 * (size_t)range.x, bytes, &mbar[0]);
+            }
+        }
+        __syncwarp();
+    } else {
+        if (range.x + lane < range.y) nxt = gather_entry(p.records, p.sorted_ids[range.x + lane]);
+    }
+    int buf = 0;
+    bool finished = false;
+    const float yc0 = (float)((tile / p.tiles_x) * SGN_TILE + strip * (2 * PPL)) + 1.0f;
+    unsigned slot_live = (1u << PPL) - 1u;  // warp-uniform: row pairs that still have a live stream (refreshed per batch)
+    constexpr bool PK = PACK && PPL >= 2;
+    constexpr int NP = PK ? PPL / 2 : 1;
+    f2 T2[NP], pr2[NP], pg2[NP], pb2[NP], pd2[NP], osum2[NP], To2[NP];
+#pragma unroll
+    for (int q = 0; q < NP; ++q) {
+        pr2[q] = pg2[q] = pb2[q] = pd2[q] = osum2[q] = dup2(0.f);
+        if (PK) { T2[q] = f2{T[2 * q], T[2 * q + 1]}; To2[q] = f2{To[2 * q], To[2 * q + 1]}; }
+    }
+    const float clampf = in_register(p.clamp_fwd), nclamp = in_register(-p.clamp_fwd);
+    for (int base = range.x; base < range.y && !finished; base += 32) {
+        if constexpr (TMA) {
+            __syncwarp();  // every lane has finished reading the other buffer (previous batch)
+            pending_buf = -1;
+            if (base + 32 < range.y) {
+                if (lane == 0) {
+                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                    const uint32_t bytes = (uint32_t)min(32, range.y - base - 32) * 48u;
+                    mbar_expect_tx(&mbar[buf ^ 1], bytes);
+                    bulk_g2s(sE[buf ^ 1], p.staged + 3 * (size_t)(base + 32), bytes, &mbar[buf ^ 1]);
+                }
+                pending_buf = buf ^ 1;
+            }
+            mbar_wait(&mbar[buf], (parity >> buf) & 1u);
+            parity ^= 1u << buf;
+        } else {
+        sA[buf][lane] = nxt.A; sB[buf][lane] = nxt.B;
+        sC[buf][lane] = make_float4(nxt.C.x, nxt.C.y, nxt.C.z, SKIP ? row_reach(nxt) + 0.5f : 0.f);
+        __syncwarp();
+        if (base + 32 + lane < range.y) nxt = gather_entry(p.records, p.sorted_ids[base + 32 + lane]);
+        }
+        if (SKIP) {
+            slot_live = 0;
+#pragma unroll
+            for (int s = 0; s < PPL; ++s) {
+                const float Ts = PK ? ((s & 1) ? T2[s / 2].y : T2[s / 2].x) : T[s];
+                const float Tos = PK ? ((s & 1) ? To2[s / 2].y : To2[s / 2].x) : To[s];
+                slot_live |= __any_sync(FULL, (CLS ? fmaxf(Ts, Tos) : Ts) > 0.f) ? (1u << s) : 0u;
+            }
+        }
+        const int n = min(32, range.y - base);
+        // strips of long lists (PPL <= 2) are the kernel's critical path, and one entry is a ~70-cycle dependency
+        // chain: unrolled, consecutive entries (independent but for the one-FMA T chain) overlap
+#pragma unroll(PPL <= 2 ? 4 : 1)
+        for (int t = 0; t < n; ++t) {
+            if ((t & 7) == 0) {  // every pixel's main stream terminated: stop traversing (checked every 8 entries)
+                float tmax = -1.f;
+#pragma unroll
+                for (int s = 0; s < PPL; ++s) tmax = fmaxf(tmax, PK ? ((s & 1) ? T2[s / 2].y : T2[s / 2].x) : T[s]);
+                if (__all_sync(FULL, tmax < 0.f)) { finished = true; break; }
+            }
+            const float4 A = TMA ? sE[buf][3 * t] : sA[buf][t];
+            const float4 B = TMA ? sE[buf][3 * t + 1] : sB[buf][t];
+            const float4 Cc = TMA ? sE[buf][3 * t + 2] : sC[buf][t];
+            const float dyc = A.y - yc0;
+            const float dx = A.x - px;
+            const float bdx = A.w * dx, ax2 = A.z * dx * dx;
+            const float dy0 = A.y - py0;
+            // valid  <=>  0 <= sg <= log2(255 o)  <=>  bits(sg) < lim1   (sg = sigma*log2e; negative and NaN have huge bits)
+            const float span = LOG2_255 + B.y;
+            const unsigned lim1 = (unsigned)(max(__float_as_int(span), -1) + 1);  // 0 when span < 0 (negative floats are negative ints)
+            const int k = base + t;
+            // OBJ (warp-uniform): an object entry, which the objects-only stream takes as well
+            auto blend_entry = [&](auto obj_tag) {
+                constexpr bool OBJ = decltype(obj_tag)::value;
+                if constexpr (PK) {
+                    // paired row slots (f2); weights and the blended channels are kept negated (nw = -alpha*T)
+#pragma unroll
+                    for (int q = 0; q < NP; ++q) {
+                        if (SKIP) {
+                            if (!((slot_live >> (2 * q)) & 3u) || fabsf(dyc - (float)(4 * q + 1)) > Cc.w + 1.f) continue;
+                        }
+                        const f2 dy = f2{dy0 - (float)(4 * q), dy0 - (float)(4 * q + 2)};
+                        const f2 sg = fma2(dy, fma2(dup2(B.x), dy, dup2(bdx)), dup2(ax2));
+                        const bool v0 = __float_as_uint(sg.x) < lim1, v1 = __float_as_uint(sg.y) < lim1;
+                        const f2 nam = f2{v0 ? fmaxf(nclamp, -fast_ex2(B.y - sg.x)) : 0.f, v1 ? fmaxf(nclamp, -fast_ex2(B.y - sg.y)) : 0.f};
+                        const f2 nT = fma2(nam, T2[q], T2[q]);
+                        const bool st0 = nT.x <= T_STOP, st1 = nT.y <= T_STOP;
+                        const f2 nau = f2{st0 ? 0.f : nam.x, st1 ? 0.f : nam.y};
+                        const f2 nw = mul2(nau, T2[q]);
+                        if (OBJ) {  // an object entry took part in the main stream (the background pass needs this pixel)
+                            osum2[q].x = T2[q].x > 0.f ? osum2[q].x + nam.x : osum2[q].x;
+                            osum2[q].y = T2[q].y > 0.f ? osum2[q].y + nam.y : osum2[q].y;
+                        }
+                        T2[q].x = st0 ? -fabsf(T2[q].x) : nT.x; T2[q].y = st1 ? -fabsf(T2[q].y) : nT.y;
+                        idx[2 * q] = (nau.x < 0.f) ? k : idx[2 * q];
+                        idx[2 * q + 1] = (nau.y < 0.f) ? k : idx[2 * q + 1];
+                        pr2[q] = fma2(dup2(B.z), nw, pr2[q]); pg2[q] = fma2(dup2(B.w), nw, pg2[q]);
+                        pb2[q] = fma2(dup2(Cc.x), nw, pb2[q]); pd2[q] = fma2(dup2(Cc.y), nw, pd2[q]);
+                        if (OBJ) {
+                            const f2 nTo = fma2(nam, To2[q], To2[q]);
+                            const bool so0 = nTo.x <= T_STOP, so1 = nTo.y <= T_STOP;
+                            idxo[2 * q] = (v0 && !so0) ? orank : idxo[2 * q];
+                            idxo[2 * q + 1] = (v1 && !so1) ? orank : idxo[2 * q + 1];
+                            To2[q].x = so0 ? -fabsf(To2[q].x) : nTo.x; To2[q].y = so1 ? -fabsf(To2[q].y) : nTo.y;
+                        }
+                    }
+                } else {
+                    // straight-line, predicated: the PPL pixel chains are independent and interleave (ILP)
+#pragma unroll
+                    for (int s = 0; s < PPL; ++s) {
+                        if (SKIP) {  // warp-uniform: the entry cannot reach this row pair, or all its pixels terminated
+                            if (!((slot_live >> s) & 1u) || fabsf(dyc - (float)(2 * s)) > Cc.w) continue;
+                        }
+                        const float dy = dy0 - (float)(2 * s);
+                        const float sg = __fmaf_rn(dy, __fmaf_rn(B.x, dy, bdx), ax2);
+                        const bool valid = __float_as_uint(sg) < lim1;
+                        const float am = valid ? fminf(clampf, fast_ex2(B.y - sg)) : 0.f;
+                        const float nT = __fmaf_rn(-am, T[s], T[s]);
+                        const bool stop = nT <= T_STOP;
+                        const float au = stop ? 0.f : am;
+                        const float w = au * T[s];
+                        if (OBJ) osum[s] = T[s] > 0.f ? osum[s] + am : osum[s];
+                        T[s] = stop ? -fabsf(T[s]) : nT;
+                        idx[s] = (au > 0.f) ? k : idx[s];
+                        pr[s] = __fmaf_rn(B.z, w, pr[s]); pg[s] = __fmaf_rn(B.w, w, pg[s]);
+                        pb[s] = __fmaf_rn(Cc.x, w, pb[s]); pd[s] = __fmaf_rn(Cc.y, w, pd[s]);
+                        if (OBJ) {
+                            const float nTo = __fmaf_rn(-am, To[s], To[s]);
+                            const bool so = nTo <= T_STOP;
+                            idxo[s] = (valid && !so) ? orank : idxo[s];
+                            To[s] = so ? -fabsf(To[s]) : nTo;
+                        }
+                    }
+                }
+                if (OBJ) ++orank;
+            };
+            if (CLS && __float_as_int(Cc.z) < 0) blend_entry(std::true_type{});
+            else blend_entry(std::false_type{});
+        }
+        buf ^= 1;
+    }
+    if constexpr (TMA) {  // a copy issued for a batch the traversal never reached must land before the CTA may exit
+        if (pending_buf >= 0) mbar_wait(&mbar[pending_buf], (parity >> pending_buf) & 1u);
+    }
+    if constexpr (PK) {
+#pragma unroll
+        for (int q = 0; q < NP; ++q) {
+            T[2 * q] = T2[q].x; T[2 * q + 1] = T2[q].y;
+            To[2 * q] = To2[q].x; To[2 * q + 1] = To2[q].y;
+            pr[2 * q] = -pr2[q].x; pr[2 * q + 1] = -pr2[q].y; pg[2 * q] = -pg2[q].x; pg[2 * q + 1] = -pg2[q].y;
+            pb[2 * q] = -pb2[q].x; pb[2 * q + 1] = -pb2[q].y; pd[2 * q] = -pd2[q].x; pd[2 * q + 1] = -pd2[q].y;
+            osum[2 * q] = -osum2[q].x; osum[2 * q + 1] = -osum2[q].y;
+        }
+    }
+    const size_t P = (size_t)p.width * p.height;
+    {   // how deep this tile was traversed: the backward sizes its strips from it
+        int kdeep = -1;
+#pragma unroll
+        for (int s = 0; s < PPL; ++s) kdeep = max(kdeep, idx[s]);
+        kdeep = warp_max(kdeep);
+        if (lane == 0 && kdeep >= 0) atomicMax(p.tile_depth + tile, kdeep + 1 - range.x);
+    }
+#pragma unroll
+    for (int s = 0; s < PPL; ++s) {
+        const int i = i0 + 2 * s;
+        if (j >= p.width || i >= p.height) continue;
+        T[s] = fabsf(T[s]);
+        const size_t pid = (size_t)i * p.width + j;
+        const float alpha = 1.f - T[s];
+        p.raw[pid] = make_float4(pr[s], pg[s], pb[s], pd[s]);
+        if (p.raw_mode) {  // gsplat rasterize_gaussians: out = blended + T_final * background
+            p.rgb[3 * pid] = pr[s] + T[s] * p.bg[0]; p.rgb[3 * pid + 1] = pg[s] + T[s] * p.bg[1];
+            p.rgb[3 * pid + 2] = pb[s] + T[s] * p.bg[2];
+            p.depth[pid] = pd[s] + T[s] * p.bg[3];
+            p.acc[pid] = alpha;
+            p.final_T[SLOT_MAIN * P + pid] = T[s];
+            p.final_idx[SLOT_MAIN * P + pid] = idx[s];
+            continue;
+        }
+        // post-ops (sgn_splatfacto.py:968-975): clamp(max=1), sky blend (premultiplied rgb times alpha again), eval clamp
+        float r = fminf(pr[s], 1.f), g = fminf(pg[s], 1.f), bl = fminf(pb[s], 1.f);
+        if (p.has_sky) {
+            const float* sk = p.sky + 3 * pid;
+            r = r * alpha + sk[0] * (1.f - alpha);
+            g = g * alpha + sk[1] * (1.f - alpha);
+            bl = bl * alpha + sk[2] * (1.f - alpha);
+        }
+        if (p.eval_clamp) {
+            r = fminf(fmaxf(r, 0.f), 1.f); g = fminf(fmaxf(g, 0.f), 1.f); bl = fminf(fmaxf(bl, 0.f), 1.f);
+        }
+        p.rgb[3 * pid] = r; p.rgb[3 * pid + 1] = g; p.rgb[3 * pid + 2] = bl;
+        p.acc[pid] = alpha;
+        p.depth[pid] = alpha > 1e-3f ? pd[s] / alpha : 10.f;  // sgn_splatfacto.py:995
+        p.final_T[SLOT_MAIN * P + pid] = T[s];
+        p.final_idx[SLOT_MAIN * P + pid] = idx[s];
+        if (CLS) {
+            const bool hit = osum[s] > 0.f;
+            p.final_idx[SLOT_BG * P + pid] = hit ? BG_TODO : BG_SAME_AS_MAIN;
+            if (!hit) { p.final_T[SLOT_BG * P + pid] = T[s]; p.bg_acc[pid] = alpha; }
+        }
+    }
+    if constexpr (CLS) {
+        // objects-only streams still live: the rest of the object sub-list, from the first object entry not yet passed
+        constexpr float DEAD = 1e18f;
+        float yo[PPL];
+        bool live = false;
+#pragma unroll
+        for (int s = 0; s < PPL; ++s) {
+            live = live || To[s] > 0.f;
+            yo[s] = To[s] > 0.f ? (float)(2 * s) : DEAD;
+            To[s] = fabsf(To[s]);
+        }
+        const int2 orange = p.cls_bins[1][tile];
+        if (__any_sync(FULL, live) && orank < orange.y) {
+            if constexpr (TMA) {  // the bulk-copy ring is idle now (every copy has landed): stage through it
+                acc_fwd_traverse<PPL, true>(p, p.cls_ids[1], tile, strip, make_int2(orank, orange.y), To, idxo, yo,
+                                            reinterpret_cast<float4(*)[32]>(&sE[0][0]), reinterpret_cast<float4(*)[32]>(&sE[0][64]));
+            } else {
+                acc_fwd_traverse<PPL, true>(p, p.cls_ids[1], tile, strip, make_int2(orank, orange.y), To, idxo, yo, sA, sB);
+            }
+            // tile_depth[object]: how far this tile's object streams ran past the main traversal (sizes the backward)
+            int kdeep = -1;
+#pragma unroll
+            for (int s = 0; s < PPL; ++s) kdeep = max(kdeep, idxo[s]);
+            kdeep = warp_max(kdeep);
+            if (lane == 0 && kdeep >= orank) atomicMax(p.tile_depth + (size_t)SLOT_OBJ * p.tiles + tile, kdeep + 1 - orank);
+        }
+#pragma unroll
+        for (int s = 0; s < PPL; ++s) {
+            const int i = i0 + 2 * s;
+            if (j >= p.width || i >= p.height) continue;
+            const size_t pid = (size_t)i * p.width + j;
+            p.final_T[SLOT_OBJ * P + pid] = To[s];
+            p.final_idx[SLOT_OBJ * P + pid] = idxo[s];
+            p.obj_acc[pid] = 1.f - To[s];
+        }
+    }
+}
+
+// accumulation-only pass over one class's per-tile sub-lists (the background-only render; the objects-only one is part of
+// the main pass)
+template <int PPL, bool SKIP>
+__device__ __forceinline__ void acc_fwd_strip(const BlendFwdParams& p, int cls, int tile, int strip, const int2 range,
+                                              float4 (*sA)[32], float4 (*sB)[32]) {
+    const int32_t* __restrict__ ids = p.cls_ids[cls];
+    const int slot = cls ? SLOT_OBJ : SLOT_BG;
+    float* __restrict__ out_acc = cls ? p.obj_acc : p.bg_acc;
+    const int tx = tile % p.tiles_x, ty = tile / p.tiles_x;
+    const int lane = threadIdx.x;
+    const int j = tx * SGN_TILE + (lane & 15);
+    const int i0 = ty * SGN_TILE + strip * (2 * PPL) + (lane >> 4);
+    constexpr unsigned ALL = (1u << PPL) - 1u;
+    constexpr float DEAD = 1e18f;  // row offset of a terminated / skipped pixel
+    float T[PPL], yoff[PPL];
+    int idx[PPL];
+    unsigned skip = 0;
+    const size_t P = (size_t)p.width * p.height;
+#pragma unroll
+    for (int s = 0; s < PPL; ++s) {
+        T[s] = 1.f; idx[s] = -1; yoff[s] = (float)(2 * s);
+        const int i = i0 + 2 * s;
+        if (!((j < p.width) && (i < p.height))) { yoff[s] = DEAD; skip |= 1u << s; }
+        else if (cls == 0 && p.final_idx[SLOT_BG * P + (size_t)i * p.width + j] != BG_TODO) {
+            yoff[s] = DEAD; skip |= 1u << s;  // the main forward already wrote this pixel's background result
+        }
+    }
+    if (__all_sync(FULL, skip == ALL)) return;
+    acc_fwd_traverse<PPL, SKIP>(p, ids, tile, strip, range, T, idx, yoff, sA, sB);
     {
         int kdeep = -1;
 #pragma unroll
@@ -704,6 +747,50 @@ __device__ __forceinline__ void acc_fwd_strip(const BlendFwdParams& p, int cls, 
         p.final_idx[slot * P + pid] = idx[s];
         out_acc[pid] = 1.f - T[s];
     }
+}
+
+template <bool CLS, bool SKIP, bool PACK>
+__global__ void __launch_bounds__(32, BLEND_FWD_MIN_BLOCKS) blend_fwd_kernel(const BlendFwdParams p) {
+    __shared__ float4 sA[2][32];
+    __shared__ float4 sB[2][32];
+    __shared__ float4 sC[2][32];
+    int tile, strip;
+    if (!take_work(p.sched, SLOT_MAIN, p.tiles, tile, strip)) return;
+    const int2 range = p.tile_bins[tile];
+    const int W = strips_for(range.y - range.x, p.split_main);
+    if (strip >= W) return;
+    switch (W) {
+        case 1: blend_fwd_strip<8, CLS, SKIP, PACK>(p, tile, strip, range, sA, sB, sC); break;
+        case 2: blend_fwd_strip<4, CLS, SKIP, PACK>(p, tile, strip, range, sA, sB, sC); break;
+        case 4: blend_fwd_strip<2, CLS, SKIP, PACK>(p, tile, strip, range, sA, sB, sC); break;
+        default: blend_fwd_strip<1, CLS, SKIP, PACK>(p, tile, strip, range, sA, sB, sC); break;
+    }
+}
+
+template <bool CLS>
+__global__ void __launch_bounds__(32) blend_fwd_tma_kernel(const BlendFwdParams p) {
+    __shared__ __align__(128) float4 sE[2][96];
+    __shared__ __align__(8) uint64_t mbar[2];
+    int tile, strip;
+    if (!take_work(p.sched, SLOT_MAIN, p.tiles, tile, strip)) return;
+    const int2 range = p.tile_bins[tile];
+    const int W = strips_for(range.y - range.x, p.split_main);
+    if (strip >= W) return;
+    switch (W) {
+        case 1: blend_fwd_strip<8, CLS, false, true, true>(p, tile, strip, range, nullptr, nullptr, nullptr, sE, mbar); break;
+        case 2: blend_fwd_strip<4, CLS, false, true, true>(p, tile, strip, range, nullptr, nullptr, nullptr, sE, mbar); break;
+        case 4: blend_fwd_strip<2, CLS, false, true, true>(p, tile, strip, range, nullptr, nullptr, nullptr, sE, mbar); break;
+        default: blend_fwd_strip<1, CLS, false, true, true>(p, tile, strip, range, nullptr, nullptr, nullptr, sE, mbar); break;
+    }
+}
+
+// materialises the per-tile lists as staged entries (the TMA experiment's input): entry k of the sorted list -> 48 bytes
+__global__ void __launch_bounds__(256)
+stage_entries_kernel(long long M, const float4* __restrict__ records, const int32_t* __restrict__ sorted_ids, float4* __restrict__ staged) {
+    const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= M) return;
+    const Staged s = gather_entry(records, sorted_ids[k]);
+    staged[3 * k] = s.A; staged[3 * k + 1] = s.B; staged[3 * k + 2] = s.C;
 }
 
 template <bool SKIP>
@@ -723,9 +810,9 @@ __global__ void __launch_bounds__(32, BLEND_ACC_MIN_BLOCKS) acc_fwd_kernel(const
     }
 }
 
-// The object accumulation pass is independent of the main pass (and the background pass only needs the
-// main pass's flags), and every blend kernel ends in a tail during which most SMs idle.  The object pass
-// is therefore forked onto an auxiliary stream and joined back with events: same results, the tails overlap.
+// The background-only backward is independent of the main backward (both only RED into v_records), and every
+// blend kernel ends in a tail during which most SMs idle.  It is therefore forked onto an auxiliary stream and
+// joined back with events: same results, the tails overlap.
 #include <mutex>
 static cudaStream_t aux_stream() {
     static std::mutex mu;
@@ -808,7 +895,7 @@ extern "C" int sgn_blend_fwd(const sgn_camera* cam, const sgn_blend_opts* opts, 
     p.tiles_x = (cam->width + SGN_TILE - 1) / SGN_TILE;
     const int tiles_y = (cam->height + SGN_TILE - 1) / SGN_TILE;
     p.clamp_fwd = opts->alpha_clamp_fwd;
-    p.split_main = opts->split_fwd_main > 0 ? opts->split_fwd_main : 1024;
+    p.split_main = opts->split_fwd_main > 0 ? opts->split_fwd_main : 768;
     p.split_acc = opts->split_fwd_acc > 0 ? opts->split_fwd_acc : 512;
     p.has_sky = opts->has_sky; p.eval_clamp = opts->eval_clamp; p.raw_mode = opts->raw_mode;
     for (int c = 0; c < 4; ++c) p.bg[c] = opts->background[c];
@@ -837,23 +924,18 @@ extern "C" int sgn_blend_fwd(const sgn_camera* cam, const sgn_blend_opts* opts, 
     SGN_CHECK_CUDA(cudaMemsetAsync(out->tile_depth, 0, sizeof(int32_t) * 3 * (size_t)tiles, (cudaStream_t)stream));
     p.sched = out->sched;
     if (out->sched) {
-        sched_kernel<<<opts->class_streams ? 3 : 1, 1024, 0, (cudaStream_t)stream>>>(tiles, p.tile_bins, p.cls_bins[0], p.cls_bins[1], nullptr,
+        sched_kernel<<<opts->class_streams ? 2 : 1, 1024, 0, (cudaStream_t)stream>>>(tiles, p.tile_bins, p.cls_bins[0], nullptr, 0,
                                                                                   p.split_main, p.split_acc, out->sched);
         SGN_CHECK_LAUNCH("sched_kernel");
     }
     if (opts->class_streams) {
-        ForkJoin fj((cudaStream_t)stream);
         const bool acc_skip = !(opts->tuning & SGN_TUNE_ACC_NO_ROW_SKIP);
         const unsigned acc_grid = tiles * 8;
-        if (acc_skip) acc_fwd_kernel<true><<<acc_grid, 32, 0, fj.side()>>>(p, 1);  // objects: independent of the main pass
-        else acc_fwd_kernel<false><<<acc_grid, 32, 0, fj.side()>>>(p, 1);
-        SGN_CHECK_LAUNCH("acc_fwd_kernel<object>");
-        launch_blend_fwd<true>(p, opts->tuning, (cudaStream_t)stream);
+        launch_blend_fwd<true>(p, opts->tuning, (cudaStream_t)stream);  // main + objects-only
         SGN_CHECK_LAUNCH("blend_fwd_kernel");
         if (acc_skip) acc_fwd_kernel<true><<<acc_grid, 32, 0, (cudaStream_t)stream>>>(p, 0);  // background: needs the main pass's flags
         else acc_fwd_kernel<false><<<acc_grid, 32, 0, (cudaStream_t)stream>>>(p, 0);
         SGN_CHECK_LAUNCH("acc_fwd_kernel<background>");
-        fj.finish();
     } else {
         launch_blend_fwd<false>(p, opts->tuning, (cudaStream_t)stream);
         SGN_CHECK_LAUNCH("blend_fwd_kernel");
@@ -900,267 +982,25 @@ __device__ __forceinline__ void accumulate_grad(const BlendBwdParams& p, float f
     else atomicAdd(p.v_records + idx, v);
 }
 
-// DEPTHG: the depth output has a cotangent.
-// (Measured and dropped: software-pipelining the reduction of entry t-1 under the arithmetic of entry t -- it
-// has to run unconditionally, which costs more than the overlap gains: 0.87 vs 0.82 ms on cfg3.)
-template <int PPL, bool DEPTHG, bool PACK>
-__device__ __forceinline__ void blend_bwd_strip(const BlendBwdParams& p, int tile, int strip, const int2 range,
-                                                float4 (*sA)[32], float4 (*sB)[32], float4 (*sC)[32]) {
-    const int tx = tile % p.tiles_x, ty = tile / p.tiles_x;
-    const int lane = threadIdx.x;
-    const int j = tx * SGN_TILE + (lane & 15);
-    const int i0 = ty * SGN_TILE + strip * (2 * PPL) + (lane >> 4);
-    const float px = (float)j + 0.5f, py0 = (float)i0 + 0.5f;
-    const size_t P = (size_t)p.width * p.height;
-
-    // ---- per-pixel prologue: cotangents of the RAW blend outputs from those of the final outputs
-    float T[PPL], tfv[PPL];
-    float vr[PPL], vg[PPL], vb[PPL], vd[PPL];
-    float bv[PPL];  // running  sum_{later k} (c_k . v_out) * alpha_k * T_k  (gsplat's `buffer` dotted with v_out)
-    int idx[PPL];
-    int kmax = -1;
-#pragma unroll
-    for (int s = 0; s < PPL; ++s) {
-        T[s] = 1.f; tfv[s] = 0.f; vr[s] = vg[s] = vb[s] = vd[s] = 0.f;
-        bv[s] = 0.f;
-        idx[s] = -1;
-        const int i = i0 + 2 * s;
-        if (j >= p.width || i >= p.height) continue;
-        const size_t pid = (size_t)i * p.width + j;
-        const float Tf = p.final_T[SLOT_MAIN * P + pid];
-        idx[s] = p.final_idx[SLOT_MAIN * P + pid];
-        T[s] = Tf;
-        const float alpha = 1.f - Tf;
-        const float4 raw = p.raw[pid];
-        float voa = p.v_acc ? p.v_acc[pid] : 0.f;
-        if (p.v_bg && p.final_idx[SLOT_BG * P + pid] == BG_SAME_AS_MAIN) voa += p.v_bg[pid];  // background_acc == accumulation here
-        if (p.raw_mode) {  // out_c = blended_c + (1 - alpha) * bg_c
-            if (p.v_rgb) {
-                vr[s] = p.v_rgb[3 * pid]; vg[s] = p.v_rgb[3 * pid + 1]; vb[s] = p.v_rgb[3 * pid + 2];
-                voa -= p.bg[0] * vr[s] + p.bg[1] * vg[s] + p.bg[2] * vb[s];
-            }
-            if (DEPTHG) { vd[s] = p.v_depth[pid]; voa -= p.bg[3] * vd[s]; }
-        } else if (p.v_rgb) {
-            float v[3] = {p.v_rgb[3 * pid], p.v_rgb[3 * pid + 1], p.v_rgb[3 * pid + 2]};
-            const float rr[3] = {raw.x, raw.y, raw.z};
-            float vraw[3];
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                const float cl = fminf(rr[c], 1.f);
-                float fin = cl;
-                float sk = 0.f;
-                if (p.has_sky) { sk = p.sky[3 * pid + c]; fin = cl * alpha + sk * (1.f - alpha); }
-                if (p.eval_clamp && (fin < 0.f || fin > 1.f)) v[c] = 0.f;
-                if (p.has_sky) {
-                    voa += v[c] * (cl - sk);
-                    if (p.v_sky) p.v_sky[3 * pid + c] = v[c] * (1.f - alpha);
-                    vraw[c] = (rr[c] <= 1.f) ? v[c] * alpha : 0.f;
-                } else {
-                    vraw[c] = (rr[c] <= 1.f) ? v[c] : 0.f;
-                }
-            }
-            vr[s] = vraw[0]; vg[s] = vraw[1]; vb[s] = vraw[2];
-        }
-        if (DEPTHG && !p.raw_mode) {
-            if (alpha > 1e-3f) {
-                const float vdep = p.v_depth[pid];
-                vd[s] = vdep / alpha;
-                voa += -vdep * raw.w / (alpha * alpha);
-            }
-        }
-        tfv[s] = Tf * voa;
-        kmax = max(kmax, idx[s]);
-    }
-    if (range.y <= range.x) return;  // empty tile (after the prologue: v_sky is written for every pixel)
-    const int wkmax = warp_max(kmax);
-    const int hi0 = min(range.y, wkmax + 1);  // entries at positions >= hi0 matter to no pixel of this tile
-    if (hi0 <= range.x) return;
-
-    Staged nxt;
-    if (hi0 - 1 - lane >= range.x) nxt = gather_entry(p.records, p.sorted_ids[hi0 - 1 - lane]);
-    int buf = 0;
-    constexpr int NV = DEPTHG ? 10 : 9;
-    const int my_comp = multi_reduce_slot<NV>(lane);
-    const float clampb = in_register(p.clamp_bwd), nclamp = -clampb;
-    const float fscale = p.v_fixed ? __ldg(p.fixed_scale) : 0.f;
-    constexpr bool PK = PACK && PPL >= 2;
-    constexpr int NP = PK ? PPL / 2 : 1;
-    f2 T2[NP], d2[NP], vr2[NP], vg2[NP], vb2[NP], vd2[NP];
-    if constexpr (PK) {
-#pragma unroll
-        for (int q = 0; q < NP; ++q) {
-            T2[q] = f2{T[2 * q], T[2 * q + 1]}; d2[q] = f2{tfv[2 * q], tfv[2 * q + 1]};
-            vr2[q] = f2{vr[2 * q], vr[2 * q + 1]}; vg2[q] = f2{vg[2 * q], vg[2 * q + 1]};
-            vb2[q] = f2{vb[2 * q], vb[2 * q + 1]}; vd2[q] = f2{vd[2 * q], vd[2 * q + 1]};
-        }
-    }
-    for (int hi = hi0; hi > range.x; hi -= 32) {
-        sA[buf][lane] = nxt.A; sB[buf][lane] = nxt.B; sC[buf][lane] = nxt.C;
-        __syncwarp();
-        if (hi - 33 - lane >= range.x) nxt = gather_entry(p.records, p.sorted_ids[hi - 33 - lane]);
-        const int n = min(32, hi - range.x);
-        for (int t = 0; t < n; ++t) {
-            const int k = hi - 1 - t;
-            const float4 A = sA[buf][t];
-            const float4 B = sB[buf][t];
-            const float4 Cc = sC[buf][t];
-            const float dx = A.x - px;
-            const float bdx = A.w * dx, ax2 = A.z * dx * dx;
-            const float dy0 = A.y - py0;
-            // valid  <=>  0 <= sg <= log2(255 o)  <=>  bits(sg) < lim1  (see blend_fwd_strip), and k <= idx
-            const unsigned lim1 = (unsigned)(max(__float_as_int(LOG2_255 + B.y), -1) + 1);
-            const float o = Cc.w;
-            float S0 = 0.f, Sy = 0.f, Syy = 0.f, cr = 0.f, cg = 0.f, cb = 0.f, cd = 0.f;
-            float activity = 0.f;  // sum of alpha*T over the valid slots: non-zero iff some pixel of this lane took the entry
-            if constexpr (PK) {
-                // packed row-slot pairs.  An invalid slot is masked ONCE, at the exponential (raw = 0): then
-                // alpha = 0, 1/(1-alpha) = 1, T and the running sums pass through unchanged and its gradient
-                // terms are exact zeros, so no further selects are needed.  The running value is
-                // d = T_final*v_acc - buffer.v, and the colour sums are kept negated (nfac = -alpha*T).
-                f2 S0p = dup2(0.f), Syp = dup2(0.f), Syyp = dup2(0.f);
-                f2 ncr = dup2(0.f), ncg = dup2(0.f), ncb = dup2(0.f), ncd = dup2(0.f), nact = dup2(0.f);
-                const f2 dyb = f2{dy0, dy0 - 2.f};
-#pragma unroll
-                for (int q = 0; q < NP; ++q) {
-                    const f2 dy = add2(dyb, dup2(-(float)(4 * q)));
-                    const f2 sg = fma2(dy, fma2(dup2(B.x), dy, dup2(bdx)), dup2(ax2));
-                    const bool v0 = (__float_as_uint(sg.x) < lim1) && (k <= idx[2 * q]);
-                    const bool v1 = (__float_as_uint(sg.y) < lim1) && (k <= idx[2 * q + 1]);
-                    const f2 nraw = f2{v0 ? -fast_ex2(B.y - sg.x) : 0.f, v1 ? -fast_ex2(B.y - sg.y) : 0.f};  // -o*exp(-sigma)
-                    const f2 nal = f2{fmaxf(nclamp, nraw.x), fmaxf(nclamp, nraw.y)};                 // -alpha
-                    const f2 om = add2(nal, dup2(1.f));
-                    const f2 ra = f2{fast_rcp(om.x), fast_rcp(om.y)};
-                    const f2 Tk = mul2(T2[q], ra);
-                    T2[q] = Tk;
-                    const f2 nfac = mul2(nal, Tk);
-                    nact = add2(nact, nfac);
-                    ncr = fma2(nfac, vr2[q], ncr); ncg = fma2(nfac, vg2[q], ncg); ncb = fma2(nfac, vb2[q], ncb);
-                    f2 dotc = fma2(dup2(B.z), vr2[q], fma2(dup2(B.w), vg2[q], mul2(dup2(Cc.x), vb2[q])));
-                    if (DEPTHG) {
-                        ncd = fma2(nfac, vd2[q], ncd);
-                        dotc = fma2(dup2(Cc.y), vd2[q], dotc);
-                    }
-                    const f2 v_alpha = fma2(Tk, dotc, mul2(ra, d2[q]));
-                    d2[q] = fma2(nfac, dotc, d2[q]);
-                    const f2 vs = mul2(nraw, v_alpha);  // d/d sigma = -o*vis*v_alpha
-                    S0p = add2(S0p, vs);
-                    const f2 vsy = mul2(vs, dy);
-                    Syp = add2(Syp, vsy);
-                    Syyp = fma2(vsy, dy, Syyp);
-                }
-                S0 = S0p.x + S0p.y; Sy = Syp.x + Syp.y; Syy = Syyp.x + Syyp.y;
-                cr = -(ncr.x + ncr.y); cg = -(ncg.x + ncg.y); cb = -(ncb.x + ncb.y);
-                if (DEPTHG) cd = -(ncd.x + ncd.y);
-                activity = nact.x + nact.y;
-            } else {
-            // straight-line, predicated (see the forward)
-#pragma unroll
-            for (int s = 0; s < PPL; ++s) {
-                const float dy = dy0 - (float)(2 * s);
-                const float sg = __fmaf_rn(dy, __fmaf_rn(B.x, dy, bdx), ax2);
-                const bool valid = (__float_as_uint(sg) < lim1) && (k <= idx[s]);
-                const float raw = fast_ex2(B.y - sg);       // o * exp(-sigma)
-                const float alpha = fminf(clampb, raw);
-                const float ra = fast_rcp(1.f - alpha);
-                const bool vm = valid;
-                const float Tk = vm ? T[s] * ra : T[s];
-                T[s] = Tk;
-                const float fac = vm ? alpha * Tk : 0.f;
-                activity += fac;
-                cr = __fmaf_rn(fac, vr[s], cr); cg = __fmaf_rn(fac, vg[s], cg); cb = __fmaf_rn(fac, vb[s], cb);
-                // v_alpha = sum_c (c*T - buffer_c*ra) * v_c + T_final*ra*v_acc  =  T*(c.v) + ra*(T_final*v_acc - buffer.v)
-                float dotc = __fmaf_rn(B.z, vr[s], __fmaf_rn(B.w, vg[s], Cc.x * vb[s]));
-                if (DEPTHG) {
-                    cd = __fmaf_rn(fac, vd[s], cd);
-                    dotc = __fmaf_rn(Cc.y, vd[s], dotc);
-                }
-                const float v_alpha = __fmaf_rn(Tk, dotc, ra * (tfv[s] - bv[s]));
-                bv[s] = __fmaf_rn(fac, dotc, bv[s]);
-                const float vs = valid ? -raw * v_alpha : 0.f;   // d/d sigma = -o*vis*v_alpha
-                S0 += vs;
-                const float vsy = vs * dy;
-                Sy += vsy;
-                Syy = __fmaf_rn(vsy, dy, Syy);
-            }
-            }
-            if (!__any_sync(FULL, activity != 0.f)) continue;
-            // true conic from the staged (log2e-scaled) one
-            const float ca = A.z * (2.f * LN2), cbb = A.w * LN2, cc = B.x * (2.f * LN2);
-            float l0 = ca * dx * S0 + cbb * Sy;     // v_xy.x
-            float l1 = cbb * dx * S0 + cc * Sy;     // v_xy.y
-            float l2 = 0.5f * dx * dx * S0;         // v_conic.x
-            float l3 = dx * Sy;                     // v_conic.y
-            float l4 = 0.5f * Syy;                  // v_conic.z
-            float l5 = -S0 / o;                     // v_opacity = sum vis * v_alpha
-            // one component of the record-layout gradient per lane pair
-            float comps[NV] = {l0, l1, l2, l3, l4, l5, cr, cg, cb};
-            if (DEPTHG) comps[NV - 1] = cd;
-            const size_t dst = (size_t)(__float_as_int(Cc.z) & ID_MASK) * SGN_RECORD_FLOATS + (my_comp >= 0 ? my_comp : 0);
-            const float mine = warp_multi_reduce<NV>(comps, lane);
-            if (my_comp >= 0) accumulate_grad(p, fscale, dst, mine);
-        }
-        buf ^= 1;
-    }
-}
-
-// the prologue (v_sky, cotangent chain) must run for every pixel, so strips are always launched for the
-// whole tile: W strips of 16/W rows
-template <bool DEPTHG, bool PACK>
-__global__ void __launch_bounds__(32, BLEND_BWD_MIN_BLOCKS) blend_bwd_kernel(const BlendBwdParams p) {
-    __shared__ float4 sA[2][32];
-    __shared__ float4 sB[2][32];
-    __shared__ float4 sC[2][32];
-    int tile, strip;
-    if (!take_work(p.sched, SLOT_MAIN, p.tiles, tile, strip)) return;
-    const int2 range = p.tile_bins[tile];
-    const int W = strips_for(p.tile_depth[tile], p.split_main);
-    if (strip >= W) return;
-    switch (W) {
-        case 1: blend_bwd_strip<8, DEPTHG, PACK>(p, tile, strip, range, sA, sB, sC); break;
-        case 2: blend_bwd_strip<4, DEPTHG, PACK>(p, tile, strip, range, sA, sB, sC); break;
-        case 4: blend_bwd_strip<2, DEPTHG, PACK>(p, tile, strip, range, sA, sB, sC); break;
-        default: blend_bwd_strip<1, DEPTHG, PACK>(p, tile, strip, range, sA, sB, sC); break;
-    }
-}
-
-// backward of the accumulation-only pass: out = 1 - T_final  =>  v_alpha_k = T_final * ra_k * v_out
+// backward of the accumulation-only pass: out = 1 - T_final  =>  v_alpha_k = T_final * ra_k * v_out.  Walks the class
+// sub-list positions [range.x, range.y) back to front; tfv = T_final * v_out and idx (a sub-list position) per pixel.
 template <int PPL, bool SKIP>
-__device__ __forceinline__ void acc_bwd_strip(const BlendBwdParams& p, int cls, int tile, int strip, const int2 range,
-                                              float4 (*sA)[32], float4 (*sB)[32], float (*sR)[32]) {
-    const int32_t* __restrict__ ids = p.cls_ids[cls];
-    const int slot = cls ? SLOT_OBJ : SLOT_BG;
-    const float* __restrict__ v_out = cls ? p.v_obj : p.v_bg;
+__device__ __forceinline__ void acc_bwd_traverse(const BlendBwdParams& p, const int32_t* __restrict__ ids, int tile, int strip,
+                                                 const int2 range, const float (&tfv)[PPL], const int (&idx)[PPL],
+                                                 float4 (*sA)[32], float4 (*sB)[32], float (*sR)[32]) {
     const float yc0 = (float)((tile / p.tiles_x) * SGN_TILE + strip * (2 * PPL)) + 1.0f;
     const int tx = tile % p.tiles_x, ty = tile / p.tiles_x;
     const int lane = threadIdx.x;
     const int j = tx * SGN_TILE + (lane & 15);
     const int i0 = ty * SGN_TILE + strip * (2 * PPL) + (lane >> 4);
     const float px = (float)j + 0.5f, py0 = (float)i0 + 0.5f;
-    if (range.y <= range.x) return;
-    const size_t P = (size_t)p.width * p.height;
-    float tfv[PPL];
-    int idx[PPL];
-    int kmax = -1;
-#pragma unroll
-    for (int s = 0; s < PPL; ++s) {
-        tfv[s] = 0.f; idx[s] = -1;
-        const int i = i0 + 2 * s;
-        if (j >= p.width || i >= p.height) continue;
-        const size_t pid = (size_t)i * p.width + j;
-        tfv[s] = p.final_T[slot * P + pid] * v_out[pid];
-        idx[s] = p.final_idx[slot * P + pid];
-        kmax = max(kmax, idx[s]);
-    }
-    const int wkmax = warp_max(kmax);
-    const int hi0 = min(range.y, wkmax + 1);
-    if (hi0 <= range.x) return;
     const int my_comp = multi_reduce_slot<6>(lane);
     const float clampb = in_register(p.clamp_bwd), nclamp = -clampb;
     const float fscale = p.v_fixed ? __ldg(p.fixed_scale) : 0.f;
     Staged nxt;
-    if (hi0 - 1 - lane >= range.x) nxt = gather_entry(p.records, ids[hi0 - 1 - lane]);
+    if (range.y - 1 - lane >= range.x) nxt = gather_entry(p.records, ids[range.y - 1 - lane]);
     int buf = 0;
-    for (int hi = hi0; hi > range.x; hi -= 32) {
+    for (int hi = range.y; hi > range.x; hi -= 32) {
         sA[buf][lane] = nxt.A; sB[buf][lane] = make_float4(nxt.B.x, nxt.B.y, nxt.C.z, nxt.C.w);
         sR[buf][lane] = row_reach(nxt) + 0.5f;
         __syncwarp();
@@ -1228,6 +1068,320 @@ __device__ __forceinline__ void acc_bwd_strip(const BlendBwdParams& p, int cls, 
         }
         buf ^= 1;
     }
+}
+
+// DEPTHG: the depth output has a cotangent.  OBJ: object_acc has one; its gradient is folded into the main traversal
+// (see below).
+// (Measured and dropped: software-pipelining the reduction of entry t-1 under the arithmetic of entry t -- it
+// has to run unconditionally, which costs more than the overlap gains: 0.87 vs 0.82 ms on cfg3.)
+template <int PPL, bool DEPTHG, bool PACK, bool OBJ>
+__device__ __forceinline__ void blend_bwd_strip(const BlendBwdParams& p, int tile, int strip, const int2 range,
+                                                float4 (*sA)[32], float4 (*sB)[32], float4 (*sC)[32]) {
+    const int tx = tile % p.tiles_x, ty = tile / p.tiles_x;
+    const int lane = threadIdx.x;
+    const int j = tx * SGN_TILE + (lane & 15);
+    const int i0 = ty * SGN_TILE + strip * (2 * PPL) + (lane >> 4);
+    const float px = (float)j + 0.5f, py0 = (float)i0 + 0.5f;
+    const size_t P = (size_t)p.width * p.height;
+
+    // ---- per-pixel prologue: cotangents of the RAW blend outputs from those of the final outputs
+    float T[PPL], tfv[PPL];
+    float vr[PPL], vg[PPL], vb[PPL], vd[PPL];
+    float bv[PPL];  // running  sum_{later k} (c_k . v_out) * alpha_k * T_k  (gsplat's `buffer` dotted with v_out)
+    int idx[PPL];
+    float tfo[PPL];  // OBJ: T_final * v_out of the objects-only accumulation
+    int idxo[PPL];   // OBJ: its last entry, as an object sub-list position
+    int kmax = -1, kmaxo = -1;
+#pragma unroll
+    for (int s = 0; s < PPL; ++s) {
+        T[s] = 1.f; tfv[s] = 0.f; vr[s] = vg[s] = vb[s] = vd[s] = 0.f;
+        bv[s] = 0.f;
+        idx[s] = -1;
+        tfo[s] = 0.f; idxo[s] = -1;
+        const int i = i0 + 2 * s;
+        if (j >= p.width || i >= p.height) continue;
+        const size_t pid = (size_t)i * p.width + j;
+        const float Tf = p.final_T[SLOT_MAIN * P + pid];
+        idx[s] = p.final_idx[SLOT_MAIN * P + pid];
+        T[s] = Tf;
+        const float alpha = 1.f - Tf;
+        const float4 raw = p.raw[pid];
+        float voa = p.v_acc ? p.v_acc[pid] : 0.f;
+        if (p.v_bg && p.final_idx[SLOT_BG * P + pid] == BG_SAME_AS_MAIN) voa += p.v_bg[pid];  // background_acc == accumulation here
+        if (p.raw_mode) {  // out_c = blended_c + (1 - alpha) * bg_c
+            if (p.v_rgb) {
+                vr[s] = p.v_rgb[3 * pid]; vg[s] = p.v_rgb[3 * pid + 1]; vb[s] = p.v_rgb[3 * pid + 2];
+                voa -= p.bg[0] * vr[s] + p.bg[1] * vg[s] + p.bg[2] * vb[s];
+            }
+            if (DEPTHG) { vd[s] = p.v_depth[pid]; voa -= p.bg[3] * vd[s]; }
+        } else if (p.v_rgb) {
+            float v[3] = {p.v_rgb[3 * pid], p.v_rgb[3 * pid + 1], p.v_rgb[3 * pid + 2]};
+            const float rr[3] = {raw.x, raw.y, raw.z};
+            float vraw[3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const float cl = fminf(rr[c], 1.f);
+                float fin = cl;
+                float sk = 0.f;
+                if (p.has_sky) { sk = p.sky[3 * pid + c]; fin = cl * alpha + sk * (1.f - alpha); }
+                if (p.eval_clamp && (fin < 0.f || fin > 1.f)) v[c] = 0.f;
+                if (p.has_sky) {
+                    voa += v[c] * (cl - sk);
+                    if (p.v_sky) p.v_sky[3 * pid + c] = v[c] * (1.f - alpha);
+                    vraw[c] = (rr[c] <= 1.f) ? v[c] * alpha : 0.f;
+                } else {
+                    vraw[c] = (rr[c] <= 1.f) ? v[c] : 0.f;
+                }
+            }
+            vr[s] = vraw[0]; vg[s] = vraw[1]; vb[s] = vraw[2];
+        }
+        if (DEPTHG && !p.raw_mode) {
+            if (alpha > 1e-3f) {
+                const float vdep = p.v_depth[pid];
+                vd[s] = vdep / alpha;
+                voa += -vdep * raw.w / (alpha * alpha);
+            }
+        }
+        tfv[s] = Tf * voa;
+        kmax = max(kmax, idx[s]);
+        if (OBJ) {
+            tfo[s] = p.final_T[SLOT_OBJ * P + pid] * p.v_obj[pid];
+            idxo[s] = p.final_idx[SLOT_OBJ * P + pid];
+            kmaxo = max(kmaxo, idxo[s]);
+        }
+    }
+    if (range.y <= range.x) return;  // empty tile (after the prologue: v_sky is written for every pixel)
+    const int wkmax = warp_max(kmax);
+    const int hi0 = min(range.y, wkmax + 1);  // entries at positions >= hi0 matter to no pixel's main stream
+    if (!OBJ && hi0 <= range.x) return;
+
+    // OBJ: the objects-only accumulation's gradient, folded into this traversal.  An object entry at list position k < hi0
+    // is the object sub-list entry of position orank (counted back to front from the number of object entries in
+    // [range.x, hi0)); it adds T_final_o * ra * v_obj to the v_alpha of the pixels whose objects-only stream took it
+    // (orank <= idxo), before the one shared reduction.  Object entries at positions >= hi0 are left to acc_bwd_traverse.
+    int orank = 0;
+    if constexpr (OBJ) {
+        int nobj = 0;
+#pragma unroll 4
+        for (int b = range.x; b < hi0; b += 32) nobj += __popc(__ballot_sync(FULL, b + lane < hi0 && p.sorted_ids[b + lane] < 0));
+        orank = p.cls_bins[1][tile].x + nobj;
+    }
+    const int orest = orank;  // first object sub-list position past this traversal
+
+    Staged nxt;
+    if (hi0 - 1 - lane >= range.x) nxt = gather_entry(p.records, p.sorted_ids[hi0 - 1 - lane]);
+    int buf = 0;
+    constexpr int NV = DEPTHG ? 10 : 9;
+    const int my_comp = multi_reduce_slot<NV>(lane);
+    const float clampb = in_register(p.clamp_bwd), nclamp = -clampb;
+    const float fscale = p.v_fixed ? __ldg(p.fixed_scale) : 0.f;
+    constexpr bool PK = PACK && PPL >= 2;
+    constexpr int NP = PK ? PPL / 2 : 1;
+    f2 T2[NP], d2[NP], vr2[NP], vg2[NP], vb2[NP], vd2[NP];
+    if constexpr (PK) {
+#pragma unroll
+        for (int q = 0; q < NP; ++q) {
+            T2[q] = f2{T[2 * q], T[2 * q + 1]}; d2[q] = f2{tfv[2 * q], tfv[2 * q + 1]};
+            vr2[q] = f2{vr[2 * q], vr[2 * q + 1]}; vg2[q] = f2{vg[2 * q], vg[2 * q + 1]};
+            vb2[q] = f2{vb[2 * q], vb[2 * q + 1]}; vd2[q] = f2{vd[2 * q], vd[2 * q + 1]};
+        }
+    }
+    for (int hi = hi0; hi > range.x; hi -= 32) {
+        sA[buf][lane] = nxt.A; sB[buf][lane] = nxt.B; sC[buf][lane] = nxt.C;
+        __syncwarp();
+        if (hi - 33 - lane >= range.x) nxt = gather_entry(p.records, p.sorted_ids[hi - 33 - lane]);
+        const int n = min(32, hi - range.x);
+        for (int t = 0; t < n; ++t) {
+            const int k = hi - 1 - t;
+            const float4 A = sA[buf][t];
+            const float4 B = sB[buf][t];
+            const float4 Cc = sC[buf][t];
+            const float dx = A.x - px;
+            const float bdx = A.w * dx, ax2 = A.z * dx * dx;
+            const float dy0 = A.y - py0;
+            // valid  <=>  0 <= sg <= log2(255 o)  <=>  bits(sg) < lim1  (see blend_fwd_strip), and k <= idx
+            const unsigned lim1 = (unsigned)(max(__float_as_int(LOG2_255 + B.y), -1) + 1);
+            const float o = Cc.w;
+            float S0 = 0.f, Sy = 0.f, Syy = 0.f, cr = 0.f, cg = 0.f, cb = 0.f, cd = 0.f;
+            float activity = 0.f;  // sum of alpha*T over the valid slots: non-zero iff some pixel of this lane took the entry
+            // OE (warp-uniform): an object entry, whose objects-only gradient is added here as well
+            auto entry = [&](auto obj_tag) {
+                constexpr bool OE = decltype(obj_tag)::value;
+                if constexpr (PK) {
+                    // packed row-slot pairs.  An invalid slot is masked ONCE, at the exponential (raw = 0): then
+                    // alpha = 0, 1/(1-alpha) = 1, T and the running sums pass through unchanged and its gradient
+                    // terms are exact zeros, so no further selects are needed.  The running value is
+                    // d = T_final*v_acc - buffer.v, and the colour sums are kept negated (nfac = -alpha*T).
+                    // (OE: a slot valid for the objects-only stream only masks the main terms with selects.)
+                    f2 S0p = dup2(0.f), Syp = dup2(0.f), Syyp = dup2(0.f);
+                    f2 ncr = dup2(0.f), ncg = dup2(0.f), ncb = dup2(0.f), ncd = dup2(0.f), nact = dup2(0.f);
+                    const f2 dyb = f2{dy0, dy0 - 2.f};
+#pragma unroll
+                    for (int q = 0; q < NP; ++q) {
+                        const f2 dy = add2(dyb, dup2(-(float)(4 * q)));
+                        const f2 sg = fma2(dy, fma2(dup2(B.x), dy, dup2(bdx)), dup2(ax2));
+                        const bool s0 = __float_as_uint(sg.x) < lim1, s1 = __float_as_uint(sg.y) < lim1;
+                        const bool v0 = s0 && (k <= idx[2 * q]), v1 = s1 && (k <= idx[2 * q + 1]);
+                        const bool o0 = OE && s0 && (orank <= idxo[2 * q]), o1 = OE && s1 && (orank <= idxo[2 * q + 1]);
+                        const f2 nraw = f2{(v0 || o0) ? -fast_ex2(B.y - sg.x) : 0.f, (v1 || o1) ? -fast_ex2(B.y - sg.y) : 0.f};  // -o*exp(-sigma)
+                        const f2 nal = f2{fmaxf(nclamp, nraw.x), fmaxf(nclamp, nraw.y)};                 // -alpha
+                        const f2 om = add2(nal, dup2(1.f));
+                        const f2 ra = f2{fast_rcp(om.x), fast_rcp(om.y)};
+                        f2 ram = ra, nalm = nal;  // the main stream's
+                        if (OE) {
+                            ram = f2{v0 ? ra.x : 1.f, v1 ? ra.y : 1.f};
+                            nalm = f2{v0 ? nal.x : 0.f, v1 ? nal.y : 0.f};
+                        }
+                        const f2 Tk = mul2(T2[q], ram);
+                        T2[q] = Tk;
+                        const f2 nfac = mul2(nalm, Tk);
+                        nact = add2(nact, nfac);
+                        ncr = fma2(nfac, vr2[q], ncr); ncg = fma2(nfac, vg2[q], ncg); ncb = fma2(nfac, vb2[q], ncb);
+                        f2 dotc = fma2(dup2(B.z), vr2[q], fma2(dup2(B.w), vg2[q], mul2(dup2(Cc.x), vb2[q])));
+                        if (DEPTHG) {
+                            ncd = fma2(nfac, vd2[q], ncd);
+                            dotc = fma2(dup2(Cc.y), vd2[q], dotc);
+                        }
+                        f2 v_alpha = fma2(Tk, dotc, mul2(ram, d2[q]));
+                        d2[q] = fma2(nfac, dotc, d2[q]);
+                        if (OE) {
+                            v_alpha = f2{v0 ? v_alpha.x : 0.f, v1 ? v_alpha.y : 0.f};
+                            v_alpha = fma2(ra, f2{o0 ? tfo[2 * q] : 0.f, o1 ? tfo[2 * q + 1] : 0.f}, v_alpha);
+                            nact = add2(nact, f2{o0 ? nal.x : 0.f, o1 ? nal.y : 0.f});
+                        }
+                        const f2 vs = mul2(nraw, v_alpha);  // d/d sigma = -o*vis*v_alpha
+                        S0p = add2(S0p, vs);
+                        const f2 vsy = mul2(vs, dy);
+                        Syp = add2(Syp, vsy);
+                        Syyp = fma2(vsy, dy, Syyp);
+                    }
+                    S0 = S0p.x + S0p.y; Sy = Syp.x + Syp.y; Syy = Syyp.x + Syyp.y;
+                    cr = -(ncr.x + ncr.y); cg = -(ncg.x + ncg.y); cb = -(ncb.x + ncb.y);
+                    if (DEPTHG) cd = -(ncd.x + ncd.y);
+                    activity = nact.x + nact.y;
+                } else {
+                // straight-line, predicated (see the forward)
+#pragma unroll
+                for (int s = 0; s < PPL; ++s) {
+                    const float dy = dy0 - (float)(2 * s);
+                    const float sg = __fmaf_rn(dy, __fmaf_rn(B.x, dy, bdx), ax2);
+                    const bool sv = __float_as_uint(sg) < lim1;
+                    const bool valid = sv && (k <= idx[s]);
+                    const bool ov = OE && sv && (orank <= idxo[s]);
+                    const float raw = fast_ex2(B.y - sg);       // o * exp(-sigma)
+                    const float alpha = fminf(clampb, raw);
+                    const float ra = fast_rcp(1.f - alpha);
+                    const bool vm = valid;
+                    const float Tk = vm ? T[s] * ra : T[s];
+                    T[s] = Tk;
+                    const float fac = vm ? alpha * Tk : 0.f;
+                    activity += fac;
+                    cr = __fmaf_rn(fac, vr[s], cr); cg = __fmaf_rn(fac, vg[s], cg); cb = __fmaf_rn(fac, vb[s], cb);
+                    // v_alpha = sum_c (c*T - buffer_c*ra) * v_c + T_final*ra*v_acc  =  T*(c.v) + ra*(T_final*v_acc - buffer.v)
+                    float dotc = __fmaf_rn(B.z, vr[s], __fmaf_rn(B.w, vg[s], Cc.x * vb[s]));
+                    if (DEPTHG) {
+                        cd = __fmaf_rn(fac, vd[s], cd);
+                        dotc = __fmaf_rn(Cc.y, vd[s], dotc);
+                    }
+                    float v_alpha = __fmaf_rn(Tk, dotc, ra * (tfv[s] - bv[s]));
+                    bv[s] = __fmaf_rn(fac, dotc, bv[s]);
+                    if (OE) {
+                        v_alpha = valid ? v_alpha : 0.f;
+                        v_alpha = ov ? __fmaf_rn(ra, tfo[s], v_alpha) : v_alpha;
+                        activity += ov ? alpha : 0.f;
+                    }
+                    const float vs = (valid || ov) ? -raw * v_alpha : 0.f;   // d/d sigma = -o*vis*v_alpha
+                    S0 += vs;
+                    const float vsy = vs * dy;
+                    Sy += vsy;
+                    Syy = __fmaf_rn(vsy, dy, Syy);
+                }
+                }
+            };
+            if (OBJ && __float_as_int(Cc.z) < 0) {
+                --orank;
+                entry(std::true_type{});
+            } else {
+                entry(std::false_type{});
+            }
+            if (!__any_sync(FULL, activity != 0.f)) continue;
+            // true conic from the staged (log2e-scaled) one
+            const float ca = A.z * (2.f * LN2), cbb = A.w * LN2, cc = B.x * (2.f * LN2);
+            float l0 = ca * dx * S0 + cbb * Sy;     // v_xy.x
+            float l1 = cbb * dx * S0 + cc * Sy;     // v_xy.y
+            float l2 = 0.5f * dx * dx * S0;         // v_conic.x
+            float l3 = dx * Sy;                     // v_conic.y
+            float l4 = 0.5f * Syy;                  // v_conic.z
+            float l5 = -S0 / o;                     // v_opacity = sum vis * v_alpha
+            // one component of the record-layout gradient per lane pair
+            float comps[NV] = {l0, l1, l2, l3, l4, l5, cr, cg, cb};
+            if (DEPTHG) comps[NV - 1] = cd;
+            const size_t dst = (size_t)(__float_as_int(Cc.z) & ID_MASK) * SGN_RECORD_FLOATS + (my_comp >= 0 ? my_comp : 0);
+            const float mine = warp_multi_reduce<NV>(comps, lane);
+            if (my_comp >= 0) accumulate_grad(p, fscale, dst, mine);
+        }
+        buf ^= 1;
+    }
+    if constexpr (OBJ) {  // object entries past this traversal: the accumulation-only backward
+        const int ohi = min(p.cls_bins[1][tile].y, warp_max(kmaxo) + 1);
+        if (ohi > orest) {
+            __syncwarp();  // every lane has finished reading the staging ring
+            acc_bwd_traverse<PPL, true>(p, p.cls_ids[1], tile, strip, make_int2(orest, ohi), tfo, idxo, sA, sB,
+                                        reinterpret_cast<float(*)[32]>(&sC[0][0]));
+        }
+    }
+}
+
+// the prologue (v_sky, cotangent chain) must run for every pixel, so strips are always launched for the
+// whole tile: W strips of 16/W rows.  OBJ: the strips are sized from the main depth plus how far the objects-only
+// streams run past it (tile_depth[object], see blend_fwd_strip).
+template <bool DEPTHG, bool PACK, bool OBJ>
+__global__ void __launch_bounds__(32, BLEND_BWD_MIN_BLOCKS) blend_bwd_kernel(const BlendBwdParams p) {
+    __shared__ float4 sA[2][32];
+    __shared__ float4 sB[2][32];
+    __shared__ float4 sC[2][32];
+    int tile, strip;
+    if (!take_work(p.sched, SLOT_MAIN, p.tiles, tile, strip)) return;
+    const int2 range = p.tile_bins[tile];
+    const int W = strips_for(p.tile_depth[tile] + (OBJ ? p.tile_depth[(size_t)SLOT_OBJ * p.tiles + tile] : 0), p.split_main);
+    if (strip >= W) return;
+    switch (W) {
+        case 1: blend_bwd_strip<8, DEPTHG, PACK, OBJ>(p, tile, strip, range, sA, sB, sC); break;
+        case 2: blend_bwd_strip<4, DEPTHG, PACK, OBJ>(p, tile, strip, range, sA, sB, sC); break;
+        case 4: blend_bwd_strip<2, DEPTHG, PACK, OBJ>(p, tile, strip, range, sA, sB, sC); break;
+        default: blend_bwd_strip<1, DEPTHG, PACK, OBJ>(p, tile, strip, range, sA, sB, sC); break;
+    }
+}
+
+// the background-only accumulation's backward (the objects-only one is part of blend_bwd_kernel)
+template <int PPL, bool SKIP>
+__device__ __forceinline__ void acc_bwd_strip(const BlendBwdParams& p, int cls, int tile, int strip, const int2 range,
+                                              float4 (*sA)[32], float4 (*sB)[32], float (*sR)[32]) {
+    const int slot = cls ? SLOT_OBJ : SLOT_BG;
+    const float* __restrict__ v_out = cls ? p.v_obj : p.v_bg;
+    const int tx = tile % p.tiles_x, ty = tile / p.tiles_x;
+    const int lane = threadIdx.x;
+    const int j = tx * SGN_TILE + (lane & 15);
+    const int i0 = ty * SGN_TILE + strip * (2 * PPL) + (lane >> 4);
+    if (range.y <= range.x) return;
+    const size_t P = (size_t)p.width * p.height;
+    float tfv[PPL];
+    int idx[PPL];
+    int kmax = -1;
+#pragma unroll
+    for (int s = 0; s < PPL; ++s) {
+        tfv[s] = 0.f; idx[s] = -1;
+        const int i = i0 + 2 * s;
+        if (j >= p.width || i >= p.height) continue;
+        const size_t pid = (size_t)i * p.width + j;
+        tfv[s] = p.final_T[slot * P + pid] * v_out[pid];
+        idx[s] = p.final_idx[slot * P + pid];
+        kmax = max(kmax, idx[s]);
+    }
+    const int wkmax = warp_max(kmax);
+    const int hi0 = min(range.y, wkmax + 1);
+    if (hi0 <= range.x) return;
+    acc_bwd_traverse<PPL, SKIP>(p, p.cls_ids[cls], tile, strip, make_int2(range.x, hi0), tfv, idx, sA, sB, sR);
 }
 
 template <bool SKIP>
@@ -1326,8 +1480,8 @@ extern "C" int sgn_blend_bwd(const sgn_camera* cam, const sgn_blend_opts* opts, 
     p.tile_depth = in->tile_depth;
     p.sched = in->sched;
     if (in->sched) {
-        sched_kernel<<<(in->v_object_acc || in->v_background_acc) ? 3 : 1, 1024, 0, stream>>>(
-            tiles, p.tile_bins, p.cls_bins[0], p.cls_bins[1], in->tile_depth, p.split_main, p.split_acc, in->sched);
+        sched_kernel<<<in->v_background_acc ? 2 : 1, 1024, 0, stream>>>(
+            tiles, p.tile_bins, p.cls_bins[0], in->tile_depth, in->v_object_acc != nullptr, p.split_main, p.split_acc, in->sched);
         SGN_CHECK_LAUNCH("sched_kernel");
     }
     {
@@ -1335,11 +1489,6 @@ extern "C" int sgn_blend_bwd(const sgn_camera* cam, const sgn_blend_opts* opts, 
         ForkJoin fj(stream);
         const bool acc_skip = !(opts->tuning & SGN_TUNE_ACC_NO_ROW_SKIP);
         const unsigned acc_grid = tiles * 8;
-        if (in->v_object_acc) {
-            if (acc_skip) acc_bwd_kernel<true><<<acc_grid, 32, 0, fj.side()>>>(p, 1);
-            else acc_bwd_kernel<false><<<acc_grid, 32, 0, fj.side()>>>(p, 1);
-            SGN_CHECK_LAUNCH("acc_bwd_kernel<object>");
-        }
         if (in->v_background_acc) {
             if (acc_skip) acc_bwd_kernel<true><<<acc_grid, 32, 0, fj.side()>>>(p, 0);
             else acc_bwd_kernel<false><<<acc_grid, 32, 0, fj.side()>>>(p, 0);
@@ -1348,11 +1497,15 @@ extern "C" int sgn_blend_bwd(const sgn_camera* cam, const sgn_blend_opts* opts, 
 
         const bool pack = (opts->tuning & SGN_TUNE_BWD_PACKED) != 0;
         const dim3 grid(tiles * 8), block(32);
-        switch ((in->v_depth ? 2 : 0) | (pack ? 1 : 0)) {
-            case 0: blend_bwd_kernel<false, false><<<grid, block, 0, stream>>>(p); break;
-            case 1: blend_bwd_kernel<false, true><<<grid, block, 0, stream>>>(p); break;
-            case 2: blend_bwd_kernel<true, false><<<grid, block, 0, stream>>>(p); break;
-            default: blend_bwd_kernel<true, true><<<grid, block, 0, stream>>>(p); break;
+        switch ((in->v_object_acc ? 4 : 0) | (in->v_depth ? 2 : 0) | (pack ? 1 : 0)) {
+            case 0: blend_bwd_kernel<false, false, false><<<grid, block, 0, stream>>>(p); break;
+            case 1: blend_bwd_kernel<false, true, false><<<grid, block, 0, stream>>>(p); break;
+            case 2: blend_bwd_kernel<true, false, false><<<grid, block, 0, stream>>>(p); break;
+            case 3: blend_bwd_kernel<true, true, false><<<grid, block, 0, stream>>>(p); break;
+            case 4: blend_bwd_kernel<false, false, true><<<grid, block, 0, stream>>>(p); break;
+            case 5: blend_bwd_kernel<false, true, true><<<grid, block, 0, stream>>>(p); break;
+            case 6: blend_bwd_kernel<true, false, true><<<grid, block, 0, stream>>>(p); break;
+            default: blend_bwd_kernel<true, true, true><<<grid, block, 0, stream>>>(p); break;
         }
         SGN_CHECK_LAUNCH("blend_bwd_kernel");
         fj.finish();

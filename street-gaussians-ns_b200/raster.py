@@ -458,7 +458,9 @@ def class_lists(cs: _lib.CameraStruct, M: int, sorted_ids, tile_bins):
 
 
 HEAVY_FIRST = os.environ.get("SGN_HEAVY_FIRST", "1") != "0"
-DEFAULT_TUNING = 4 | 8  # paired row-slot bodies, no row skipping in the main kernels
+# paired row-slot bodies in the main forward, scalar ones in the backward (with the objects-only gradient folded in, the
+# scalar backward body is the faster one on an H100; DESIGN.md §5), no row skipping in the main kernels
+DEFAULT_TUNING = 4
 
 
 def blend_opts(s: RenderSettings, has_sky: bool) -> _lib.BlendOpts:
