@@ -190,8 +190,9 @@ int sgn_l1_sh(int N, int K, int degree, const float* viewdirs, const float* coef
 int sgn_bin_count(int N, const sgn_camera* cam, const float* records, const int32_t* radii,
                   const uint16_t* tile_bbox, int32_t* tiles_touched, uint32_t* touch_mask, void* stream);
 /* step 1: stable depth order of the N rows (invisible rows last) and the inclusive scan of tiles_touched IN THAT
- * ORDER (cum[rank]); order[g] = where row g's run of entries starts in the depth-ordered entry sequence (the
- * exclusive scan value of its rank); the total M is also written to *total_dev (int64). */
+ * ORDER (cum[rank]); order[rank] = the entry payload of the row at that depth rank (row | object class << 31, the
+ * sorted_ids layout below), so the run of entries of rank r is [cum[r-1], cum[r]) with that payload; the total M is
+ * also written to *total_dev (int64). */
 size_t sgn_bin_scan_scratch_bytes(int N);
 int sgn_bin_scan(int N, const float* records, const int32_t* radii, const int32_t* tiles_touched,
                  int32_t* order, int32_t* cum, int64_t* total_dev, void* scratch, size_t scratch_bytes, void* stream);

@@ -4,8 +4,8 @@
 // ordered like a stable sort of (tile_id << 32 | float_bits(depth)) with emission order (Gaussian index)
 // as the tie break.  That order is produced in two cheaper stable steps instead of one 46-bit sort of
 // the M intersections:
-//   1. the N Gaussians are stably sorted by depth bits (32-bit keys, N elements);
-//   2. intersections are emitted in that order and stably sorted by their 14-bit tile id only.
+//   1. the N Gaussians are stably sorted by depth bits (32-bit keys, N elements), carrying their entry payloads;
+//   2. intersections are emitted in that order, rank by rank, and stably sorted by their 14-bit tile id only.
 // Step 2 moves 12 B per entry twice instead of 24 B six times.
 #include <cub/cub.cuh>
 
@@ -52,30 +52,30 @@ depth_keys_kernel(int N, const float4* __restrict__ records, const int32_t* __re
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= N) return;
     // invisible rows sort last (no positive float has all bits set) and emit nothing
-    keys[g] = radii[g] > 0 ? (uint32_t)__float_as_int(records[3 * (size_t)g + 2].y) : 0xffffffffu;
-    vals[g] = g;
+    uint32_t key = 0xffffffffu;
+    int32_t payload = g;
+    if (radii[g] > 0) {
+        const float4 r2 = records[3 * (size_t)g + 2];
+        key = (uint32_t)__float_as_int(r2.y);
+        // the entry payload travels with the depth key: Gaussian row in the low 31 bits, object-class flag in bit 31
+        if (__float_as_int(r2.z) & SGN_AUX_OBJECT) payload |= (int32_t)0x80000000;
+    }
+    keys[g] = key;
+    vals[g] = payload;
 }
 
 struct PermutedCount {
     const int32_t* order;
     const int32_t* counts;
-    __host__ __device__ int32_t operator()(int i) const { return counts[order[i]]; }
+    __host__ __device__ int32_t operator()(int i) const { return counts[order[i] & 0x7fffffff]; }
 };
-
-// start[g] = where the run of Gaussian g begins in the depth-ordered entry sequence: the exclusive scan value of its
-// depth rank, scattered back to row order so that the emit kernel reads it coalesced (no rank -> cum gathers)
-__global__ void __launch_bounds__(256)
-start_offsets_kernel(int N, const int32_t* __restrict__ rows_by_depth, const int32_t* __restrict__ cum, int32_t* __restrict__ start) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < N) start[rows_by_depth[i]] = (i == 0) ? 0 : cum[i - 1];
-}
 
 __global__ void write_total_kernel(const int32_t* __restrict__ cum, int N, int64_t* __restrict__ total) {
     if (threadIdx.x == 0 && blockIdx.x == 0) *total = (N > 0) ? (int64_t)cum[N - 1] : 0;
 }
 
 struct ScanLayout {
-    size_t keys_in, keys_out, vals_in, vals_out, temp, temp_bytes, total;
+    size_t keys_in, keys_out, vals_in, temp, temp_bytes, total;
 };
 static ScanLayout scan_layout(int N) {
     ScanLayout L;
@@ -87,8 +87,7 @@ static ScanLayout scan_layout(int N) {
     L.keys_in = 0;
     L.keys_out = align_up(n * 4, 256);
     L.vals_in = L.keys_out + align_up(n * 4, 256);
-    L.vals_out = L.vals_in + align_up(n * 4, 256);
-    L.temp = L.vals_out + align_up(n * 4, 256);
+    L.temp = L.vals_in + align_up(n * 4, 256);
     L.temp_bytes = t1 > t2 ? t1 : t2;
     L.total = L.temp + align_up(L.temp_bytes, 256) + 256;
     return L;
@@ -97,7 +96,7 @@ static ScanLayout scan_layout(int N) {
 extern "C" size_t sgn_bin_scan_scratch_bytes(int N) { return scan_layout(N).total; }
 
 extern "C" int sgn_bin_scan(int N, const float* records, const int32_t* radii, const int32_t* tiles_touched,
-                            int32_t* order /* out: rank[g], the position of row g in depth order */, int32_t* cum,
+                            int32_t* order /* out: entry payloads (row | class << 31) in depth order */, int32_t* cum,
                             int64_t* total_dev, void* scratch, size_t scratch_bytes, void* stream_) {
     SGN_RANGE("sgn_bin_scan");
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -114,89 +113,209 @@ extern "C" int sgn_bin_scan(int N, const float* records, const int32_t* radii, c
         int32_t* vals_in = (int32_t*)(base + L.vals_in);
         depth_keys_kernel<<<(N + 255) / 256, 256, 0, stream>>>(N, reinterpret_cast<const float4*>(records), radii, keys_in, vals_in);
         SGN_CHECK_LAUNCH("depth_keys_kernel");
-        int32_t* sorted_rows = (int32_t*)(base + L.vals_out);
         size_t temp = L.temp_bytes;
-        SGN_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(base + L.temp, temp, keys_in, keys_out, vals_in, sorted_rows, N, 0, 32, stream));
+        SGN_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(base + L.temp, temp, keys_in, keys_out, vals_in, order, N, 0, 32, stream));
         sgn_count_launch(1);
         // counts scanned IN DEPTH ORDER: cum[r] = number of entries emitted by the first r+1 rows of that order
         cub::CountingInputIterator<int> idx(0);
-        cub::TransformInputIterator<int32_t, PermutedCount, cub::CountingInputIterator<int>> it(idx, PermutedCount{sorted_rows, tiles_touched});
+        cub::TransformInputIterator<int32_t, PermutedCount, cub::CountingInputIterator<int>> it(idx, PermutedCount{order, tiles_touched});
         temp = L.temp_bytes;
         SGN_CHECK_CUDA(cub::DeviceScan::InclusiveSum(base + L.temp, temp, it, cum, N, stream));
         sgn_count_launch(1);
-        start_offsets_kernel<<<(N + 255) / 256, 256, 0, stream>>>(N, sorted_rows, cum, order);
-        SGN_CHECK_LAUNCH("start_offsets_kernel");
     }
+    // the synchronous path reads the total back before the emit, so it cannot wait for a later kernel
     write_total_kernel<<<1, 32, 0, stream>>>(cum, N, total_dev);
     SGN_CHECK_LAUNCH("write_total_kernel");
     return SGN_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
-// step 2: key emit (thread g handles Gaussian g -- coalesced reads -- and writes its run of entries at the
-// offset of its depth rank, so the emitted sequence is in depth order), stable sort by tile, bin edges
-__global__ void __launch_bounds__(256)
-emit_keys_kernel(int N, int tiles_x, int width, int height, int bw, const float4* __restrict__ records,
-                 const int32_t* __restrict__ radii, const ushort4* __restrict__ tile_bbox,
-                 const uint32_t* __restrict__ touch_mask, const int32_t* __restrict__ start, int end,
-                 uint16_t* __restrict__ keys, int32_t* __restrict__ vals) {
-    const int g = blockIdx.x * blockDim.x + threadIdx.x;
-    const int lane = threadIdx.x & 31;
-    const bool vis = (g < N) && radii[g] > 0;
-    ushort4 bb = make_ushort4(0, 0, 0, 0);
-    TouchCtx t = {};
-    int32_t payload = 0;
-    uint32_t mask = 0;
-    int cur = 0;  // `end` (= M) only guards the buffers: the counts come from the same test as the counting pass
-    if (vis) {
-        bb = tile_bbox[g];
-        // payload: Gaussian row in the low 31 bits, object-class flag in bit 31 (no gather needed later)
-        payload = g | ((__float_as_int(records[3 * (size_t)g + 2].z) & SGN_AUX_OBJECT) ? (int32_t)0x80000000 : 0);
-        mask = touch_mask[g];
-        cur = start[g];
+// step 2: key emit in depth order, stable sort by tile, bin edges.
+// Thread i handles depth rank i, so the 32 runs of a warp are adjacent in the entry sequence: run i occupies
+// [cum[i-1], cum[i]).  Runs of AABBs of at most COOP_AREA tiles are laid end to end and written 32 consecutive
+// entries per store: entry f of the warp's flattened sequence belongs to the last lane whose exclusive prefix is <= f
+// (as in count_touched_tiles), and is the k-th tile the owner reaches, i.e. the k-th set bit of the touch mask
+// project_fwd stored (no re-test).  Larger AABBs are listed and tested by emit_big_kernel.
+#define HUGE_AREA 1024  // AABBs above this many tiles are tested by a whole CTA
+
+// position of the k-th (0-based) set bit of m; m has more than k set bits
+__device__ __forceinline__ int nth_set_bit(uint32_t m, int k) {
+    int pos = 0;
+#pragma unroll
+    for (int w = 16; w > 0; w >>= 1) {
+        const int c = __popc(m & ((1u << w) - 1u));
+        if (k >= c) { k -= c; m >>= w; pos += w; }
     }
-    const int bwid = bb.z - bb.x, area = bwid * (bb.w - bb.y);
-    if (vis && area <= COOP_AREA) {
-        // the projection kernel already decided every tile of a small AABB: replay its bit mask, one AABB row
-        // at a time (no per-tile division by the AABB width)
-        const unsigned row_bits = bwid >= 32 ? 0xffffffffu : ((1u << bwid) - 1u);
-        for (int ty = bb.y; ty < bb.w && mask && cur < end; ++ty) {
-            unsigned rm = mask & row_bits;
-            mask = bwid >= 32 ? 0u : (mask >> bwid);
-            const int base = ty * tiles_x + bb.x;
-            while (rm && cur < end) {
-                const int bit = __ffs(rm) - 1;
-                rm &= rm - 1;
-                keys[cur] = (uint16_t)(base + bit);
-                vals[cur] = payload;
-                ++cur;
+    return pos;
+}
+
+// `end` bounds the buffers (M, or the capacity); with `total` (capped form) the slots [min(*total, end), end) get the
+// padding key, which sorts behind every tile
+__global__ void __launch_bounds__(256)
+emit_keys_kernel(int N, int tiles_x, const ushort4* __restrict__ tile_bbox, const uint32_t* __restrict__ touch_mask,
+                 const int32_t* __restrict__ order, const int32_t* __restrict__ cum, int end, const int64_t* __restrict__ total,
+                 uint16_t sentinel, uint16_t* __restrict__ keys, int32_t* __restrict__ vals, int32_t* __restrict__ big_ranks,
+                 unsigned int* __restrict__ big_count) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int lane = threadIdx.x & 31;
+    int start = 0, n = 0;
+    int32_t payload = 0;
+    if (i < N) {
+        const int c = cum[i];
+        start = i > 0 ? cum[i - 1] : 0;
+        n = c - start;
+        payload = order[i];
+    }
+    if (start >= end) n = 0;  // truncated (capped form): the run lies past the buffers
+    // invisible rows come last in depth order and reach no tile: a warp of them has nothing to emit
+    if (__ballot_sync(0xffffffffu, n > 0)) {
+        const int row = payload & 0x7fffffff;
+        ushort4 bb = make_ushort4(0, 0, 0, 0);
+        uint32_t mask = 0;
+        if (n > 0) {
+            bb = tile_bbox[row];
+            mask = touch_mask[row];
+        }
+        const int bwid = bb.z - bb.x, area = bwid * (bb.w - bb.y);
+        const int mine = (n > 0 && area <= COOP_AREA) ? __popc(mask) : 0;
+        int pre = mine;  // inclusive scan
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, pre, o);
+            if (lane >= o) pre += v;
+        }
+        const int flat = __shfl_sync(0xffffffffu, pre, 31);
+        pre -= mine;  // exclusive
+        const int delta = start - pre;  // entry f of this lane's run goes to f + delta
+        const int tbase = bb.y * tiles_x + bb.x;
+        for (int base = 0; base < flat; base += 32) {
+            const int f = base + lane;
+            int o = 0;
+#pragma unroll
+            for (int step = 16; step > 0; step >>= 1) {
+                const int cand = o + step;  // <= 31
+                const int pc = __shfl_sync(0xffffffffu, pre, cand);
+                if (pc <= f) o = cand;
+            }
+            const int k = f - __shfl_sync(0xffffffffu, pre, o);
+            const uint32_t m = __shfl_sync(0xffffffffu, mask, o);
+            const int w = __shfl_sync(0xffffffffu, bwid, o);
+            const int tb = __shfl_sync(0xffffffffu, tbase, o);
+            const int pos = f + __shfl_sync(0xffffffffu, delta, o);
+            const int32_t pl = __shfl_sync(0xffffffffu, payload, o);
+            if (f < flat && pos < end) {
+                const int bit = nth_set_bit(m, k);
+                // bit < 32, w in [1, 32]: (bit + 0.5) / w lies at least 1/64 from an integer, far beyond the error of the
+                // approximate quotient, so the truncation is exact
+                const int r = (int)__fdividef((float)bit + 0.5f, (float)w);
+                keys[pos] = (uint16_t)(tb + r * tiles_x + (bit - r * w));
+                vals[pos] = pl;
             }
         }
+        // AABBs above COOP_AREA tiles go to lists the whole grid works through (emit_big_kernel): the nearest, widest
+        // Gaussians come first in depth order, and one warp testing all of them would serialise the kernel's tail.  Runs
+        // up to HUGE_AREA tiles are counted from the front of big_ranks, larger ones from the back (each listed run has an
+        // entry below `end`, so the two never meet)
+        const unsigned big = __ballot_sync(0xffffffffu, n > 0 && area > COOP_AREA && area <= HUGE_AREA);
+        const unsigned huge = __ballot_sync(0xffffffffu, n > 0 && area > HUGE_AREA);
+        if (big) {
+            int at = 0;
+            if (lane == 0) at = (int)atomicAdd(&big_count[0], (unsigned)__popc(big));
+            at = __shfl_sync(0xffffffffu, at, 0);
+            if ((big >> lane) & 1u) big_ranks[at + __popc(big & ((1u << lane) - 1u))] = i;
+        }
+        if (huge) {
+            int at = 0;
+            if (lane == 0) at = (int)atomicAdd(&big_count[1], (unsigned)__popc(huge));
+            at = __shfl_sync(0xffffffffu, at, 0);
+            if ((huge >> lane) & 1u) big_ranks[end - 1 - (at + __popc(huge & ((1u << lane) - 1u)))] = i;
+        }
     }
-    unsigned big = __ballot_sync(0xffffffffu, vis && area > COOP_AREA);
-    if (big) {
-        if (vis && area > COOP_AREA) t = make_touch_ctx(records[3 * (size_t)g], records[3 * (size_t)g + 1]);
-        while (big) {
-            const int src = __ffs(big) - 1;
-            big &= big - 1;
-            const TouchCtx c = shfl_ctx(t, src);
-            const int x0 = __shfl_sync(0xffffffffu, (int)bb.x, src), y0 = __shfl_sync(0xffffffffu, (int)bb.y, src);
-            const int w = __shfl_sync(0xffffffffu, bwid, src), ar = __shfl_sync(0xffffffffu, area, src);
-            const int32_t pl = __shfl_sync(0xffffffffu, payload, src);
-            int pos = __shfl_sync(0xffffffffu, cur, src);
-            const int lim = end;
-            for (int base = 0; base < ar; base += 32) {
-                const int ti = base + lane;
-                const int tx = x0 + ti % w, ty = y0 + ti / w;
-                const bool ok = (ti < ar) && tile_touched(c, tx, ty, width, height, bw);
-                const unsigned m = __ballot_sync(0xffffffffu, ok);
-                const int my = pos + __popc(m & ((1u << lane) - 1u));
-                if (ok && my < lim) {  // my >= lim cannot happen: same test as the counting pass
-                    keys[my] = (uint16_t)(ty * tiles_x + tx);
-                    vals[my] = pl;
-                }
-                pos += __popc(m);
+    if (total) {
+        const int64_t m = min(*total, (int64_t)end);
+        for (int64_t j = m + i; j < end; j += (int64_t)gridDim.x * blockDim.x) {
+            keys[j] = sentinel;
+            vals[j] = 0;
+        }
+    }
+}
+
+// The runs of the AABBs above COOP_AREA tiles.  The tiles of an AABB are tested in row-major steps, the reached ones written
+// contiguously from the run's start, so a run is a serial chain of steps: runs above HUGE_AREA tiles are taken by whole CTAs
+// (EMIT_BIG_THREADS tiles per step), the others by single warps (32 tiles per step), the CTAs / warps of the grid taking the
+// listed ranks in turn.
+#define EMIT_BIG_THREADS 256
+
+struct BigRun {
+    TouchCtx c;
+    int32_t pl;
+    int x0, y0, wd, ar, pos;
+};
+
+__device__ __forceinline__ BigRun big_run(int i, const float4* __restrict__ records, const ushort4* __restrict__ tile_bbox,
+                                          const int32_t* __restrict__ order, const int32_t* __restrict__ cum) {
+    BigRun r;
+    r.pl = order[i];
+    const int row = r.pl & 0x7fffffff;
+    const ushort4 bb = tile_bbox[row];
+    r.c = make_touch_ctx(records[3 * (size_t)row], records[3 * (size_t)row + 1]);
+    r.x0 = bb.x; r.y0 = bb.y; r.wd = bb.z - bb.x; r.ar = r.wd * (bb.w - bb.y);
+    r.pos = i > 0 ? cum[i - 1] : 0;
+    return r;
+}
+
+__global__ void __launch_bounds__(EMIT_BIG_THREADS)
+emit_big_kernel(int tiles_x, int width, int height, int bw, const float4* __restrict__ records, const ushort4* __restrict__ tile_bbox,
+                const int32_t* __restrict__ order, const int32_t* __restrict__ cum, int end, const int32_t* __restrict__ big_ranks,
+                const unsigned int* __restrict__ big_count, uint16_t* __restrict__ keys, int32_t* __restrict__ vals) {
+    constexpr int WARPS = EMIT_BIG_THREADS / 32;
+    __shared__ int warp_hits[2][WARPS];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const unsigned lt = (1u << lane) - 1u;
+    // runs above HUGE_AREA tiles: a CTA per run
+    const int huge = (int)big_count[1];
+    int buf = 0;
+    for (int h = blockIdx.x; h < huge; h += gridDim.x) {
+        BigRun r = big_run(big_ranks[end - 1 - h], records, tile_bbox, order, cum);
+        for (int b = 0; b < r.ar && r.pos < end; b += EMIT_BIG_THREADS) {
+            const int ti = b + threadIdx.x;
+            const int tx = r.x0 + ti % r.wd, ty = r.y0 + ti / r.wd;
+            const bool ok = (ti < r.ar) && tile_touched(r.c, tx, ty, width, height, bw);
+            const unsigned bal = __ballot_sync(0xffffffffu, ok);
+            if (lane == 0) warp_hits[buf][warp] = __popc(bal);
+            __syncthreads();  // one barrier per step: the counts alternate between two buffers
+            int before = 0, all = 0;
+#pragma unroll
+            for (int k = 0; k < WARPS; ++k) {
+                const int c = warp_hits[buf][k];
+                before += k < warp ? c : 0;
+                all += c;
             }
+            const int my = r.pos + before + __popc(bal & lt);
+            if (ok && my < end) {
+                keys[my] = (uint16_t)(ty * tiles_x + tx);
+                vals[my] = r.pl;
+            }
+            r.pos += all;
+            buf ^= 1;
+        }
+    }
+    // the others: a warp per run
+    const int warps = (gridDim.x * blockDim.x) >> 5;
+    const int count = (int)big_count[0];
+    for (int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < count; w += warps) {
+        BigRun r = big_run(big_ranks[w], records, tile_bbox, order, cum);
+        for (int b = 0; b < r.ar && r.pos < end; b += 32) {
+            const int ti = b + lane;
+            const int tx = r.x0 + ti % r.wd, ty = r.y0 + ti / r.wd;
+            const bool ok = (ti < r.ar) && tile_touched(r.c, tx, ty, width, height, bw);
+            const unsigned bal = __ballot_sync(0xffffffffu, ok);
+            const int my = r.pos + __popc(bal & lt);
+            if (ok && my < end) {
+                keys[my] = (uint16_t)(ty * tiles_x + tx);
+                vals[my] = r.pl;
+            }
+            r.pos += __popc(bal);
         }
     }
 }
@@ -217,14 +336,7 @@ bin_edges_kernel(int64_t M, const uint16_t* __restrict__ keys_sorted, int32_t* _
     if (i == M - 1) tile_bins[2 * cur + 1] = (int32_t)M;
 }
 
-// capacity-bounded form: the number of entries stays on the device (no host read-back between the scan and the sort).
-// Slots [min(total, cap), cap) are filled with a key that sorts behind every tile, so the sort runs over `cap` items.
-__global__ void __launch_bounds__(256)
-pad_keys_kernel(int64_t cap, const int64_t* __restrict__ total, uint16_t sentinel, uint16_t* __restrict__ keys, int32_t* __restrict__ vals) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int64_t m = min(*total, cap);
-    if (i >= m && i < cap) { keys[i] = sentinel; vals[i] = 0; }
-}
+// capacity-bounded form: the number of entries stays on the device (no host read-back between the scan and the sort)
 __global__ void __launch_bounds__(256)
 bin_edges_capped_kernel(int64_t cap, const int64_t* __restrict__ total, const uint16_t* __restrict__ keys_sorted, int32_t* __restrict__ tile_bins,
                         int32_t* __restrict__ overflow) {
@@ -245,7 +357,7 @@ bin_edges_capped_kernel(int64_t cap, const int64_t* __restrict__ total, const ui
 }
 
 struct SortLayout {
-    size_t keys_in, keys_out, vals_in, temp, temp_bytes, total;
+    size_t keys_in, keys_out, vals_in, big, temp, temp_bytes, total;
 };
 
 static SortLayout sort_layout(int64_t M) {
@@ -257,7 +369,8 @@ static SortLayout sort_layout(int64_t M) {
     L.keys_in = 0;
     L.keys_out = align_up(L.keys_in + m * 2, 256);
     L.vals_in = align_up(L.keys_out + m * 2, 256);
-    L.temp = align_up(L.vals_in + m * 4, 256);
+    L.big = align_up(L.vals_in + m * 4, 256);  // two counts (256 B), then the ranks of the runs above COOP_AREA tiles (each has an entry)
+    L.temp = align_up(L.big + 256 + m * 4, 256);
     L.temp_bytes = temp;
     L.total = align_up(L.temp + temp, 256);
     return L;
@@ -289,18 +402,23 @@ static int bin_sort_impl(int N, int64_t M, const int64_t* total_dev, int32_t* ov
     uint16_t* keys_in = (uint16_t*)(base + L.keys_in);
     uint16_t* keys_out = (uint16_t*)(base + L.keys_out);
     int32_t* vals_in = (int32_t*)(base + L.vals_in);
-    emit_keys_kernel<<<(N + 255) / 256, 256, 0, stream>>>(N, tiles_x, cam->width, cam->height, bw,
-                                                          reinterpret_cast<const float4*>(records), radii,
-                                                          reinterpret_cast<const ushort4*>(tile_bbox), touch_mask, order, (int)M,
-                                                          keys_in, vals_in);
-    SGN_CHECK_LAUNCH("emit_keys_kernel");
+    unsigned int* big_count = (unsigned int*)(base + L.big);
+    int32_t* big_ranks = (int32_t*)(base + L.big + 256);
+    SGN_CHECK_CUDA(cudaMemsetAsync(big_count, 0, 2 * sizeof(unsigned int), stream));
     int tile_bits = 1;
     while ((1 << tile_bits) < tiles + (total_dev ? 1 : 0)) ++tile_bits;  // capped: one more key value, the padding sentinel
-    if (total_dev) {
-        SGN_REQUIRE(tile_bits <= 16, "sgn_bin_sort_capped: %d tiles leave no 16-bit key for the padding", tiles);
-        pad_keys_kernel<<<(unsigned)((M + 255) / 256), 256, 0, stream>>>(M, total_dev, (uint16_t)((1u << tile_bits) - 1u), keys_in, vals_in);
-        SGN_CHECK_LAUNCH("pad_keys_kernel");
-    }
+    SGN_REQUIRE(!total_dev || tile_bits <= 16, "sgn_bin_sort_capped: %d tiles leave no 16-bit key for the padding", tiles);
+    emit_keys_kernel<<<(N + 255) / 256, 256, 0, stream>>>(N, tiles_x, reinterpret_cast<const ushort4*>(tile_bbox), touch_mask, order, cum, (int)M,
+                                                          total_dev, (uint16_t)((1u << tile_bits) - 1u), keys_in, vals_in, big_ranks,
+                                                          big_count);
+    SGN_CHECK_LAUNCH("emit_keys_kernel");
+    int sms = 0, dev = 0;
+    SGN_CHECK_CUDA(cudaGetDevice(&dev));
+    SGN_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    emit_big_kernel<<<4 * sms, EMIT_BIG_THREADS, 0, stream>>>(tiles_x, cam->width, cam->height, bw, reinterpret_cast<const float4*>(records),
+                                                 reinterpret_cast<const ushort4*>(tile_bbox), order, cum, (int)M, big_ranks, big_count,
+                                                 keys_in, vals_in);
+    SGN_CHECK_LAUNCH("emit_big_kernel");
     size_t temp = L.temp_bytes;
     SGN_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(base + L.temp, temp, keys_in, keys_out, vals_in, sorted_ids, M, 0, tile_bits, stream));
     sgn_count_launch(1);
@@ -336,62 +454,102 @@ extern "C" int sgn_bin_sort_capped(int N, int64_t capacity, const int64_t* total
 // per-tile class sub-lists: stable partition of every tile's list into its object entries and its
 // background entries.  The objects-only / background-only accumulation renders of the reference
 // (get_submodel_output, scene graph :255-303,364-366) see exactly these entries in exactly this order.
-// Layout: class c (0 = background, 1 = object) owns cls_ids[c*M ...) and cls_bins[c][tiles][2].
-__global__ void __launch_bounds__(256)
-class_count_kernel(int tiles, const int2* __restrict__ tile_bins, const int32_t* __restrict__ sorted_ids,
-                   int32_t* __restrict__ counts /*[2][tiles]*/) {
-    const int tile = blockIdx.x;
-    const int2 range = tile_bins[tile];
-    int c = 0;
-    for (int k = range.x + threadIdx.x; k < range.y; k += blockDim.x) c += (sorted_ids[k] < 0) ? 1 : 0;
-    typedef cub::BlockReduce<int, 256> BR;
-    __shared__ typename BR::TempStorage tmp;
-    const int total = BR(tmp).Sum(c);
-    if (threadIdx.x == 0) {
-        counts[tiles + tile] = total;
-        counts[tile] = (range.y - range.x) - total;
-    }
+// Layout: class c (0 = background, 1 = object) owns cls_ids[c*M ...) and cls_bins[c][tiles][2]; class c of tile t starts
+// at the number of class-c entries in tiles 0..t-1 (also when the tile is empty).
+// One launch: a warp per tile, tiles taken in order through a ticket, so every tile a warp looks back at already belongs to a
+// running warp.  The warp counts its object entries with ballots, publishes the (background, object) pair, finds the sum over
+// the earlier tiles by decoupled look-back, then writes both sub-lists at ballot / popc positions.
+// Tile state: flag (bits 62-63: 0 = not yet, 1 = this tile's counts, 2 = inclusive over tiles 0..t) | background << 31 | object;
+// both counts are below 2^31.
+#define CLS_AGG 1ull
+#define CLS_INC 2ull
+#define CLS_CHUNK 16  // list entries per lane per step (loads in flight: a long tile list is one warp's serial chain)
+
+__device__ __forceinline__ unsigned long long cls_pack(unsigned long long flag, int bg, int obj) {
+    return (flag << 62) | ((unsigned long long)bg << 31) | (unsigned long long)obj;
 }
 
 __global__ void __launch_bounds__(256)
-class_compact_kernel(int tiles, int64_t M, const int2* __restrict__ tile_bins, const int32_t* __restrict__ sorted_ids,
-                     const int32_t* __restrict__ offsets /* exclusive scan over [2][tiles] */,
-                     const int32_t* __restrict__ counts, int32_t* __restrict__ cls_ids, int2* __restrict__ cls_bins) {
-    const int tile = blockIdx.x;
-    const int2 range = tile_bins[tile];
-    // offsets run over the concatenation [background tiles..., object tiles...]; class 1's base within its own
-    // array is offsets - (total background) = offsets - offsets[tiles]
-    const int base0 = offsets[tile];
-    const int base1 = offsets[tiles + tile] - offsets[tiles];
-    if (threadIdx.x == 0) {
-        cls_bins[tile] = make_int2(base0, base0 + counts[tile]);
-        cls_bins[tiles + tile] = make_int2(base1, base1 + counts[tiles + tile]);
-    }
-    typedef cub::BlockScan<int, 256> BS;
-    __shared__ typename BS::TempStorage tmp;
-    int run0 = 0, run1 = 0;
-    for (int k0 = range.x; k0 < range.y; k0 += blockDim.x) {
-        const int k = k0 + threadIdx.x;
-        const bool in = k < range.y;
-        const int id = in ? sorted_ids[k] : 0;
-        const int flag = (in && id < 0) ? 1 : 0;
-        int pos, total;
-        BS(tmp).ExclusiveSum(flag, pos, total);
-        if (in) {
-            if (flag) cls_ids[M + base1 + run1 + pos] = id;
-            else cls_ids[base0 + run0 + (threadIdx.x - pos)] = id;
+class_lists_kernel(int tiles, int64_t M, const int2* __restrict__ tile_bins, const int32_t* __restrict__ sorted_ids,
+                   unsigned long long* __restrict__ state, unsigned int* __restrict__ ticket, int32_t* __restrict__ cls_ids,
+                   int2* __restrict__ cls_bins) {
+    const int lane = threadIdx.x & 31;
+    int t = 0;
+    if (lane == 0) t = (int)atomicAdd(ticket, 1u);
+    t = __shfl_sync(0xffffffffu, t, 0);
+    if (t >= tiles) return;
+    const int2 range = tile_bins[t];
+    const unsigned lt = (1u << lane) - 1u;
+    int obj = 0;
+    for (int k0 = range.x; k0 < range.y; k0 += 32 * CLS_CHUNK) {
+        int32_t id[CLS_CHUNK];
+#pragma unroll
+        for (int j = 0; j < CLS_CHUNK; ++j) {
+            const int k = k0 + 32 * j + lane;
+            id[j] = k < range.y ? sorted_ids[k] : 0;
         }
-        run1 += total;
-        run0 += min((int)blockDim.x, range.y - k0) - total;
-        __syncthreads();
+#pragma unroll
+        for (int j = 0; j < CLS_CHUNK; ++j) obj += __popc(__ballot_sync(0xffffffffu, id[j] < 0));
+    }
+    const int bg = (range.y - range.x) - obj;
+    volatile unsigned long long* vs = state;
+    int bg0 = 0, obj0 = 0;  // exclusive prefix over tiles 0..t-1
+    if (t == 0) {
+        if (lane == 0) vs[0] = cls_pack(CLS_INC, bg, obj);
+    } else {
+        if (lane == 0) vs[t] = cls_pack(CLS_AGG, bg, obj);
+        // look back 32 tiles at a time: lane j reads tile w - j
+        for (int w = t - 1; ; w -= 32) {
+            unsigned long long s;
+            do {
+                s = w - lane >= 0 ? vs[w - lane] : cls_pack(CLS_INC, 0, 0);
+            } while (__any_sync(0xffffffffu, (s >> 62) == 0));
+            const unsigned inc = __ballot_sync(0xffffffffu, (s >> 62) == CLS_INC);
+            const int stop = inc ? __ffs(inc) - 1 : 31;  // the nearest inclusive value ends the look-back
+            int b = lane <= stop ? (int)((s >> 31) & 0x7fffffffu) : 0;
+            int o = lane <= stop ? (int)(s & 0x7fffffffu) : 0;
+#pragma unroll
+            for (int d = 16; d > 0; d >>= 1) {
+                b += __shfl_xor_sync(0xffffffffu, b, d);
+                o += __shfl_xor_sync(0xffffffffu, o, d);
+            }
+            bg0 += b;
+            obj0 += o;
+            if (inc) break;
+        }
+        if (lane == 0) vs[t] = cls_pack(CLS_INC, bg0 + bg, obj0 + obj);
+    }
+    if (lane == 0) {
+        cls_bins[t] = make_int2(bg0, bg0 + bg);
+        cls_bins[tiles + t] = make_int2(obj0, obj0 + obj);
+    }
+    int32_t* bg_out = cls_ids + bg0;
+    int32_t* obj_out = cls_ids + M + obj0;
+    for (int k0 = range.x; k0 < range.y; k0 += 32 * CLS_CHUNK) {
+        int32_t id[CLS_CHUNK];
+#pragma unroll
+        for (int j = 0; j < CLS_CHUNK; ++j) {
+            const int k = k0 + 32 * j + lane;
+            id[j] = k < range.y ? sorted_ids[k] : 0;
+        }
+#pragma unroll
+        for (int j = 0; j < CLS_CHUNK; ++j) {
+            const bool in = k0 + 32 * j + lane < range.y;
+            const unsigned ob = __ballot_sync(0xffffffffu, in && id[j] < 0);
+            const unsigned valid = __ballot_sync(0xffffffffu, in);
+            if (in) {
+                if (id[j] < 0) obj_out[__popc(ob & lt)] = id[j];
+                else bg_out[__popc(valid & ~ob & lt)] = id[j];
+            }
+            obj_out += __popc(ob);
+            bg_out += __popc(valid & ~ob);
+        }
     }
 }
 
+// tile state, then the ticket counter
 extern "C" size_t sgn_bin_class_scratch_bytes(int tiles) {
-    size_t temp = 0;
-    const int n = 2 * (tiles > 0 ? tiles : 1);
-    cub::DeviceScan::ExclusiveSum(nullptr, temp, (const int32_t*)nullptr, (int32_t*)nullptr, n);
-    return align_up(temp, 256) + 2 * align_up(sizeof(int32_t) * (size_t)n, 256);
+    return align_up(sizeof(unsigned long long) * (size_t)(tiles > 0 ? tiles : 1), 256) + 256;
 }
 
 extern "C" int sgn_bin_class_lists(const sgn_camera* cam, int64_t M, const int32_t* sorted_ids, const int32_t* tile_bins,
@@ -399,24 +557,21 @@ extern "C" int sgn_bin_class_lists(const sgn_camera* cam, int64_t M, const int32
     SGN_RANGE("sgn_bin_class_lists");
     cudaStream_t stream = (cudaStream_t)stream_;
     SGN_REQUIRE(cam && tile_bins && cls_ids && cls_bins && scratch, "sgn_bin_class_lists: null pointer");
+    SGN_REQUIRE(M >= 0 && M < ((int64_t)1 << 31), "sgn_bin_class_lists: M=%lld out of the int32 range", (long long)M);
     const int bw = cam->block_width;
     const int tiles = ((cam->width + bw - 1) / bw) * ((cam->height + bw - 1) / bw);
-    if (scratch_bytes < sgn_bin_class_scratch_bytes(tiles)) {
+    const size_t bytes = sgn_bin_class_scratch_bytes(tiles);
+    if (scratch_bytes < bytes) {
         sgn_set_error("sgn_bin_class_lists: scratch too small");
         return SGN_ERR_WORKSPACE;
     }
+    if (tiles == 0) return SGN_OK;
     char* base = (char*)scratch;
-    const size_t arr = align_up(sizeof(int32_t) * 2 * (size_t)tiles, 256);
-    int32_t* counts = (int32_t*)base;
-    int32_t* offsets = (int32_t*)(base + arr);
-    void* temp = base + 2 * arr;
-    size_t temp_bytes = scratch_bytes - 2 * arr;
-    class_count_kernel<<<tiles, 256, 0, stream>>>(tiles, reinterpret_cast<const int2*>(tile_bins), sorted_ids, counts);
-    SGN_CHECK_LAUNCH("class_count_kernel");
-    SGN_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(temp, temp_bytes, counts, offsets, 2 * tiles, stream));
-    sgn_count_launch(1);
-    class_compact_kernel<<<tiles, 256, 0, stream>>>(tiles, M, reinterpret_cast<const int2*>(tile_bins), sorted_ids, offsets, counts,
-                                                    cls_ids, reinterpret_cast<int2*>(cls_bins));
-    SGN_CHECK_LAUNCH("class_compact_kernel");
+    unsigned long long* state = (unsigned long long*)base;
+    unsigned int* ticket = (unsigned int*)(base + bytes - 256);
+    SGN_CHECK_CUDA(cudaMemsetAsync(scratch, 0, bytes, stream));
+    class_lists_kernel<<<(tiles + 7) / 8, 256, 0, stream>>>(tiles, M, reinterpret_cast<const int2*>(tile_bins), sorted_ids, state, ticket,
+                                                            cls_ids, reinterpret_cast<int2*>(cls_bins));
+    SGN_CHECK_LAUNCH("class_lists_kernel");
     return SGN_OK;
 }
