@@ -974,17 +974,47 @@ struct BlendBwdParams {
     const float* fixed_scale;  // device scalar: fixed-point units per unit of gradient
 };
 
+// Deterministic mode: how many binary places the fixed-point grid of record component idx (= row * 12 + component) gives
+// up, from the Gaussian's own record.  A conic gradient is a sum of 1/2 dx^2 v_sigma (dx dy, 1/2 dy^2) over the pixels the
+// Gaussian covers, which grows like o sigma^4 -- about pi/4 E^2 per unit of v_alpha with E = trace of the 2D covariance in
+// px^2 (the support ellipse holds ~2 pi sigma^2 pixels).  At sigma = 200 px that is ~4e9, twice the 2^31 units of headroom
+// of the grid; the conic components of a Gaussian with E > 2^13 (sigma above ~64 px) are therefore accumulated 2^-(2 ceil(log2
+// E) - 26) coarser, which keeps their sums below ~2^26 units per unit of v_alpha.  Smaller Gaussians keep the full grid.
+// Exact double operations on the record's floats: the same value wherever it is computed (accumulate_grad and
+// fixed_to_float_kernel).
+__device__ __forceinline__ int fixed_shift(const float* __restrict__ records, size_t idx) {
+    const int comp = (int)(idx % SGN_RECORD_FLOATS);
+    if (comp < 2 || comp > 4) return 0;
+    const float* r = records + (idx - comp);
+    const double a = __ldg(r + 2), b = __ldg(r + 3), c = __ldg(r + 4);
+    const double det = __dsub_rn(__dmul_rn(a, c), __dmul_rn(b, b));
+    if (!(det > 0.0)) return 0;  // not positive definite (or NaN): such an entry is valid for no pixel or a few
+    const double E = __ddiv_rn(__dadd_rn(a, c), det);
+    if (!(E > 0.0)) return 0;
+    int e;
+    frexp(fmin(E, 1e18), &e);  // E < 2^e
+    return min(max(2 * e - 26, 0), 100);
+}
+
 // Per-Gaussian gradient accumulation.  Default: float RED (summation order varies from run to run).  Deterministic mode
 // (sgn_blend_bwd_in.v_fixed): the addend is rounded ONCE to 64-bit fixed point and added as an integer -- integer addition
 // is associative, so the total is bit-identical whatever order the tiles and strips arrive in.
+// DET is a template parameter of the backward kernels: the float path's instantiations carry no fixed-point code (with the
+// shift computation behind a run-time branch, blend_bwd took 0.85 instead of 0.75 ms at config 3).
+template <bool DET>
 __device__ __forceinline__ void accumulate_grad(const BlendBwdParams& p, float fscale, size_t idx, float v) {
-    if (p.v_fixed) atomicAdd(reinterpret_cast<unsigned long long*>(p.v_fixed) + idx, (unsigned long long)__float2ll_rn(v * fscale));
-    else atomicAdd(p.v_records + idx, v);
+    if constexpr (DET) {
+        const int sh = fixed_shift(reinterpret_cast<const float*>(p.records), idx);
+        const float m = v * fscale * __int_as_float((127 - sh) << 23);  // times 2^-sh: exact
+        atomicAdd(reinterpret_cast<unsigned long long*>(p.v_fixed) + idx, (unsigned long long)__float2ll_rn(m));
+    } else {
+        atomicAdd(p.v_records + idx, v);
+    }
 }
 
 // backward of the accumulation-only pass: out = 1 - T_final  =>  v_alpha_k = T_final * ra_k * v_out.  Walks the class
 // sub-list positions [range.x, range.y) back to front; tfv = T_final * v_out and idx (a sub-list position) per pixel.
-template <int PPL, bool SKIP>
+template <int PPL, bool SKIP, bool DET>
 __device__ __forceinline__ void acc_bwd_traverse(const BlendBwdParams& p, const int32_t* __restrict__ ids, int tile, int strip,
                                                  const int2 range, const float (&tfv)[PPL], const int (&idx)[PPL],
                                                  float4 (*sA)[32], float4 (*sB)[32], float (*sR)[32]) {
@@ -996,7 +1026,7 @@ __device__ __forceinline__ void acc_bwd_traverse(const BlendBwdParams& p, const 
     const float px = (float)j + 0.5f, py0 = (float)i0 + 0.5f;
     const int my_comp = multi_reduce_slot<6>(lane);
     const float clampb = in_register(p.clamp_bwd), nclamp = -clampb;
-    const float fscale = p.v_fixed ? __ldg(p.fixed_scale) : 0.f;
+    const float fscale = DET ? __ldg(p.fixed_scale) : 0.f;
     Staged nxt;
     if (range.y - 1 - lane >= range.x) nxt = gather_entry(p.records, ids[range.y - 1 - lane]);
     int buf = 0;
@@ -1064,7 +1094,7 @@ __device__ __forceinline__ void acc_bwd_traverse(const BlendBwdParams& p, const 
             float l5 = -S0 / o;
             float comps[6] = {l0, l1, l2, l3, l4, l5};
             const float mine = warp_multi_reduce<6>(comps, lane);
-            if (my_comp >= 0) accumulate_grad(p, fscale, (size_t)(__float_as_int(B.z) & ID_MASK) * SGN_RECORD_FLOATS + my_comp, mine);
+            if (my_comp >= 0) accumulate_grad<DET>(p, fscale, (size_t)(__float_as_int(B.z) & ID_MASK) * SGN_RECORD_FLOATS + my_comp, mine);
         }
         buf ^= 1;
     }
@@ -1074,7 +1104,7 @@ __device__ __forceinline__ void acc_bwd_traverse(const BlendBwdParams& p, const 
 // (see below).
 // (Measured and dropped: software-pipelining the reduction of entry t-1 under the arithmetic of entry t -- it
 // has to run unconditionally, which costs more than the overlap gains: 0.87 vs 0.82 ms on cfg3.)
-template <int PPL, bool DEPTHG, bool PACK, bool OBJ>
+template <int PPL, bool DEPTHG, bool PACK, bool OBJ, bool DET>
 __device__ __forceinline__ void blend_bwd_strip(const BlendBwdParams& p, int tile, int strip, const int2 range,
                                                 float4 (*sA)[32], float4 (*sB)[32], float4 (*sC)[32]) {
     const int tx = tile % p.tiles_x, ty = tile / p.tiles_x;
@@ -1174,7 +1204,7 @@ __device__ __forceinline__ void blend_bwd_strip(const BlendBwdParams& p, int til
     constexpr int NV = DEPTHG ? 10 : 9;
     const int my_comp = multi_reduce_slot<NV>(lane);
     const float clampb = in_register(p.clamp_bwd), nclamp = -clampb;
-    const float fscale = p.v_fixed ? __ldg(p.fixed_scale) : 0.f;
+    const float fscale = DET ? __ldg(p.fixed_scale) : 0.f;
     constexpr bool PK = PACK && PPL >= 2;
     constexpr int NP = PK ? PPL / 2 : 1;
     f2 T2[NP], d2[NP], vr2[NP], vg2[NP], vb2[NP], vd2[NP];
@@ -1318,7 +1348,7 @@ __device__ __forceinline__ void blend_bwd_strip(const BlendBwdParams& p, int til
             if (DEPTHG) comps[NV - 1] = cd;
             const size_t dst = (size_t)(__float_as_int(Cc.z) & ID_MASK) * SGN_RECORD_FLOATS + (my_comp >= 0 ? my_comp : 0);
             const float mine = warp_multi_reduce<NV>(comps, lane);
-            if (my_comp >= 0) accumulate_grad(p, fscale, dst, mine);
+            if (my_comp >= 0) accumulate_grad<DET>(p, fscale, dst, mine);
         }
         buf ^= 1;
     }
@@ -1326,7 +1356,7 @@ __device__ __forceinline__ void blend_bwd_strip(const BlendBwdParams& p, int til
         const int ohi = min(p.cls_bins[1][tile].y, warp_max(kmaxo) + 1);
         if (ohi > orest) {
             __syncwarp();  // every lane has finished reading the staging ring
-            acc_bwd_traverse<PPL, true>(p, p.cls_ids[1], tile, strip, make_int2(orest, ohi), tfo, idxo, sA, sB,
+            acc_bwd_traverse<PPL, true, DET>(p, p.cls_ids[1], tile, strip, make_int2(orest, ohi), tfo, idxo, sA, sB,
                                         reinterpret_cast<float(*)[32]>(&sC[0][0]));
         }
     }
@@ -1335,7 +1365,7 @@ __device__ __forceinline__ void blend_bwd_strip(const BlendBwdParams& p, int til
 // the prologue (v_sky, cotangent chain) must run for every pixel, so strips are always launched for the
 // whole tile: W strips of 16/W rows.  OBJ: the strips are sized from the main depth plus how far the objects-only
 // streams run past it (tile_depth[object], see blend_fwd_strip).
-template <bool DEPTHG, bool PACK, bool OBJ>
+template <bool DEPTHG, bool PACK, bool OBJ, bool DET>
 __global__ void __launch_bounds__(32, BLEND_BWD_MIN_BLOCKS) blend_bwd_kernel(const BlendBwdParams p) {
     __shared__ float4 sA[2][32];
     __shared__ float4 sB[2][32];
@@ -1346,15 +1376,15 @@ __global__ void __launch_bounds__(32, BLEND_BWD_MIN_BLOCKS) blend_bwd_kernel(con
     const int W = strips_for(p.tile_depth[tile] + (OBJ ? p.tile_depth[(size_t)SLOT_OBJ * p.tiles + tile] : 0), p.split_main);
     if (strip >= W) return;
     switch (W) {
-        case 1: blend_bwd_strip<8, DEPTHG, PACK, OBJ>(p, tile, strip, range, sA, sB, sC); break;
-        case 2: blend_bwd_strip<4, DEPTHG, PACK, OBJ>(p, tile, strip, range, sA, sB, sC); break;
-        case 4: blend_bwd_strip<2, DEPTHG, PACK, OBJ>(p, tile, strip, range, sA, sB, sC); break;
-        default: blend_bwd_strip<1, DEPTHG, PACK, OBJ>(p, tile, strip, range, sA, sB, sC); break;
+        case 1: blend_bwd_strip<8, DEPTHG, PACK, OBJ, DET>(p, tile, strip, range, sA, sB, sC); break;
+        case 2: blend_bwd_strip<4, DEPTHG, PACK, OBJ, DET>(p, tile, strip, range, sA, sB, sC); break;
+        case 4: blend_bwd_strip<2, DEPTHG, PACK, OBJ, DET>(p, tile, strip, range, sA, sB, sC); break;
+        default: blend_bwd_strip<1, DEPTHG, PACK, OBJ, DET>(p, tile, strip, range, sA, sB, sC); break;
     }
 }
 
 // the background-only accumulation's backward (the objects-only one is part of blend_bwd_kernel)
-template <int PPL, bool SKIP>
+template <int PPL, bool SKIP, bool DET>
 __device__ __forceinline__ void acc_bwd_strip(const BlendBwdParams& p, int cls, int tile, int strip, const int2 range,
                                               float4 (*sA)[32], float4 (*sB)[32], float (*sR)[32]) {
     const int slot = cls ? SLOT_OBJ : SLOT_BG;
@@ -1381,10 +1411,10 @@ __device__ __forceinline__ void acc_bwd_strip(const BlendBwdParams& p, int cls, 
     const int wkmax = warp_max(kmax);
     const int hi0 = min(range.y, wkmax + 1);
     if (hi0 <= range.x) return;
-    acc_bwd_traverse<PPL, SKIP>(p, p.cls_ids[cls], tile, strip, make_int2(range.x, hi0), tfv, idx, sA, sB, sR);
+    acc_bwd_traverse<PPL, SKIP, DET>(p, p.cls_ids[cls], tile, strip, make_int2(range.x, hi0), tfv, idx, sA, sB, sR);
 }
 
-template <bool SKIP>
+template <bool SKIP, bool DET>
 __global__ void __launch_bounds__(32, BLEND_ACC_MIN_BLOCKS) acc_bwd_kernel(const BlendBwdParams p, const int cls) {
     __shared__ float4 sA[2][32];
     __shared__ float4 sB[2][32];
@@ -1395,15 +1425,16 @@ __global__ void __launch_bounds__(32, BLEND_ACC_MIN_BLOCKS) acc_bwd_kernel(const
     const int W = strips_for(p.tile_depth[(size_t)(cls ? SLOT_OBJ : SLOT_BG) * p.tiles + tile], p.split_acc);
     if (strip >= W) return;
     switch (W) {
-        case 1: acc_bwd_strip<8, SKIP>(p, cls, tile, strip, range, sA, sB, sR); break;
-        case 2: acc_bwd_strip<4, SKIP>(p, cls, tile, strip, range, sA, sB, sR); break;
-        case 4: acc_bwd_strip<2, SKIP>(p, cls, tile, strip, range, sA, sB, sR); break;
-        default: acc_bwd_strip<1, SKIP>(p, cls, tile, strip, range, sA, sB, sR); break;
+        case 1: acc_bwd_strip<8, SKIP, DET>(p, cls, tile, strip, range, sA, sB, sR); break;
+        case 2: acc_bwd_strip<4, SKIP, DET>(p, cls, tile, strip, range, sA, sB, sR); break;
+        case 4: acc_bwd_strip<2, SKIP, DET>(p, cls, tile, strip, range, sA, sB, sR); break;
+        default: acc_bwd_strip<1, SKIP, DET>(p, cls, tile, strip, range, sA, sB, sR); break;
     }
 }
 
 // ---- deterministic mode helpers: scale = 2^32 / max |cotangent| (gradients are linear in the cotangents: the fixed-point
-// grid adapts to their magnitude; 2^31 of headroom above it), then fixed point -> float
+// grid adapts to their magnitude; 2^31 of headroom above it, and the conic components of large Gaussians give up more
+// places, fixed_shift), then fixed point -> float
 __global__ void __launch_bounds__(256)
 cot_max_kernel(const float* __restrict__ a, long long n, unsigned* __restrict__ out_bits) {
     float m = 0.f;
@@ -1420,9 +1451,34 @@ __global__ void fixed_scale_kernel(float* scale) {
     scale[0] = m > 0.f ? exp2f(32.f - ceilf(log2f(m))) : 4294967296.f;  // a power of two: scaling is exact
 }
 __global__ void __launch_bounds__(256)
-fixed_to_float_kernel(const long long* __restrict__ fx, const float* __restrict__ scale, float* __restrict__ out, long long n) {
+fixed_to_float_kernel(const long long* __restrict__ fx, const float* __restrict__ scale, const float* __restrict__ records,
+                      float* __restrict__ out, long long n) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = (float)((double)fx[i] / (double)scale[0]);
+    if (i < n) out[i] = (float)(ldexp((double)fx[i], fixed_shift(records, (size_t)i)) / (double)scale[0]);
+}
+
+template <bool DET>
+static int launch_blend_bwd(const BlendBwdParams& p, int tuning, cudaStream_t side, cudaStream_t stream) {
+    const unsigned acc_grid = p.tiles * 8;
+    if (p.v_bg) {
+        if (!(tuning & SGN_TUNE_ACC_NO_ROW_SKIP)) acc_bwd_kernel<true, DET><<<acc_grid, 32, 0, side>>>(p, 0);
+        else acc_bwd_kernel<false, DET><<<acc_grid, 32, 0, side>>>(p, 0);
+        SGN_CHECK_LAUNCH("acc_bwd_kernel<background>");
+    }
+    const bool pack = (tuning & SGN_TUNE_BWD_PACKED) != 0;
+    const dim3 grid(p.tiles * 8), block(32);
+    switch ((p.v_obj ? 4 : 0) | (p.v_depth ? 2 : 0) | (pack ? 1 : 0)) {
+        case 0: blend_bwd_kernel<false, false, false, DET><<<grid, block, 0, stream>>>(p); break;
+        case 1: blend_bwd_kernel<false, true, false, DET><<<grid, block, 0, stream>>>(p); break;
+        case 2: blend_bwd_kernel<true, false, false, DET><<<grid, block, 0, stream>>>(p); break;
+        case 3: blend_bwd_kernel<true, true, false, DET><<<grid, block, 0, stream>>>(p); break;
+        case 4: blend_bwd_kernel<false, false, true, DET><<<grid, block, 0, stream>>>(p); break;
+        case 5: blend_bwd_kernel<false, true, true, DET><<<grid, block, 0, stream>>>(p); break;
+        case 6: blend_bwd_kernel<true, false, true, DET><<<grid, block, 0, stream>>>(p); break;
+        default: blend_bwd_kernel<true, true, true, DET><<<grid, block, 0, stream>>>(p); break;
+    }
+    SGN_CHECK_LAUNCH("blend_bwd_kernel");
+    return SGN_OK;
 }
 
 extern "C" int sgn_blend_bwd(const sgn_camera* cam, const sgn_blend_opts* opts, const float* records,
@@ -1487,33 +1543,15 @@ extern "C" int sgn_blend_bwd(const sgn_camera* cam, const sgn_blend_opts* opts, 
     {
         // all three kernels only accumulate (RED) into v_records: they may run concurrently
         ForkJoin fj(stream);
-        const bool acc_skip = !(opts->tuning & SGN_TUNE_ACC_NO_ROW_SKIP);
-        const unsigned acc_grid = tiles * 8;
-        if (in->v_background_acc) {
-            if (acc_skip) acc_bwd_kernel<true><<<acc_grid, 32, 0, fj.side()>>>(p, 0);
-            else acc_bwd_kernel<false><<<acc_grid, 32, 0, fj.side()>>>(p, 0);
-            SGN_CHECK_LAUNCH("acc_bwd_kernel<background>");
-        }
-
-        const bool pack = (opts->tuning & SGN_TUNE_BWD_PACKED) != 0;
-        const dim3 grid(tiles * 8), block(32);
-        switch ((in->v_object_acc ? 4 : 0) | (in->v_depth ? 2 : 0) | (pack ? 1 : 0)) {
-            case 0: blend_bwd_kernel<false, false, false><<<grid, block, 0, stream>>>(p); break;
-            case 1: blend_bwd_kernel<false, true, false><<<grid, block, 0, stream>>>(p); break;
-            case 2: blend_bwd_kernel<true, false, false><<<grid, block, 0, stream>>>(p); break;
-            case 3: blend_bwd_kernel<true, true, false><<<grid, block, 0, stream>>>(p); break;
-            case 4: blend_bwd_kernel<false, false, true><<<grid, block, 0, stream>>>(p); break;
-            case 5: blend_bwd_kernel<false, true, true><<<grid, block, 0, stream>>>(p); break;
-            case 6: blend_bwd_kernel<true, false, true><<<grid, block, 0, stream>>>(p); break;
-            default: blend_bwd_kernel<true, true, true><<<grid, block, 0, stream>>>(p); break;
-        }
-        SGN_CHECK_LAUNCH("blend_bwd_kernel");
+        const int rc = in->v_fixed ? launch_blend_bwd<true>(p, opts->tuning, fj.side(), stream)
+                                   : launch_blend_bwd<false>(p, opts->tuning, fj.side(), stream);
         fj.finish();
+        if (rc) return rc;
     }
     if (in->v_fixed) {
         const long long n = (long long)in->num_gaussians * SGN_RECORD_FLOATS;
         fixed_to_float_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const long long*>(in->v_fixed), in->fixed_scale,
-                                                                                v_records, n);
+                                                                                records, v_records, n);
         SGN_CHECK_LAUNCH("fixed_to_float_kernel");
     }
     return SGN_OK;

@@ -471,7 +471,8 @@ def blend_opts(s: RenderSettings, has_sky: bool) -> _lib.BlendOpts:
     bo.split_fwd_acc = int(os.environ.get("SGN_SPLIT_FWD_ACC", "0"))
     bo.split_bwd_main = int(os.environ.get("SGN_SPLIT_BWD_MAIN", "0"))
     bo.split_bwd_acc = int(os.environ.get("SGN_SPLIT_BWD_ACC", "0"))
-    # SGN_TUNE_* bits (include/sgn_raster.h): 1 fwd row skip, 2 bwd row skip, 4 fwd paired row slots, 8 bwd paired row slots, 32 fwd TMA staging
+    # SGN_TUNE_* bits (include/sgn_raster.h): 1 fwd row skip, 4 fwd paired row slots, 8 bwd paired row slots, 16 no row skip in the
+    # accumulation-only kernels, 32 fwd TMA staging
     bo.tuning = int(os.environ.get("SGN_TUNING", str(DEFAULT_TUNING)))
     return bo
 
