@@ -326,6 +326,17 @@ int sgn_loss_fwd(int H, int W, const sgn_loss_in* in, float* losses, void* scrat
 int sgn_loss_bwd(int H, int W, const sgn_loss_in* in, const float* grad_losses, float* v_rgb, float* v_accumulation,
                  float* v_object_acc, void* stream);
 
+/* SSIM term (sgn_splatfacto.py:1085-1087): weight * (1 - SSIM(gt*mask, rgb*mask)) with pytorch_msssim.SSIM(data_range=1,
+ * size_average=True, channel=3): 11-tap Gaussian window (sigma 1.5), valid padding, mean of the (H-10) x (W-10) x 3 map.
+ * The forward stores three derivative maps (36 B per valid pixel) in the caller's workspace for the backward.  H or W < 11,
+ * a null rgb / gt, both gt pointers, or a short workspace return an error and launch nothing. */
+size_t sgn_ssim_workspace_bytes(int H, int W);
+/* *loss (device) = weight * (1 - SSIM(gt*mask, rgb*mask)); uses in->rgb, in->gt_u8 | in->gt_f32, in->mask only */
+int sgn_ssim_fwd(int H, int W, const sgn_loss_in* in, float weight, float* loss, void* workspace, size_t workspace_bytes, void* stream);
+/* v_rgb [H,W,3] = d(grad_loss * loss)/d rgb, from the workspace sgn_ssim_fwd filled (grad_loss: device scalar; NULL = 1) */
+int sgn_ssim_bwd(int H, int W, const sgn_loss_in* in, float weight, const float* grad_loss, const void* workspace, float* v_rgb,
+                 void* stream);
+
 /* ---- densification statistics (SURVEY.md 8f rank 3) -------------------------------------------------------
  * What each sub-model's `after_train` accumulates after backward (sgn_splatfacto.py:513-541), for all visible
  * sub-models of the frame in one launch: grads = ||v_records[:,0:2]||; on a sub-model's first call

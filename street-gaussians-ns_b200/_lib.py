@@ -127,7 +127,8 @@ EXPORTS = [
     "sgn_upload", "sgn_bin_count", "sgn_project_fwd", "sgn_project_bwd", "sgn_l1_project_fwd", "sgn_l1_project_bwd", "sgn_l1_sh", "sgn_bin_scan_scratch_bytes", "sgn_bin_scan",
     "sgn_bin_sort_scratch_bytes", "sgn_bin_sort", "sgn_bin_class_scratch_bytes", "sgn_bin_class_lists", "sgn_blend_sched_ints",
     "sgn_blend_fwd", "sgn_blend_bwd", "sgn_sizeof_adam_tensor", "sgn_adam_chunk_elems", "sgn_adam_step",
-    "sgn_loss_scratch_bytes", "sgn_loss_fwd", "sgn_loss_bwd", "sgn_sizeof_densify_segment", "sgn_densify_stats",
+    "sgn_loss_scratch_bytes", "sgn_loss_fwd", "sgn_loss_bwd", "sgn_ssim_workspace_bytes", "sgn_ssim_fwd", "sgn_ssim_bwd",
+    "sgn_sizeof_densify_segment", "sgn_densify_stats",
     "sgn_sizeof_refine_config", "sgn_sizeof_refine_tensors", "sgn_refine_decide", "sgn_refine_apply",
     "sgn_bin_local_cap", "sgn_bin_local_scratch_bytes", "sgn_bin_local_count", "sgn_bin_local_sort",
     "sgn_project_bwd_range", "sgn_allreduce_sym", "sgn_blend_extra_fwd", "sgn_blend_extra_bwd",
@@ -209,6 +210,11 @@ def load():
     L.sgn_loss_fwd.restype = C.c_int
     L.sgn_loss_bwd.argtypes = [i32, i32, C.POINTER(LossIn), vp, vp, vp, vp, vp]
     L.sgn_loss_bwd.restype = C.c_int
+    L.sgn_ssim_workspace_bytes.argtypes = [i32, i32]
+    L.sgn_ssim_workspace_bytes.restype = sz
+    L.sgn_ssim_fwd.argtypes = [i32, i32, C.POINTER(LossIn), fl, vp, vp, sz, vp]
+    L.sgn_ssim_bwd.argtypes = [i32, i32, C.POINTER(LossIn), fl, vp, vp, vp, vp]
+    L.sgn_ssim_fwd.restype = L.sgn_ssim_bwd.restype = C.c_int
     L.sgn_sizeof_adam_tensor.restype = sz
     L.sgn_adam_chunk_elems.restype = C.c_int
     L.sgn_adam_step.argtypes = [vp, i32, i32, vp, vp, vp, vp]

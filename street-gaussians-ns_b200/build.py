@@ -23,6 +23,7 @@ SOURCES = {
     "binning_local.cu": [],
     "blend.cu": ["--use_fast_math"],
     "loss.cu": [],
+    "ssim.cu": [],  # IEEE divisions (no fast math); contraction allowed
     "densify.cu": ["--fmad=false"],
     "adam.cu": ["--fmad=false"],  # keep torch.optim.Adam's rounding sequence (no contraction)
     "refine.cu": ["--fmad=false"],

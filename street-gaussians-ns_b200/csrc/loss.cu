@@ -2,8 +2,8 @@
 // the rasterizer's outputs straight after the render -- L1 (street_gaussians_ns/sgn_splatfacto.py:1079-1084),
 // sky accumulation (:1090-1093) and the object-accumulation entropy (sgn_splatfacto_scene_graph.py:386-389) --
 // and their cotangents, in two HBM-bound passes (forward sums, backward cotangents) instead of ~25 torch
-// elementwise / reduction launches.  SSIM stays in torch.  The ground truth may be the uint8 image the data
-// loader holds (gt = u8 / 255, as the reference's `.float() / 255`).
+// elementwise / reduction launches.  The SSIM term (:1085-1087) has its own kernels (ssim.cu).  The ground truth may be the
+// uint8 image the data loader holds (gt = u8 / 255, as the reference's `.float() / 255`).
 //
 // Arithmetic follows torch: |a - b|, clamp(x, 1e-5, 1 - 1e-5) with pass-through gradient inside the closed
 // interval, natural log, means as sum / count (fp32 sums of per-block partials, summed in a fixed order: the

@@ -1,7 +1,8 @@
 """Fused loss epilogue (SURVEY.md 8f rank 2): the image-space terms of the reference's ``get_loss_dict``
 (street_gaussians_ns/sgn_splatfacto.py:1042-1094, sgn_splatfacto_scene_graph.py:376-391) that re-read the
 rasterizer's outputs -- L1, sky accumulation, object-accumulation entropy -- as two HBM-bound kernels of
-libsgn_raster.so (forward sums, backward cotangents) behind one autograd node.  SSIM stays in torch."""
+libsgn_raster.so (forward sums, backward cotangents) behind one autograd node; and the SSIM term
+(sgn_splatfacto.py:1085-1087) as its own forward / backward pair (csrc/ssim.cu) behind a second one."""
 from __future__ import annotations
 
 import ctypes as C
@@ -86,3 +87,38 @@ def fused_image_losses(rgb: torch.Tensor, gt: torch.Tensor, accumulation: Option
     """Returns (Ll1, sky_accumulation, object_acc_entropy) 0-d tensors, already weighted; terms without
     inputs / with zero weight are exact zeros with no gradient.  ``gt`` may be float32 or uint8 (gt/255)."""
     return _FusedImageLosses.apply(rgb, accumulation, object_acc, gt, mask, sky_mask, float(w_l1), float(w_sky), float(w_entropy))
+
+
+class _FusedSSIM(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, rgb, gt, mask, weight: float):
+        L = _lib.load()
+        if not rgb.is_cuda:
+            raise _lib.SgnError("the fused SSIM term has no CPU path")
+        H, W = rgb.shape[0], rgb.shape[1]
+        li, keep = _loss_in(rgb, gt, mask, None, None, None, (0.0, 0.0, 0.0))
+        loss = torch.empty((), device=rgb.device, dtype=torch.float32)
+        wb = L.sgn_ssim_workspace_bytes(H, W)
+        ws = torch.empty(max(wb, 1), device=rgb.device, dtype=torch.uint8)  # the derivative maps the backward reads
+        _lib.check(L.sgn_ssim_fwd(H, W, C.byref(li), weight, _ptr(loss), _ptr(ws), wb, _stream()), "sgn_ssim_fwd")
+        ctx.li, ctx.keep, ctx.ws, ctx.shape, ctx.weight = li, keep, ws, (H, W), weight
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        L = _lib.load()
+        H, W = ctx.shape
+        g = g.reshape(()).float().contiguous()
+        v_rgb = torch.empty(H, W, 3, device=ctx.ws.device)
+        _lib.check(L.sgn_ssim_bwd(H, W, C.byref(ctx.li), ctx.weight, _ptr(g), _ptr(ctx.ws), _ptr(v_rgb), _stream()), "sgn_ssim_bwd")
+        return v_rgb, None, None, None
+
+
+def fused_ssim_loss(rgb: torch.Tensor, gt: torch.Tensor, mask: Optional[torch.Tensor] = None, weight: float = 1.0) -> torch.Tensor:
+    """``weight * (1 - SSIM(gt * mask, rgb * mask))`` as a 0-d tensor: pytorch_msssim.SSIM(data_range=1, size_average=True,
+    channel=3) as the reference applies it (sgn_splatfacto.py:1081-1087).  ``rgb`` is [H,W,3] float32, ``gt`` [H,W,3] float32
+    or uint8 (gt/255), ``mask`` [H,W,1] or None; H and W must be at least 11.  The gradient flows to ``rgb`` only.  With
+    ``weight == 0`` the result is an exact zero and nothing is launched."""
+    if float(weight) == 0.0:
+        return torch.zeros((), device=rgb.device)
+    return _FusedSSIM.apply(rgb, gt, mask, float(weight))

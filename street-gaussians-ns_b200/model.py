@@ -57,7 +57,7 @@ class SceneGraphConfig:
     alpha_clamp_fwd: float = 0.999
     alpha_clamp_bwd: float = 0.99
     render_background_acc: bool = True
-    fused_loss: bool = True  # L1 / sky / entropy terms through the fused loss epilogue (loss.py) instead of torch ops
+    fused_loss: bool = True  # L1 / sky / entropy and SSIM terms through the loss kernels (loss.py) instead of torch ops
     # refinement (sgn_splatfacto.py:550-646): the sub-model configs of sgn_config.py:46-66 (background / object template)
     refine: RefineSettings = field(default_factory=lambda: RefineSettings(cull_alpha_thresh=0.02))
     object_refine: RefineSettings = field(default_factory=lambda: RefineSettings(cull_alpha_thresh=0.005))
@@ -748,7 +748,11 @@ class SceneGraphRasterModel(torch.nn.Module):
         else:
             gt_img, rgb = float_pair()
             losses["Ll1"] = (1 - c.ssim_lambda) * torch.abs(gt_img - rgb).mean()
-        if c.ssim_lambda > 0:
+        if c.ssim_lambda > 0 and fused:
+            # SSIM forward + backward kernels (loss.py, csrc/ssim.cu); a uint8 image is read as it is
+            from .loss import fused_ssim_loss
+            losses["simloss"] = fused_ssim_loss(outputs["rgb"], batch["image"], mask=batch.get("mask"), weight=c.ssim_lambda)
+        elif c.ssim_lambda > 0:
             gt_img, rgb = float_pair()
             simloss = 1 - ssim(gt_img.permute(2, 0, 1)[None, ...], rgb.permute(2, 0, 1)[None, ...])
             losses["simloss"] = c.ssim_lambda * simloss

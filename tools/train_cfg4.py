@@ -25,7 +25,7 @@ sys.path.insert(0, ROOT)
 
 def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int = 100, start_step: int = 600,
         actor_range: float = 45.0, pipeline_chunks: int = 0, overlap: bool = False, resident_table: bool = True,
-        async_binning: bool = True) -> dict:
+        async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True) -> dict:
     """One measurement.  torch.distributed must already be initialised when WORLD_SIZE > 1.  Returns the result dict on
     rank 0 (None elsewhere)."""
     import torch
@@ -52,7 +52,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         return [ActorPose(str(a), rot, center, f, frame_list) for a, rot, center in sc.boxes_at(f)]
 
     rs = RefineSettings(refine_every=refine_every)
-    cfg = SceneGraphConfig(use_sky_sphere=False, ssim_lambda=0.0, full_gradient_arena=world > 1, refine=rs, async_binning=async_binning,
+    cfg = SceneGraphConfig(use_sky_sphere=False, ssim_lambda=ssim_lambda, fused_loss=fused_loss, full_gradient_arena=world > 1, refine=rs, async_binning=async_binning,
                            object_refine=RefineSettings(refine_every=refine_every, cull_alpha_thresh=0.005),
                            num_train_data=len(cams), refine_record=True)
     model = SceneGraphRasterModel(sc.background.to(dev), {k: v.to(dev) for k, v in sc.actors.items()}, cfg, poses_at=poses_at).to(dev)
@@ -157,13 +157,14 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     counts1 = [sub.num_points for sub in model.all_models.values()]
     ms = float(dev_ms[0].item())
     return {
-        "metric": "training steps/s (render 1 camera per rank + L1 + backward + gradient all-reduce + fused Adam + densification "
+        "metric": f"training steps/s (render 1 camera per rank + L1{' + SSIM' if ssim_lambda > 0 else ''} + backward + gradient all-reduce + fused Adam + densification "
                   f"statistics, refinement every {refine_every} steps; timed steps {start_step + warmup}..{start_step + warmup + steps - 1})", "value": world / (ms * 1e-3), "unit": "steps/s",
         "n_gpus": world, "steps": steps, "warmup": warmup, "ms_per_step": ms, "wall_ms_per_step": float(dev_ms[1].item()),
         "higher_is_better": True, "scaling": "weak", "dtype": "f32", "data": "synthetic",
         "config": {"workload": f"cfg{4 if world == 1 else 5}: 5 cameras x 85 frames, {sc.n_bg} background + 32 x {sc.n_act} actor Gaussians, "
                                f"{W}x{H}; rank r renders camera (step*g + r) mod 425; actors have a box within {actor_range} m of the ego vehicle",
-                   "parallelism": f"camera-sharded dp{world}", "start_step": start_step, "refine_every": refine_every,
+                   "parallelism": f"camera-sharded dp{world}", "ssim_lambda": ssim_lambda,
+                   "loss": "fused kernels" if fused_loss else "torch ops", "start_step": start_step, "refine_every": refine_every,
                    "refinement_kernels_loaded_before_timing": refine_warm,
                    "binning": "no host read-back of the intersection count" if async_binning else "one read-back per frame",
                    "segment_table": "device-resident (staged up front; re-staged per timestamp on first use after a refinement)" if resident_table else "host build per frame",
@@ -187,6 +188,8 @@ def main():
     ap.add_argument("--pipeline-chunks", type=int, default=0, help="> 0: all-reduce and Adam pipelined over that many arena ranges")
     ap.add_argument("--overlap", action="store_true", help="all-reduce launched per arena range from project_bwd's ranges (dp.OverlappedStep)")
     ap.add_argument("--host-table", action="store_true", help="build the segment table on the host per frame instead of prepare_frames")
+    ap.add_argument("--ssim-lambda", type=float, default=0.0, help="weight of the SSIM term (the reference trains with 0.2)")
+    ap.add_argument("--torch-loss", action="store_true", help="loss terms as torch ops (SceneGraphConfig.fused_loss = False)")
     args = ap.parse_args()
 
     import torch
@@ -198,7 +201,7 @@ def main():
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     res = run(args.steps, args.warmup, args.scale, args.refine_every, args.start_step, args.actor_range, args.pipeline_chunks,
-              args.overlap, not args.host_table)
+              args.overlap, not args.host_table, ssim_lambda=args.ssim_lambda, fused_loss=not args.torch_loss)
     if res is not None:
         print(json.dumps(res))
     if world > 1:
