@@ -355,9 +355,9 @@ extern "C" int sgn_project_fwd(const sgn_segment* segs_dev, int nseg, int N, int
     SGN_REQUIRE(sgn_aligned16(records), "records must be 16-byte aligned");
     if (N == 0 || num_chunks == 0) return SGN_OK;
     // SGN_PROJECT_STAGED=1: the two-phase form (compaction + shared-memory staging of the visible rows' colour parameters);
-    // the direct form is the default
-    static const bool staged = [] { const char* e = getenv("SGN_PROJECT_STAGED"); return e && e[0] == '1'; }();
-    if (staged)
+    // the direct form is the default.  Read on every call (one getenv per frame), so one process can run both forms.
+    const char* staged_env = getenv("SGN_PROJECT_STAGED");
+    if (staged_env && staged_env[0] == '1')
         project_fwd_staged_kernel<<<num_chunks, CH, nseg * sizeof(int), (cudaStream_t)stream>>>(
             segs_dev, nseg, *cam, reinterpret_cast<float4*>(records), radii, num_tiles_hit,
             reinterpret_cast<ushort4*>(tile_bbox), tiles_touched, touch_mask);
