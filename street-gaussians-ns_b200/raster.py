@@ -398,7 +398,9 @@ def bin_and_sort(cs: _lib.CameraStruct, records, radii, tiles_hit=None, bbox=Non
     bw = cs.block_width
     tiles = ((cs.width + bw - 1) // bw) * ((cs.height + bw - 1) // bw)
     tile_bins = torch.empty(tiles, 2, device=device, dtype=torch.int32)
-    if use_async and N > 0:
+    # the capped form keys its padding as one more tile: a camera of 65536 tiles leaves it no 16-bit key, so such a frame
+    # reads the count back like the synchronous form
+    if use_async and N > 0 and tiles < 65536:
         st = _async_state(device)
         _async_poll(st)
         if st["max_m"] > 0:  # a capacity is known: no read-back in this frame

@@ -16,10 +16,10 @@ import torch
 import street_gaussians_ns_b200.synthetic as syn
 from street_gaussians_ns_b200 import raster
 from street_gaussians_ns_b200.scene import Frame, Segment
+from oracle.bin_ref64 import COOP_AREA, check_lists, emission_prefix, expected_pairs, list_order
 
 pytestmark = pytest.mark.gpu
 
-COOP_AREA = 32
 SCENES = {
     "actors_in_front": lambda: syn.make_frame(n_background=60000, n_actors=4, n_per_actor=3000, width=128, height=96, seed=12,
                                               actor_shift=np.array([0.0, 0.0, 4.0])),
@@ -46,49 +46,6 @@ def host_rows(proj):
                 touched=proj.tiles_touched.cpu().numpy().astype(np.int64), mask=proj.touch_mask.cpu().numpy().view(np.uint32))
 
 
-def expected_pairs(h, tiles_x):
-    """(tile, row) of every entry the masks decode to (AABBs of at most 32 tiles)."""
-    bb, mask = h["bbox"], h["mask"].astype(np.int64)
-    w, area = bb[:, 2] - bb[:, 0], (bb[:, 2] - bb[:, 0]) * (bb[:, 3] - bb[:, 1])
-    small = np.nonzero((h["radii"] > 0) & (area <= COOP_AREA) & (mask != 0))[0]
-    tiles, rows = [], []
-    for b in range(32):
-        r = small[((mask[small] >> b) & 1).astype(bool)]
-        assert np.all(b < area[r])
-        tiles.append((bb[r, 1] + b // w[r]) * tiles_x + bb[r, 0] + b % w[r])
-        rows.append(r)
-    return np.concatenate(tiles), np.concatenate(rows), area
-
-
-def check_lists(h, tiles_x, tiles, ids, tile_bins, cls_ids, cls_bins, want_entries):
-    """want_entries: (tile, row) of every listed entry, in list order (tile, depth bits, row)."""
-    M = len(want_entries[0])
-    ids = ids[:M]
-    row = ids & 0x7FFFFFFF
-    tile_of = np.repeat(np.arange(tiles), tile_bins[:, 1] - tile_bins[:, 0])
-    # tile_bins: contiguous in tile order, (0, 0) when empty
-    cnt = tile_bins[:, 1] - tile_bins[:, 0]
-    assert np.all(cnt >= 0) and cnt.sum() == M
-    nz = cnt > 0
-    assert np.array_equal(tile_bins[nz, 0], (np.cumsum(cnt) - cnt)[nz])
-    assert np.all(tile_bins[~nz] == 0)
-    # the entries are the specified (tile, row) pairs, in the specified order
-    assert np.array_equal(tile_of, want_entries[0])
-    assert np.array_equal(row, want_entries[1])
-    assert np.array_equal(ids < 0, h["obj"][row])
-    key = (h["depth"][row] << np.uint64(32)) | row.astype(np.uint64)
-    same = tile_of[1:] == tile_of[:-1]
-    assert np.all(key[1:][same] > key[:-1][same]), "a tile's ids are not strictly increasing in (depth bits, row)"
-    # class sub-lists: stable partition, offsets are exclusive scans of the class counts
-    is_obj = ids < 0
-    for c, sel in ((0, ~is_obj), (1, is_obj)):
-        n_c = np.bincount(tile_of[sel], minlength=tiles)
-        scan = np.cumsum(n_c) - n_c
-        assert np.array_equal(cls_bins[c, :, 0], scan), c
-        assert np.array_equal(cls_bins[c, :, 1], scan + n_c), c
-        assert np.array_equal(cls_ids[c, :int(n_c.sum())], ids[sel]), c  # per tile in order, tiles in order: the stable partition
-
-
 def spec_entries(h, tiles_x, lists_tile, lists_row):
     """All entries in list order: the small AABBs from their masks, the big ones as listed (checked against tiles_touched)."""
     st, sr, area = expected_pairs(h, tiles_x)
@@ -106,18 +63,6 @@ def spec_entries(h, tiles_x, lists_tile, lists_row):
     tile = np.concatenate([st, bt])
     row = np.concatenate([sr, br])
     return tile, row
-
-
-def list_order(h, tile, row):
-    """Sort (tile, row) pairs by (tile, depth bits, row)."""
-    o = np.lexsort((row, h["depth"][row], tile))
-    return tile[o], row[o]
-
-
-def emission_prefix(h, tile, row, n):
-    """The first n entries of the depth-ordered entry sequence: runs in (depth bits, row) order, tiles ascending in a run."""
-    o = np.lexsort((tile, row, h["depth"][row]))[:n]
-    return tile[o], row[o]
 
 
 @pytest.fixture(scope="module", params=list(SCENES))
