@@ -337,6 +337,23 @@ int sgn_ssim_fwd(int H, int W, const sgn_loss_in* in, float weight, float* loss,
 int sgn_ssim_bwd(int H, int W, const sgn_loss_in* in, float weight, const float* grad_loss, const void* workspace, float* v_rgb,
                  void* stream);
 
+/* ---- sky cube map (EnvLight, sgn_splatfacto.py:109-150; use_sky_sphere = True) ------------------------------
+ * nvdiffrast dr.texture(tex[None], l, filter_mode='linear', boundary_mode='cube') on a learnable [6,R,R,3] map, and its
+ * gradient for the map (no gradient for the directions).  The camera path generates the reference's per-pixel world
+ * directions itself: d = normalize(((x - cx + ju) / fx, (y - cy + jv) / fy, 1)), rotated by c2w[:3,:3] (recovered from
+ * cam->viewmat), then l = (d.x, d.z, -d.y); ju = jv = 0.5 in eval (jitter pointers NULL), two [H,W] uniform draws in
+ * training.  The backward recomputes the directions from the same jitter.  v_tex is ACCUMULATED into (zero it first); it
+ * uses float atomics, so it is not bit-reproducible.  R < 1, a null required pointer, a single jitter array or sizes
+ * beyond 32-bit indexing return SGN_ERR_INVALID and launch nothing. */
+/* sky[H,W,3]; dirs[H,W,3] (the lookup directions l) or NULL */
+int sgn_sky_fwd(const sgn_camera* cam, const float* jitter_u, const float* jitter_v, const float* tex, int R, float* sky, float* dirs,
+                void* stream);
+int sgn_sky_bwd(const sgn_camera* cam, const float* jitter_u, const float* jitter_v, int R, const float* v_sky, float* v_tex,
+                void* stream);
+/* The same sampler on given directions uv[P,3]: out[P,3]; backward accumulates into v_tex. */
+int sgn_cube_texture_fwd(int P, const float* uv, const float* tex, int R, float* out, void* stream);
+int sgn_cube_texture_bwd(int P, const float* uv, int R, const float* v_out, float* v_tex, void* stream);
+
 /* ---- densification statistics (SURVEY.md 8f rank 3) -------------------------------------------------------
  * What each sub-model's `after_train` accumulates after backward (sgn_splatfacto.py:513-541), for all visible
  * sub-models of the frame in one launch: grads = ||v_records[:,0:2]||; on a sub-model's first call

@@ -128,6 +128,7 @@ EXPORTS = [
     "sgn_bin_sort_scratch_bytes", "sgn_bin_sort", "sgn_bin_class_scratch_bytes", "sgn_bin_class_lists", "sgn_blend_sched_ints",
     "sgn_blend_fwd", "sgn_blend_bwd", "sgn_sizeof_adam_tensor", "sgn_adam_chunk_elems", "sgn_adam_step",
     "sgn_loss_scratch_bytes", "sgn_loss_fwd", "sgn_loss_bwd", "sgn_ssim_workspace_bytes", "sgn_ssim_fwd", "sgn_ssim_bwd",
+    "sgn_sky_fwd", "sgn_sky_bwd", "sgn_cube_texture_fwd", "sgn_cube_texture_bwd",
     "sgn_sizeof_densify_segment", "sgn_densify_stats",
     "sgn_sizeof_refine_config", "sgn_sizeof_refine_tensors", "sgn_refine_decide", "sgn_refine_apply",
     "sgn_bin_local_cap", "sgn_bin_local_scratch_bytes", "sgn_bin_local_count", "sgn_bin_local_sort",
@@ -215,6 +216,12 @@ def load():
     L.sgn_ssim_fwd.argtypes = [i32, i32, C.POINTER(LossIn), fl, vp, vp, sz, vp]
     L.sgn_ssim_bwd.argtypes = [i32, i32, C.POINTER(LossIn), fl, vp, vp, vp, vp]
     L.sgn_ssim_fwd.restype = L.sgn_ssim_bwd.restype = C.c_int
+    L.sgn_sky_fwd.argtypes = [C.POINTER(CameraStruct), vp, vp, vp, i32, vp, vp, vp]
+    L.sgn_sky_bwd.argtypes = [C.POINTER(CameraStruct), vp, vp, i32, vp, vp, vp]
+    L.sgn_cube_texture_fwd.argtypes = [i32, vp, vp, i32, vp, vp]
+    L.sgn_cube_texture_bwd.argtypes = [i32, vp, i32, vp, vp, vp]
+    for f in ("sgn_sky_fwd", "sgn_sky_bwd", "sgn_cube_texture_fwd", "sgn_cube_texture_bwd"):
+        getattr(L, f).restype = C.c_int
     L.sgn_sizeof_adam_tensor.restype = sz
     L.sgn_adam_chunk_elems.restype = C.c_int
     L.sgn_adam_step.argtypes = [vp, i32, i32, vp, vp, vp, vp]

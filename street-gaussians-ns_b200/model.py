@@ -308,7 +308,9 @@ class SceneGraphRasterModel(torch.nn.Module):
         for obj_id, ps in actors.items():
             self.all_models[self.get_object_model_name(obj_id)] = GaussianSubModel(ps)
         self.poses_at = poses_at or (lambda t: [])
-        self.env_map = sky  # stays on nvdiffrast in the reference (EnvLight, sgn_splatfacto.py:109-150)
+        # the learnable sky (EnvLight, sgn_splatfacto.py:109-150): sky.CubeMapSky on this library's kernels, or any callable
+        # (camera, train) -> [H, W, 3] such as the reference's EnvLight on nvdiffrast
+        self.env_map = sky
         self.step = 0
         self.visible_model_names: List[str] = ["background"]
         self.xys = self.depths = self.radii = self.conics = self.num_tiles_hit = None

@@ -117,6 +117,10 @@ class FusedAdam:
         self._extra_ptrs = {t.data_ptr() for t, _ in self._extra.values()}
         self._lr_vec = np.array([self.lrs[k] for k in self.kinds], np.float64)
 
+    def extra_tensors(self) -> Dict[str, torch.Tensor]:
+        """The further tensors this optimizer steps (``extra``), by name."""
+        return {name: t for name, (t, _) in self._extra.items()}
+
     def set_lr(self, kind: str, lr: float) -> None:
         """Schedulers (e.g. the exponential decay of the means lr, sgn_config.py:85-90) update rates here."""
         self.lrs[kind] = lr

@@ -68,11 +68,18 @@ class TrainStep:
         if world > 1:
             assert full, "data parallel needs SceneGraphConfig(full_gradient_arena=True): replicas see different actors"
             assert all_cameras is not None and len(all_cameras) == world
+        extras = opt.extra_tensors()                      # the optimizer's further groups (the sky cube map)
+        if world > 1 and any(t.requires_grad for t in extras.values()):
+            # refused before anything is rendered or exchanged: the gradient exchange covers the arena only
+            raise NotImplementedError(f"data-parallel training does not exchange the gradients of {sorted(extras)}: the "
+                                      "replicas would diverge")
         if world > 1:
             self._ensure_exchange()
         m.step = step                                     # step_cb (sgn_splatfacto.py:754-755)
         for p in m.parameters():                          # Optimizers.zero_grad_all()
             p.grad = None
+        for t in extras.values():
+            t.grad = None
         out = m.get_outputs(camera)
         if world > 1 and self._exchange is not None:  # which background rows this replica sees (rows nobody sees are not exchanged)
             h = m._holder
@@ -97,6 +104,8 @@ class TrainStep:
                 self._maybe_refine(step)
                 return losses
             arena = m.zero_gradient_arena()
+        # the further tensors of the optimizer (the sky cube map, sky.CubeMapSky.base) step with the gradient autograd left
+        extra_grads = {name: t.grad for name, t in extras.items() if t.grad is not None}
         if world > 1:
             present = sorted(set(i for cam in all_cameras for i in self.submodels_in_view(cam)))
         else:
@@ -109,7 +118,7 @@ class TrainStep:
         else:
             if world > 1:
                 dp.allreduce_gradients(arena, average=True, group=self.group)
-            opt.step(arena, present=None if everything else present, full_layout=full)
+            opt.step(arena, present=None if everything else present, full_layout=full, extra_grads=extra_grads or None)
         if rendered:
             m.after_train(step)                           # AFTER_TRAIN_ITERATION callbacks, in the reference's order
         self._maybe_refine(step)

@@ -25,9 +25,10 @@ sys.path.insert(0, ROOT)
 
 def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int = 100, start_step: int = 600,
         actor_range: float = 45.0, pipeline_chunks: int = 0, overlap: bool = False, resident_table: bool = True,
-        async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True) -> dict:
+        async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True, sky: bool = False) -> dict:
     """One measurement.  torch.distributed must already be initialised when WORLD_SIZE > 1.  Returns the result dict on
-    rank 0 (None elsewhere)."""
+    rank 0 (None elsewhere).  ``sky``: the reference's default learnable sky (use_sky_sphere, a 1024^2 cube map stepped by
+    the same Adam launch at the ``sky_sphere`` group's lr 0.005, sgn_config.py:72-75)."""
     import torch
     import torch.distributed as dist
 
@@ -52,12 +53,18 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         return [ActorPose(str(a), rot, center, f, frame_list) for a, rot, center in sc.boxes_at(f)]
 
     rs = RefineSettings(refine_every=refine_every)
-    cfg = SceneGraphConfig(use_sky_sphere=False, ssim_lambda=ssim_lambda, fused_loss=fused_loss, full_gradient_arena=world > 1, refine=rs, async_binning=async_binning,
+    cfg = SceneGraphConfig(use_sky_sphere=sky, ssim_lambda=ssim_lambda, fused_loss=fused_loss, full_gradient_arena=world > 1, refine=rs, async_binning=async_binning,
                            object_refine=RefineSettings(refine_every=refine_every, cull_alpha_thresh=0.005),
                            num_train_data=len(cams), refine_record=True)
-    model = SceneGraphRasterModel(sc.background.to(dev), {k: v.to(dev) for k, v in sc.actors.items()}, cfg, poses_at=poses_at).to(dev)
+    env_map = None
+    if sky:
+        from street_gaussians_ns_b200.sky import CubeMapSky
+        env_map = CubeMapSky(1024)
+    model = SceneGraphRasterModel(sc.background.to(dev), {k: v.to(dev) for k, v in sc.actors.items()}, cfg, poses_at=poses_at,
+                                  sky=env_map).to(dev)
     model.train()
-    opt = FusedAdam(model.optimizer_params(), reserve_spare=True)  # no cudaMalloc of moment arenas inside the training loop
+    extra = {"sky": (model.env_map.base, 0.005)} if sky else None
+    opt = FusedAdam(model.optimizer_params(), extra=extra, reserve_spare=True)  # no cudaMalloc of moment arenas inside the training loop
     step_fn = TrainStep(model, opt, refine_every=refine_every, pipeline_chunks=pipeline_chunks, overlap=overlap)
     g = torch.Generator().manual_seed(5)
     gt = (torch.rand(H, W, 3, generator=g) * 255).to(torch.uint8).to(dev)  # get_loss_dict consumes uint8 directly
@@ -164,6 +171,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         "config": {"workload": f"cfg{4 if world == 1 else 5}: 5 cameras x 85 frames, {sc.n_bg} background + 32 x {sc.n_act} actor Gaussians, "
                                f"{W}x{H}; rank r renders camera (step*g + r) mod 425; actors have a box within {actor_range} m of the ego vehicle",
                    "parallelism": f"camera-sharded dp{world}", "ssim_lambda": ssim_lambda,
+                   **({"sky": "CubeMapSky(1024), Adam lr 0.005"} if sky else {}),
                    "loss": "fused kernels" if fused_loss else "torch ops", "start_step": start_step, "refine_every": refine_every,
                    "refinement_kernels_loaded_before_timing": refine_warm,
                    "binning": "no host read-back of the intersection count" if async_binning else "one read-back per frame",
@@ -190,6 +198,7 @@ def main():
     ap.add_argument("--host-table", action="store_true", help="build the segment table on the host per frame instead of prepare_frames")
     ap.add_argument("--ssim-lambda", type=float, default=0.0, help="weight of the SSIM term (the reference trains with 0.2)")
     ap.add_argument("--torch-loss", action="store_true", help="loss terms as torch ops (SceneGraphConfig.fused_loss = False)")
+    ap.add_argument("--sky", action="store_true", help="train the learnable sky cube map (the reference's use_sky_sphere = True)")
     args = ap.parse_args()
 
     import torch
@@ -201,7 +210,7 @@ def main():
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     res = run(args.steps, args.warmup, args.scale, args.refine_every, args.start_step, args.actor_range, args.pipeline_chunks,
-              args.overlap, not args.host_table, ssim_lambda=args.ssim_lambda, fused_loss=not args.torch_loss)
+              args.overlap, not args.host_table, ssim_lambda=args.ssim_lambda, fused_loss=not args.torch_loss, sky=args.sky)
     if res is not None:
         print(json.dumps(res))
     if world > 1:
