@@ -173,6 +173,9 @@ extern "C" int sgn_allreduce_sym(void* local, void* multicast, const uint64_t* p
         SGN_REQUIRE(sl.width[s] >= 0 && sl.width[s] <= 4096 && sl.row0[s] >= 0 && sl.nrows[s] >= 0 &&
                         sl.nrows[s] * (int64_t)sl.width[s] <= slice_lengths[s],
                     "sgn_allreduce_sym: slice %d has a bad row description", s);
+        // rows_unseen indexes a row-skipping slice with 32-bit arithmetic
+        SGN_REQUIRE(sl.width[s] == 0 || slice_lengths[s] < ((int64_t)1 << 31),
+                    "sgn_allreduce_sym: row-skipping slice %d has %lld floats (at most 2^31 - 1)", s, (long long)slice_lengths[s]);
         total4 += sl.len4[s];
     }
     if (total4 == 0) return SGN_OK;

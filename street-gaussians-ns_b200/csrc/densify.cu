@@ -25,7 +25,8 @@ densify_stats_kernel(const sgn_densify_segment* __restrict__ table, int nseg, in
     }
     const sgn_densify_segment sg = table[lo];
     const int i = g - sg.row0;
-    if (i >= sg.count) return;
+    // rows in front of the first segment (a table whose first row0 > 0) give i < 0; rows in a gap give i >= count
+    if (i < 0 || i >= sg.count) return;
     const float4 v = __ldg(v_records + 3 * (size_t)g);  // (v_x, v_y, ...)
     // torch.linalg.vector_norm over 2 elements: sqrt(x*x + y*y)
     const float gn = sqrtf(__fadd_rn(__fmul_rn(v.x, v.x), __fmul_rn(v.y, v.y)));

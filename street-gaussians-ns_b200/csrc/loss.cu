@@ -5,7 +5,8 @@
 // elementwise / reduction launches.  The SSIM term (:1085-1087) has its own kernels (ssim.cu).  The ground truth may be the
 // uint8 image the data loader holds (gt = u8 / 255, as the reference's `.float() / 255`).
 //
-// Arithmetic follows torch: |a - b|, clamp(x, 1e-5, 1 - 1e-5) with pass-through gradient inside the closed
+// Arithmetic follows torch: gt*mask and rgb*mask rounded separately (no fma: an exact tie gt == rgb gives a zero difference
+// and a zero gradient under any mask), |a - b|, clamp(x, 1e-5, 1 - 1e-5) with pass-through gradient inside the closed
 // interval, natural log, means as sum / count (fp32 sums of per-block partials, summed in a fixed order: the
 // result is deterministic run to run).
 #include "sgn_common.cuh"
@@ -67,7 +68,7 @@ __global__ void __launch_bounds__(LOSS_THREADS) loss_fwd_kernel(const LossParams
         } else {
             for (long long e = tid; e < n3; e += stride) {
                 const float m = p.mask ? p.mask[e / 3] : 1.f;
-                s_l1 += fabsf(gt_at(p, e) * m - p.rgb[e] * m);
+                s_l1 += fabsf(__fmul_rn(gt_at(p, e), m) - __fmul_rn(p.rgb[e], m));
             }
         }
     }
@@ -129,7 +130,7 @@ __global__ void __launch_bounds__(LOSS_THREADS) loss_bwd_kernel(const LossParams
         } else {
             for (long long e = tid; e < n3; e += stride) {
                 const float m = p.mask ? p.mask[e / 3] : 1.f;
-                v_rgb[e] = -k * sgn(gt_at(p, e) * m - p.rgb[e] * m) * m;
+                v_rgb[e] = -k * sgn(__fmul_rn(gt_at(p, e), m) - __fmul_rn(p.rgb[e], m)) * m;
             }
         }
     }

@@ -72,6 +72,11 @@ class FusedAdam:
         self._extra = dict(extra or {})
         self.step_count = 0  # calls of step(); the bias correction uses the per-tensor counts below
         self._install(params)
+        if self.device.type == "cuda" and chunk_elems is not None and chunk_elems != _lib.load().sgn_adam_chunk_elems():
+            # every block of the kernel steps sgn_adam_chunk_elems() elements: a table cut at another chunk size would
+            # leave elements unstepped or step them twice (``chunk_elems`` is for host stand-ins of the kernel)
+            raise ValueError(f"FusedAdam on CUDA: chunk_elems={chunk_elems}, the kernel's chunk is "
+                             f"{_lib.load().sgn_adam_chunk_elems()}")
         self.exp_avg, self.exp_avg_sq = self._new_moments(), self._new_moments()
         if reserve_spare:
             # a refinement needs the old and the new arenas at the same time: put a second pair into the caching allocator's

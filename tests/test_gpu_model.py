@@ -179,6 +179,54 @@ def test_after_train_statistics_match_reference_expressions(setup):
         model.step = 30000
 
 
+def test_after_train_past_the_background_stop_split_at(setup):
+    """object_refine.stop_split_at > refine.stop_split_at, at a step between the two: after_train collects the actors'
+    statistics only, so the segment table starts at the first actor's row (row0 > 0).  The actors' statistics follow the
+    torch statements of after_train (sgn_splatfacto.py:513-541) and the background's are left as they were."""
+    fr, model, gt = setup
+    c = model.config
+    saved = (c.refine.stop_split_at, c.object_refine.stop_split_at)
+    c.refine.stop_split_at, c.object_refine.stop_split_at = 100, 200
+    model.step = 150
+    try:
+        for sub in model.all_models.values():
+            sub.xys_grad_norm = sub.vis_counts = sub.max_2Dsize = None
+        bgm = model.all_models["background"]
+        n_bg = bgm.num_points
+        fill = [torch.full((n_bg,), v, device=gt.device) for v in (0.25, 3.0, 0.125)]
+        bgm.xys_grad_norm, bgm.vis_counts, bgm.max_2Dsize = (t.clone() for t in fill)
+        ref = {}
+        for it in range(2):
+            for p in model.parameters():
+                p.grad = None
+            _loss(model, model.get_outputs(fr.camera), gt).backward()
+            model.after_train(model.step)
+            for name in model.visible_model_names:
+                if name == "background":
+                    continue
+                sub = model.all_models[name]
+                vis = (sub.radii > 0).flatten()
+                grads = sub.xys.grad.detach().norm(dim=-1)
+                if name not in ref:
+                    ref[name] = r = dict(g=grads.clone(), c=torch.ones_like(grads), m=torch.zeros_like(sub.radii, dtype=torch.float32))
+                else:
+                    r = ref[name]
+                    r["c"][vis] = r["c"][vis] + 1
+                    r["g"][vis] = grads[vis] + r["g"][vis]
+                r["m"][vis] = torch.maximum(r["m"][vis], sub.radii.detach()[vis] / float(max(model.last_size)))
+        assert len(ref) == 4 and model._slices[1][1].start == n_bg
+        for name, r in ref.items():
+            sub = model.all_models[name]
+            assert torch.equal(sub.vis_counts, r["c"]), name
+            assert torch.allclose(sub.max_2Dsize, r["m"], rtol=2e-6, atol=0), name
+            assert torch.allclose(sub.xys_grad_norm, r["g"], rtol=2e-6, atol=1e-12), name
+        for got, want in zip((bgm.xys_grad_norm, bgm.vis_counts, bgm.max_2Dsize), fill):
+            assert torch.equal(got, want)
+    finally:
+        c.refine.stop_split_at, c.object_refine.stop_split_at = saved
+        model.step = 30000
+
+
 def test_device_resident_frame_table_and_pose_content_key():
     """SURVEY 8f rank 4: prepare_frames() builds every timestamp's segment rows once (one upload); get_outputs then indexes
     the resident table.  Same images as the per-frame host build; a box moved IN PLACE at a fixed timestamp (what the
