@@ -302,6 +302,16 @@ int sgn_blend_extra_fwd(const sgn_camera* cam, const sgn_blend_opts* opts, const
 int sgn_blend_extra_bwd(const sgn_camera* cam, const sgn_blend_opts* opts, const float* records, const int32_t* sorted_ids,
                         const int32_t* tile_bins, const float* final_T, const int32_t* final_idx, const float* extra, int C,
                         const float* v_out /*[H,W,C]*/, float* v_extra /*[N,C]*/, float* v_records /*[N,12]*/, void* stream);
+/* Deterministic form of sgn_blend_extra_bwd (the extra channels under sgn_blend_bwd_in.v_fixed): the per-Gaussian sums are
+ * accumulated in 64-bit fixed point (one rounding per addend, integer adds: bit-identical totals whatever the execution
+ * order), converted, and then ADDED to v_extra and to the geometry part of v_records, as the float form adds.
+ * fixed_geom [num_gaussians,6] and fixed_extra [num_gaussians,C] int64, ZERO on entry; fixed_scale: two floats of device
+ * scratch. */
+int sgn_blend_extra_bwd_det(const sgn_camera* cam, const sgn_blend_opts* opts, const float* records, const int32_t* sorted_ids,
+                            const int32_t* tile_bins, const float* final_T, const int32_t* final_idx, const float* extra, int C,
+                            int64_t num_gaussians, const float* v_out /*[H,W,C]*/, float* v_extra /*[N,C]*/,
+                            float* v_records /*[N,12]*/, int64_t* fixed_geom, int64_t* fixed_extra, float* fixed_scale,
+                            void* stream);
 
 /* ---- loss epilogue (SURVEY.md 8f rank 2) ------------------------------------------------------------------
  * The image-space loss terms of the reference that re-read the rasterizer's outputs right after the render, and

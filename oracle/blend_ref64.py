@@ -143,11 +143,12 @@ class _Stream:
             for kk in (np.minimum(self.ks, L - 1), np.maximum(self.last, 0)):
                 np.minimum.at(gm, gid[G, kk], np.where(inside, m_stop, np.inf))
 
-    def backward(self, rec, v_ch, cols, tfv_acc, T_final, clamp, out, out_abs):
-        """Adds this stream's per-Gaussian gradients to out[N+1,12], and to out_abs the same sums taken over the absolute
-        values of their terms (what bounds the rounding error of an fp32 evaluation: these sums cancel, e.g. the depth
-        cotangent's terms of a Gaussian that alone makes up a pixel's depth).  v_ch [G,P,C] channel cotangents of the
-        blended sums (C = len(cols), may be 0), tfv_acc [G,P] the cotangent of 1 - T_final, T_final [G,P]."""
+    def backward(self, values, v_ch, tfv_acc, T_final, clamp, out, out_abs, v_val=None, v_val_abs=None):
+        """Adds this stream's per-Gaussian geometry gradients to out[N+1, 0:6] and its channel gradients to v_val[N+1,C],
+        and to out_abs / v_val_abs the same sums taken over the absolute values of their terms (what bounds the rounding
+        error of an fp32 evaluation: these sums cancel, e.g. the depth cotangent's terms of a Gaussian that alone makes up
+        a pixel's depth).  values [N+1,C] the blended channels (None: none), v_ch [G,P,C] their cotangents, tfv_acc [G,P]
+        the cotangent of 1 - T_final, T_final [G,P]."""
         B = self.blended
         with np.errstate(all="ignore"):
             ab = np.minimum(clamp, self.raw)
@@ -156,8 +157,8 @@ class _Stream:
             fac = np.where(B, ab * Tp, 0.0)
             v_alpha = T_final[:, :, None] * ra * tfv_acc[:, :, None]
             v_abs = np.abs(v_alpha)
-            if cols:
-                colors = rec[self.gid][:, :, cols]  # [G,L,C]
+            if values is not None and values.shape[1]:
+                colors = values[self.gid]  # [G,L,C]
                 cv = np.einsum("glc,gpc->gpl", colors, v_ch)
                 cva = np.einsum("glc,gpc->gpl", np.abs(colors), np.abs(v_ch))
                 x, xa = fac * cv, fac * cva
@@ -167,9 +168,8 @@ class _Stream:
                 v_abs = v_abs + Tp * cva + ra * behind_a
                 vc = np.einsum("gpl,gpc->glc", fac, v_ch)
                 vca = np.einsum("gpl,gpc->glc", fac, np.abs(v_ch))
-                for n, col in enumerate(cols):
-                    np.add.at(out[:, col], self.gid, vc[:, :, n])
-                    np.add.at(out_abs[:, col], self.gid, vca[:, :, n])
+                np.add.at(v_val, self.gid, vc)
+                np.add.at(v_val_abs, self.gid, vca)
             v_alpha = np.where(B, v_alpha, 0.0)
             vs = np.where(B, -self.raw * v_alpha, 0.0)  # d/d sigma
             vsa = np.where(B, np.abs(self.raw) * v_abs, 0.0)
@@ -390,11 +390,71 @@ def backward(inp: Inputs, opts: Opts, cot: Dict[str, Optional[np.ndarray]]):
             return np.where(inside.reshape(inside.shape + (1,) * (g.ndim - 2)), g, 0.0)
 
         m = e["main"]
-        m.backward(rec, tile_view(vch), COL_RGBD, tile_view(voa), m.T_final, opts.clamp_bwd, out, out_abs)
+        m.backward(rec[:, COL_RGBD], tile_view(vch), tile_view(voa), m.T_final, opts.clamp_bwd, out, out_abs,
+                   out[:, 6:10], out_abs[:, 6:10])
         if v_obj is not None:
-            e["obj"].backward(rec, None, [], tile_view(v_obj[:, 0]), e["obj"].T_final, opts.clamp_bwd, out, out_abs)
+            e["obj"].backward(None, None, tile_view(v_obj[:, 0]), e["obj"].T_final, opts.clamp_bwd, out, out_abs)
         if v_bg is not None:
-            e["bg"].backward(rec, None, [], tile_view(v_bg[:, 0]), e["bg"].T_final, opts.clamp_bwd, out, out_abs)
+            e["bg"].backward(None, None, tile_view(v_bg[:, 0]), e["bg"].T_final, opts.clamp_bwd, out, out_abs)
     if opts.has_sky and v_sky is None and v_rgb is None:
         v_sky = np.zeros((H, W, 3))
     return out[:N], v_sky, fw, out_abs[:N]
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# generic channels: the main stream (slot 0) compositing values[N,C] -- sgn_blend_extra_fwd / _bwd, and the Level-1
+# rasterize_gaussians (out = blended + T_final * background, alpha = 1 - T_final)
+# ------------------------------------------------------------------------------------------------------------------
+def _channels(values, N):
+    v = np.asarray(values, np.float64).reshape(N, -1)
+    return np.concatenate([v, np.zeros((1, v.shape[1]))], 0)  # row N: the padding dummy
+
+
+def forward_channels(inp: Inputs, opts: Opts, values, background=None) -> Dict[str, np.ndarray]:
+    """out [H,W,C] = sum_k values[k,c] alpha_k T_k (+ T_final background[c]), abs [H,W,C] the same sum over |terms|,
+    final_T / final_idx [H,W] of the main stream, margin [H,W] and gauss_margin [N] as in ``forward``."""
+    rec, streams, o = _run(inp, opts)
+    N = rec.shape[0] - 1
+    vals = _channels(values, N)
+    H, W, Cn = inp.height, inp.width, vals.shape[1]
+    out = np.zeros((H * W, Cn))
+    out_abs = np.zeros((H * W, Cn))
+    for e in streams:
+        pid, inside, m = e["pid"], e["inside"], e["main"]
+        out[pid[inside]] = np.einsum("gpl,glc->gpc", m.w, vals[m.gid])[inside]
+        out_abs[pid[inside]] = np.einsum("gpl,glc->gpc", m.w, np.abs(vals[m.gid]))[inside]
+    T = o["final_T"][0]
+    if background is not None:
+        bg = np.asarray(background, np.float64).reshape(Cn)
+        out += T[:, None] * bg[None, :]
+        out_abs += T[:, None] * np.abs(bg)[None, :]
+    return dict(out=out.reshape(H, W, Cn), abs=out_abs.reshape(H, W, Cn), final_T=T.reshape(H, W),
+                final_idx=o["final_idx"][0].reshape(H, W), margin=o["margin"].reshape(H, W), gauss_margin=o["gauss_margin"][:-1])
+
+
+def backward_channels(inp: Inputs, opts: Opts, values, v_out, v_alpha=None, background=None):
+    """(v_values [N,C], v_records [N,12] with the geometry in columns 0..5 (the rest 0), and the sums of the absolute
+    values of each gradient's terms in the same two layouts) for the cotangents v_out [H,W,C] of ``forward_channels``'s out
+    and v_alpha [H,W] of 1 - T_final."""
+    rec, streams, o = _run(inp, opts)
+    N = rec.shape[0] - 1
+    vals = _channels(values, N)
+    H, W, Cn = inp.height, inp.width, vals.shape[1]
+    P = H * W
+    vch = np.asarray(v_out, np.float64).reshape(P, Cn)
+    voa = np.zeros(P) if v_alpha is None else np.asarray(v_alpha, np.float64).reshape(P).copy()
+    if background is not None:  # out_c = blended_c + T_final bg_c: T_final = 1 - alpha
+        voa -= vch @ np.asarray(background, np.float64).reshape(Cn)
+    out = np.zeros((N + 1, RECORD_FLOATS))
+    out_abs = np.zeros((N + 1, RECORD_FLOATS))
+    v_val = np.zeros((N + 1, Cn))
+    v_val_abs = np.zeros((N + 1, Cn))
+    for e in streams:
+        pid, inside, m = e["pid"], e["inside"], e["main"]
+
+        def tile_view(x):
+            g = x[pid]
+            return np.where(inside.reshape(inside.shape + (1,) * (g.ndim - 2)), g, 0.0)
+
+        m.backward(vals, tile_view(vch), tile_view(voa), m.T_final, opts.clamp_bwd, out, out_abs, v_val, v_val_abs)
+    return v_val[:N], out[:N], v_val_abs[:N], out_abs[:N]

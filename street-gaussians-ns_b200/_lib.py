@@ -132,7 +132,7 @@ EXPORTS = [
     "sgn_sizeof_densify_segment", "sgn_densify_stats",
     "sgn_sizeof_refine_config", "sgn_sizeof_refine_tensors", "sgn_refine_decide", "sgn_refine_apply",
     "sgn_bin_local_cap", "sgn_bin_local_scratch_bytes", "sgn_bin_local_count", "sgn_bin_local_sort",
-    "sgn_project_bwd_range", "sgn_allreduce_sym", "sgn_blend_extra_fwd", "sgn_blend_extra_bwd",
+    "sgn_project_bwd_range", "sgn_allreduce_sym", "sgn_blend_extra_fwd", "sgn_blend_extra_bwd", "sgn_blend_extra_bwd_det",
     "sgn_bin_sort_capped", "sgn_visible_flags", "sgn_visible_union",
 ]
 AR_MAX_SLICES = 48  # SGN_AR_MAX_SLICES
@@ -167,7 +167,9 @@ def load():
     L.sgn_allreduce_sym.restype = L.sgn_visible_flags.restype = L.sgn_visible_union.restype = C.c_int
     L.sgn_blend_extra_fwd.argtypes = [C.POINTER(CameraStruct), C.POINTER(BlendOpts), vp, vp, vp, vp, vp, vp, i32, vp, vp]
     L.sgn_blend_extra_bwd.argtypes = [C.POINTER(CameraStruct), C.POINTER(BlendOpts), vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp]
-    L.sgn_blend_extra_fwd.restype = L.sgn_blend_extra_bwd.restype = C.c_int
+    L.sgn_blend_extra_bwd_det.argtypes = [C.POINTER(CameraStruct), C.POINTER(BlendOpts), vp, vp, vp, vp, vp, vp, i32, i64, vp, vp, vp,
+                                          vp, vp, vp, vp]
+    L.sgn_blend_extra_fwd.restype = L.sgn_blend_extra_bwd.restype = L.sgn_blend_extra_bwd_det.restype = C.c_int
     fl = C.c_float
     L.sgn_l1_project_fwd.argtypes = [i32, vp, vp, fl, vp, C.POINTER(CameraStruct), vp, vp, vp, vp, vp, vp, vp, vp]
     L.sgn_l1_project_bwd.argtypes = [i32, vp, vp, fl, vp, C.POINTER(CameraStruct), vp, vp, vp, vp, vp, vp, vp, vp]

@@ -1581,10 +1581,26 @@ struct ExtraParams {
     float* v_extra;            // backward: [N, C] (accumulated)
     float* v_records;          // backward: [N, 12] (geometry part accumulated)
 };
+// the deterministic backward's own arguments: a separate kernel parameter type, so that the float instantiations keep
+// theirs (and their register allocation) unchanged
+struct ExtraDetParams {
+    ExtraParams p;
+    long long* fx_geom;     // [N, 6] fixed-point geometry accumulators (zeroed)
+    long long* fx_extra;    // [N, C] fixed-point channel accumulators (zeroed)
+    const float* fx_scale;  // units per unit of gradient: [0] geometry, [1] channels
+};
+template <bool DET>
+using ExtraArgs = typename std::conditional<DET, ExtraDetParams, ExtraParams>::type;
+__device__ __forceinline__ const ExtraParams& extra_base(const ExtraParams& p) { return p; }
+__device__ __forceinline__ const ExtraParams& extra_base(const ExtraDetParams& q) { return q.p; }
 
-// one warp per tile, lane = (column, row parity), 8 pixels per lane (rows two apart); blockIdx.y = channel group
-template <bool BWD>
-__global__ void __launch_bounds__(32) extra_kernel(const ExtraParams p) {
+// one warp per tile, lane = (column, row parity), 8 pixels per lane (rows two apart); blockIdx.y = channel group.
+// DET (backward only): the per-Gaussian sums go to the fixed-point accumulators, one rounding per addend and integer adds,
+// as accumulate_grad does for the main backward; the float instantiations carry no fixed-point code.
+template <bool BWD, bool DET = false>
+__global__ void __launch_bounds__(32) extra_kernel(const ExtraArgs<DET> args) {
+    static_assert(BWD || !DET, "the forward has no accumulators");
+    const ExtraParams& p = extra_base(args);
     constexpr int PPL = 8;
     __shared__ float4 sA[32], sB[32];
     __shared__ float sX[32][EXTRA_CG + 1];
@@ -1714,8 +1730,19 @@ __global__ void __launch_bounds__(32) extra_kernel(const ExtraParams p) {
                 const float mine = warp_multi_reduce<NV>(comps, lane);
                 if (my_comp >= 0) {
                     const size_t g = (size_t)sId[t];
-                    if (my_comp < 6) atomicAdd(p.v_records + g * SGN_RECORD_FLOATS + my_comp, mine);
-                    else if (my_comp - 6 < nch) atomicAdd(p.v_extra + g * p.C + c0 + (my_comp - 6), mine);
+                    if constexpr (DET) {
+                        if (my_comp < 6) {
+                            const int sh = fixed_shift(reinterpret_cast<const float*>(p.records), g * SGN_RECORD_FLOATS + my_comp);
+                            const float m = mine * __ldg(args.fx_scale) * __int_as_float((127 - sh) << 23);  // times 2^-sh: exact
+                            atomicAdd(reinterpret_cast<unsigned long long*>(args.fx_geom) + g * 6 + my_comp, (unsigned long long)__float2ll_rn(m));
+                        } else if (my_comp - 6 < nch) {
+                            atomicAdd(reinterpret_cast<unsigned long long*>(args.fx_extra) + g * p.C + c0 + (my_comp - 6),
+                                      (unsigned long long)__float2ll_rn(mine * __ldg(args.fx_scale + 1)));
+                        }
+                    } else {
+                        if (my_comp < 6) atomicAdd(p.v_records + g * SGN_RECORD_FLOATS + my_comp, mine);
+                        else if (my_comp - 6 < nch) atomicAdd(p.v_extra + g * p.C + c0 + (my_comp - 6), mine);
+                    }
                 }
             }
         }
@@ -1773,5 +1800,57 @@ extern "C" int sgn_blend_extra_bwd(const sgn_camera* cam, const sgn_blend_opts* 
     p.v_out = v_out; p.v_extra = v_extra; p.v_records = v_records;
     extra_kernel<true><<<dim3(p.tiles, (C + EXTRA_CG - 1) / EXTRA_CG), 32, 0, (cudaStream_t)stream>>>(p);
     SGN_CHECK_LAUNCH("extra_kernel<bwd>");
+    return SGN_OK;
+}
+
+// ---- deterministic extra backward: the fixed-point grids are powers of two.  An entry's alpha cotangent is
+// sum_c extra_c v_c, at most C max|extra| max|v_out|: the geometry grid is 2^32 units per unit of that bound (the
+// conic components of wide Gaussians give up fixed_shift places, as in the main backward).  A channel gradient is a sum
+// of weights times v_out: its grid is 2^32 units per max|v_out|.  Both keep 2^31 units of headroom.
+__global__ void extra_fixed_scale_kernel(float* scale, int C) {
+    const float mv = scale[0], me = fmaxf(1.f, scale[1]);  // the bits cot_max_kernel left are the floats themselves
+    const double eg = ceil(log2((double)mv * (double)me * (double)C)), ev = ceil(log2((double)mv));
+    scale[0] = mv > 0.f ? (float)exp2(32.0 - fmin(eg, 150.0)) : 4294967296.f;
+    scale[1] = mv > 0.f ? (float)exp2(32.0 - fmin(ev, 150.0)) : 4294967296.f;
+}
+__global__ void __launch_bounds__(256)
+extra_fixed_add_kernel(const long long* __restrict__ fx_geom, const long long* __restrict__ fx_extra, const float* __restrict__ scale,
+                       const float* __restrict__ records, float* __restrict__ v_records, float* __restrict__ v_extra, long long N, int C) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < 6 * N) {
+        const size_t idx = (size_t)(i / 6) * SGN_RECORD_FLOATS + (size_t)(i % 6);
+        v_records[idx] += (float)(ldexp((double)fx_geom[i], fixed_shift(records, idx)) / (double)scale[0]);
+    } else if (i < 6 * N + (long long)C * N) {
+        const long long k = i - 6 * N;
+        v_extra[k] += (float)((double)fx_extra[k] / (double)scale[1]);
+    }
+}
+
+extern "C" int sgn_blend_extra_bwd_det(const sgn_camera* cam, const sgn_blend_opts* opts, const float* records, const int32_t* sorted_ids,
+                                       const int32_t* tile_bins, const float* final_T, const int32_t* final_idx, const float* extra, int C,
+                                       int64_t num_gaussians, const float* v_out, float* v_extra, float* v_records, int64_t* fixed_geom,
+                                       int64_t* fixed_extra, float* fixed_scale, void* stream_) {
+    SGN_RANGE("sgn_blend_extra_bwd_det");
+    cudaStream_t stream = (cudaStream_t)stream_;
+    ExtraDetParams q;
+    ExtraParams& p = q.p;
+    if (int rc = extra_params(p, cam, opts, records, sorted_ids, tile_bins, final_T, final_idx, extra, C)) return rc;
+    SGN_REQUIRE(v_out && v_extra && v_records && fixed_geom && fixed_extra && fixed_scale, "sgn_blend_extra_bwd_det: null pointer");
+    SGN_REQUIRE(num_gaussians > 0, "sgn_blend_extra_bwd_det: num_gaussians=%lld", (long long)num_gaussians);
+    p.v_out = v_out; p.v_extra = v_extra; p.v_records = v_records;
+    q.fx_geom = reinterpret_cast<long long*>(fixed_geom); q.fx_extra = reinterpret_cast<long long*>(fixed_extra);
+    q.fx_scale = fixed_scale;
+    SGN_CHECK_CUDA(cudaMemsetAsync(fixed_scale, 0, 2 * sizeof(float), stream));
+    cot_max_kernel<<<296, 256, 0, stream>>>(v_out, (long long)p.width * p.height * C, reinterpret_cast<unsigned*>(fixed_scale));
+    cot_max_kernel<<<296, 256, 0, stream>>>(extra, (long long)num_gaussians * C, reinterpret_cast<unsigned*>(fixed_scale) + 1);
+    SGN_CHECK_LAUNCH("cot_max_kernel");
+    extra_fixed_scale_kernel<<<1, 1, 0, stream>>>(fixed_scale, C);
+    SGN_CHECK_LAUNCH("extra_fixed_scale_kernel");
+    extra_kernel<true, true><<<dim3(p.tiles, (C + EXTRA_CG - 1) / EXTRA_CG), 32, 0, stream>>>(q);
+    SGN_CHECK_LAUNCH("extra_kernel<bwd, det>");
+    const long long n = (6 + (long long)C) * num_gaussians;
+    extra_fixed_add_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(q.fx_geom, q.fx_extra, fixed_scale, records, v_records, v_extra,
+                                                                              num_gaussians, C);
+    SGN_CHECK_LAUNCH("extra_fixed_add_kernel");
     return SGN_OK;
 }

@@ -691,7 +691,8 @@ class _SceneGraphRasterize(torch.autograd.Function):
         v_extra = None
         if v_extra_img is not None:  # adds the extra channels' share of the geometry gradients to v_records before project_bwd
             v_extra = blend_extra_bwd(ctx.cs, ctx.bo, ctx.records, ctx.sorted_ids, ctx.tile_bins, ctx.saved["final_T"],
-                                      ctx.saved["final_idx"], ctx.extra, v_extra_img, v_records)
+                                      ctx.saved["final_idx"], ctx.extra, v_extra_img, v_records,
+                                      deterministic=ctx.settings.deterministic)
         h = ctx.holder
         sink = h.grad_sink
         if sink is not None:
@@ -771,15 +772,28 @@ def blend_extra_fwd(cs, bo, records, sorted_ids, tile_bins, final_T, final_idx, 
     return out
 
 
-def blend_extra_bwd(cs, bo, records, sorted_ids, tile_bins, final_T, final_idx, extra, v_out, v_records) -> torch.Tensor:
-    """Returns v_extra[N,C]; adds the geometry part (xy, conic, opacity) to ``v_records`` in place."""
+def blend_extra_bwd(cs, bo, records, sorted_ids, tile_bins, final_T, final_idx, extra, v_out, v_records,
+                    deterministic: Optional[bool] = None) -> torch.Tensor:
+    """Returns v_extra[N,C]; adds the geometry part (xy, conic, opacity) to ``v_records`` in place.  ``deterministic``
+    (default: SGN_DETERMINISTIC): fixed-point accumulation, bit-identical from run to run (sgn_blend_extra_bwd_det)."""
     L = _lib.load()
     v_extra = torch.zeros_like(extra)
     v_out = v_out.contiguous()
+    det = DETERMINISTIC if deterministic is None else deterministic
     with _timed("blend_extra_bwd"):
-        _lib.check(L.sgn_blend_extra_bwd(C.byref(cs), C.byref(bo), _ptr(records), _ptr(sorted_ids), _ptr(tile_bins), _ptr(final_T),
-                                         _ptr(final_idx), _ptr(extra), extra.shape[1], _ptr(v_out), _ptr(v_extra), _ptr(v_records),
-                                         _stream()), "sgn_blend_extra_bwd")
+        if det:
+            N, Cn = extra.shape
+            fx_geom = torch.zeros(N, 6, device=records.device, dtype=torch.int64)
+            fx_extra = torch.zeros(N, Cn, device=records.device, dtype=torch.int64)
+            fx_scale = torch.empty(2, device=records.device, dtype=torch.float32)
+            _lib.check(L.sgn_blend_extra_bwd_det(C.byref(cs), C.byref(bo), _ptr(records), _ptr(sorted_ids), _ptr(tile_bins),
+                                                 _ptr(final_T), _ptr(final_idx), _ptr(extra), Cn, N, _ptr(v_out), _ptr(v_extra),
+                                                 _ptr(v_records), _ptr(fx_geom), _ptr(fx_extra), _ptr(fx_scale), _stream()),
+                       "sgn_blend_extra_bwd_det")
+        else:
+            _lib.check(L.sgn_blend_extra_bwd(C.byref(cs), C.byref(bo), _ptr(records), _ptr(sorted_ids), _ptr(tile_bins), _ptr(final_T),
+                                             _ptr(final_idx), _ptr(extra), extra.shape[1], _ptr(v_out), _ptr(v_extra), _ptr(v_records),
+                                             _stream()), "sgn_blend_extra_bwd")
     return v_extra
 
 

@@ -118,3 +118,106 @@ def test_cases_exercise_what_they_are_built_for():
     assert [ref.strips_for(n, 768) for n in lens[:7]] == [1, 2, 2, 4, 4, 8, 8]
     c = bc.get("large")
     assert c.inp.tile_bins.shape[0] == 120 * 80 and np.diff(c.inp.tile_bins, axis=1).sum() > 5000
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# the channel form (forward_channels / backward_channels): what sgn_blend_extra_* and Level-1 rasterize_gaussians compute
+# ------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("name", ["raw_mode", "lengths"])
+def test_channels_reproduce_the_record_form(name):
+    """values = records[:, 6:10] with the background in raw mode: the channel form is forward()'s rgb / depth and
+    backward()'s columns 0..9, to rounding."""
+    case = bc.get(name)
+    bg = (0.2, 0.4, 0.6, 5.0)
+    opts = ref.Opts(raw_mode=True, class_streams=case.opts.class_streams, background=bg)
+    vals = case.inp.records[:, 6:10]
+    fw = ref.forward(case.inp, opts)
+    ch = ref.forward_channels(case.inp, opts, vals, background=bg)
+    np.testing.assert_allclose(ch["out"][..., :3], fw["rgb"], rtol=0, atol=1e-12)
+    np.testing.assert_allclose(ch["out"][..., 3], fw["depth"], rtol=0, atol=1e-12)
+    np.testing.assert_array_equal(ch["final_idx"], fw["final_idx"][0])
+    np.testing.assert_allclose(ch["final_T"], fw["final_T"][0], rtol=0, atol=1e-12)
+    assert np.all(ch["abs"] >= np.abs(ch["out"]) - 1e-12)
+    cot = bc.cotangents(case, "rand", seed=5)
+    cot = {k: cot[k] for k in ("rgb", "depth", "accumulation")}
+    g, _, _, gabs = ref.backward(case.inp, opts, cot)
+    v_out = np.concatenate([cot["rgb"], cot["depth"][..., None]], -1)
+    vv, vr, vva, vra = ref.backward_channels(case.inp, opts, vals, v_out, v_alpha=cot["accumulation"], background=bg)
+    scale = np.abs(g).max()
+    np.testing.assert_allclose(vv, g[:, 6:10], rtol=0, atol=1e-12 * scale)
+    np.testing.assert_allclose(vr[:, 0:6], g[:, 0:6], rtol=0, atol=1e-12 * scale)
+    assert np.all(vr[:, 6:] == 0)
+    np.testing.assert_allclose(vva, gabs[:, 6:10], rtol=0, atol=1e-12 * scale)
+
+
+def _channels_loss(inp, opts, rec, vals, v_out, v_alpha, bg):
+    fw = ref.forward_channels(ref.Inputs(inp.width, inp.height, rec, inp.sorted_ids, inp.tile_bins, inp.cls_ids, inp.cls_bins),
+                              opts, vals, background=bg)
+    return float((v_out * fw["out"]).sum() + (v_alpha * (1.0 - fw["final_T"])).sum())
+
+
+@pytest.mark.parametrize("shape", [(16, 16, 1, 3), (20, 18, 2, 1), (9, 21, 3, 5)])
+def test_channels_backward_matches_central_differences(shape):
+    w, h, seed, Cn = shape
+    case = bc.tiny(w, h, seed, sky=False)
+    opts = case.opts
+    rng = np.random.default_rng(seed)
+    N = case.inp.records.shape[0]
+    vals = rng.uniform(-2.0, 2.0, (N, Cn))
+    bg = rng.uniform(-1.0, 1.0, Cn)
+    v_out = rng.uniform(-1.0, 1.0, (h, w, Cn))
+    v_alpha = rng.uniform(-1.0, 1.0, (h, w))
+    vv, vr, _, _ = ref.backward_channels(case.inp, opts, vals, v_out, v_alpha=v_alpha, background=bg)
+    rec = case.inp.records.astype(np.float64)
+    loss = lambda r, v: _channels_loss(case.inp, opts, r, v, v_out, v_alpha, bg)
+    worst = 0.0
+    for n in range(N):
+        for col in range(6):
+            hstep = 1e-6 * max(1.0, abs(rec[n, col]))
+            rp, rm = rec.copy(), rec.copy()
+            rp[n, col] += hstep
+            rm[n, col] -= hstep
+            fd = (loss(rp, vals) - loss(rm, vals)) / (2 * hstep)
+            scale = np.abs(vr[:, col]).max() + 1e-12
+            worst = max(worst, abs(fd - vr[n, col]) / (abs(vr[n, col]) + 1e-3 * scale))
+        for c in range(Cn):  # linear in the values: a unit step is exact
+            vp = vals.copy()
+            vp[n, c] += 1.0
+            fd = loss(rec, vp) - loss(rec, vals)
+            worst = max(worst, abs(fd - vv[n, c]) / (abs(vv[n, c]) + 1e-3 * (np.abs(vv).max() + 1e-12)))
+    assert worst < 1e-4, worst
+
+
+def test_channels_match_c_oracle_generic_c():
+    """C = 19 channels on the small_actors lists: the forward against the C oracle's generic-C blend, the backward against
+    its sgn_oracle_blend_bwd (cotangents only on pixels whose decisions are not fragile)."""
+    import ctypes as Cc
+    fr = syn.make_frame(**PARITY_SCENES["small_actors"])
+    orc = oracle_c.Oracle(fr)
+    fw = orc.forward(class_renders=False)
+    N, H, W, Cn = fw.N, fr.camera.height, fr.camera.width, 19
+    rec = np.zeros((N, 12), np.float32)
+    rec[:, 0:2], rec[:, 2:5], rec[:, 5] = fw.xys, fw.conics, fw.opac
+    inp = ref.Inputs(W, H, rec, fw.sorted_ids, fw.tile_bins)
+    opts = ref.Opts(class_streams=False)
+    rng = np.random.default_rng(19)
+    extra = rng.standard_normal((N, Cn)).astype(np.float32)
+    img, _, _, _ = orc.blend(dict(xys=fw.xys, conics=fw.conics, opac=fw.opac), fw.sorted_ids, fw.tile_bins, extra)
+    ch = ref.forward_channels(inp, opts, extra)
+    ok = (fw.fragile == 0) & (ch["margin"] >= 1e-4)
+    assert ok.mean() > 0.95
+    err = np.abs(ch["out"] - img)[ok]
+    assert (err <= 2e-5 * np.maximum(1.0, ch["abs"][ok])).all(), err.max()
+    w = (rng.uniform(0.0, 1.0, (H, W, Cn)) * ok[..., None]).astype(np.float32)
+    vv, vr, vva, vra = ref.backward_channels(inp, opts, extra, w)
+    vc, vxy, vcon, vop = np.zeros((N, Cn)), np.zeros((N, 2)), np.zeros((N, 3)), np.zeros(N)
+    rc = orc.L.sgn_oracle_blend_bwd(
+        Cc.c_int(W), Cc.c_int(H), Cc.c_int(16), Cc.c_int(Cn), oracle_c._p(fw.sorted_ids), oracle_c._p(fw.tile_bins),
+        oracle_c._p(fw.xys), oracle_c._p(fw.conics), oracle_c._p(extra), oracle_c._p(fw.opac),
+        oracle_c._p(np.zeros(Cn, np.float32)), Cc.c_float(0.99), oracle_c._p(orc.cls), Cc.c_int(-1),
+        oracle_c._p(np.ascontiguousarray(fw.final_T)), oracle_c._p(np.ascontiguousarray(fw.final_idx)), oracle_c._p(w),
+        oracle_c._p(np.zeros((H, W), np.float32)), oracle_c._p(vxy), oracle_c._p(vcon), oracle_c._p(vc), oracle_c._p(vop))
+    assert rc == 0
+    for got, want, S in ((vc, vv, vva), (vxy, vr[:, 0:2], vra[:, 0:2]), (vcon, vr[:, 2:5], vra[:, 2:5]), (vop, vr[:, 5], vra[:, 5])):
+        bad = np.abs(got - want) > 1e-5 * np.abs(want) + 1e-5 * S
+        assert not bad.any(), (np.argwhere(bad)[:5].tolist(), np.abs(got - want).max())
