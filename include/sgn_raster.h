@@ -353,8 +353,8 @@ int sgn_ssim_bwd(int H, int W, const sgn_loss_in* in, float weight, const float*
  * directions itself: d = normalize(((x - cx + ju) / fx, (y - cy + jv) / fy, 1)), rotated by c2w[:3,:3] (recovered from
  * cam->viewmat), then l = (d.x, d.z, -d.y); ju = jv = 0.5 in eval (jitter pointers NULL), two [H,W] uniform draws in
  * training.  The backward recomputes the directions from the same jitter.  v_tex is ACCUMULATED into (zero it first); it
- * uses float atomics, so it is not bit-reproducible.  R < 1, a null required pointer, a single jitter array or sizes
- * beyond 32-bit indexing return SGN_ERR_INVALID and launch nothing. */
+ * uses float atomics, so it is not bit-reproducible (the _det entry points below are).  R < 1, a null required pointer, a
+ * single jitter array or sizes beyond 32-bit indexing return SGN_ERR_INVALID and launch nothing. */
 /* sky[H,W,3]; dirs[H,W,3] (the lookup directions l) or NULL */
 int sgn_sky_fwd(const sgn_camera* cam, const float* jitter_u, const float* jitter_v, const float* tex, int R, float* sky, float* dirs,
                 void* stream);
@@ -363,6 +363,16 @@ int sgn_sky_bwd(const sgn_camera* cam, const float* jitter_u, const float* jitte
 /* The same sampler on given directions uv[P,3]: out[P,3]; backward accumulates into v_tex. */
 int sgn_cube_texture_fwd(int P, const float* uv, const float* tex, int R, float* out, void* stream);
 int sgn_cube_texture_bwd(int P, const float* uv, int R, const float* v_out, float* v_tex, void* stream);
+/* Deterministic backward: the same arguments and the same accumulation into v_tex, bit-identical from run to run and
+ * whatever the order of the lookups.  Every addend is rounded once to 64-bit fixed point (2^32 units per unit of
+ * max|v_out|, a power of two) and added as an integer; the sums are then converted and added to v_tex.  scratch: at least
+ * sgn_sky_det_scratch_bytes(R) bytes of device memory, 8-byte aligned (int64 [6,R,R,3] and the grid scale); the library
+ * zeroes it on the stream itself.  A null, misaligned or too small scratch returns SGN_ERR_INVALID and launches nothing. */
+size_t sgn_sky_det_scratch_bytes(int R); /* 0 for an invalid R */
+int sgn_sky_bwd_det(const sgn_camera* cam, const float* jitter_u, const float* jitter_v, int R, const float* v_sky, float* v_tex,
+                    void* scratch, size_t scratch_bytes, void* stream);
+int sgn_cube_texture_bwd_det(int P, const float* uv, int R, const float* v_out, float* v_tex, void* scratch, size_t scratch_bytes,
+                             void* stream);
 
 /* ---- densification statistics (SURVEY.md 8f rank 3) -------------------------------------------------------
  * What each sub-model's `after_train` accumulates after backward (sgn_splatfacto.py:513-541), for all visible

@@ -129,6 +129,7 @@ EXPORTS = [
     "sgn_blend_fwd", "sgn_blend_bwd", "sgn_sizeof_adam_tensor", "sgn_adam_chunk_elems", "sgn_adam_step",
     "sgn_loss_scratch_bytes", "sgn_loss_fwd", "sgn_loss_bwd", "sgn_ssim_workspace_bytes", "sgn_ssim_fwd", "sgn_ssim_bwd",
     "sgn_sky_fwd", "sgn_sky_bwd", "sgn_cube_texture_fwd", "sgn_cube_texture_bwd",
+    "sgn_sky_det_scratch_bytes", "sgn_sky_bwd_det", "sgn_cube_texture_bwd_det",
     "sgn_sizeof_densify_segment", "sgn_densify_stats",
     "sgn_sizeof_refine_config", "sgn_sizeof_refine_tensors", "sgn_refine_decide", "sgn_refine_apply",
     "sgn_bin_local_cap", "sgn_bin_local_scratch_bytes", "sgn_bin_local_count", "sgn_bin_local_sort",
@@ -222,7 +223,11 @@ def load():
     L.sgn_sky_bwd.argtypes = [C.POINTER(CameraStruct), vp, vp, i32, vp, vp, vp]
     L.sgn_cube_texture_fwd.argtypes = [i32, vp, vp, i32, vp, vp]
     L.sgn_cube_texture_bwd.argtypes = [i32, vp, i32, vp, vp, vp]
-    for f in ("sgn_sky_fwd", "sgn_sky_bwd", "sgn_cube_texture_fwd", "sgn_cube_texture_bwd"):
+    L.sgn_sky_det_scratch_bytes.argtypes = [i32]
+    L.sgn_sky_det_scratch_bytes.restype = sz
+    L.sgn_sky_bwd_det.argtypes = [C.POINTER(CameraStruct), vp, vp, i32, vp, vp, vp, sz, vp]
+    L.sgn_cube_texture_bwd_det.argtypes = [i32, vp, i32, vp, vp, vp, sz, vp]
+    for f in ("sgn_sky_fwd", "sgn_sky_bwd", "sgn_cube_texture_fwd", "sgn_cube_texture_bwd", "sgn_sky_bwd_det", "sgn_cube_texture_bwd_det"):
         getattr(L, f).restype = C.c_int
     L.sgn_sizeof_adam_tensor.restype = sz
     L.sgn_adam_chunk_elems.restype = C.c_int

@@ -27,6 +27,7 @@
 //
 // Sorted payloads carry the Gaussian row in bits 0-30 and the object-class flag in bit 31.
 #include "sgn_common.cuh"
+#include "sgn_fixed.cuh"
 
 #include <type_traits>
 
@@ -1432,24 +1433,7 @@ __global__ void __launch_bounds__(32, BLEND_ACC_MIN_BLOCKS) acc_bwd_kernel(const
     }
 }
 
-// ---- deterministic mode helpers: scale = 2^32 / max |cotangent| (gradients are linear in the cotangents: the fixed-point
-// grid adapts to their magnitude; 2^31 of headroom above it, and the conic components of large Gaussians give up more
-// places, fixed_shift), then fixed point -> float
-__global__ void __launch_bounds__(256)
-cot_max_kernel(const float* __restrict__ a, long long n, unsigned* __restrict__ out_bits) {
-    float m = 0.f;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-        const float v = fabsf(a[i]);
-        m = (v == v && v < 3.0e38f) ? fmaxf(m, v) : m;
-    }
-    m = fmaxf(m, __shfl_xor_sync(FULL, m, 16)); m = fmaxf(m, __shfl_xor_sync(FULL, m, 8)); m = fmaxf(m, __shfl_xor_sync(FULL, m, 4));
-    m = fmaxf(m, __shfl_xor_sync(FULL, m, 2)); m = fmaxf(m, __shfl_xor_sync(FULL, m, 1));
-    if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(out_bits, __float_as_uint(m));  // non-negative floats order like their bits
-}
-__global__ void fixed_scale_kernel(float* scale) {
-    const float m = scale[0];  // the bits cot_max_kernel left are the float itself
-    scale[0] = m > 0.f ? exp2f(32.f - ceilf(log2f(m))) : 4294967296.f;  // a power of two: scaling is exact
-}
+// ---- deterministic mode: the grid comes from cot_max_kernel + fixed_scale_kernel (sgn_fixed.cuh), then fixed point -> float
 __global__ void __launch_bounds__(256)
 fixed_to_float_kernel(const long long* __restrict__ fx, const float* __restrict__ scale, const float* __restrict__ records,
                       float* __restrict__ out, long long n) {

@@ -24,15 +24,34 @@
 // Backward: a CTA owns a 32 x 32 pixel tile (each thread four rows).  It reduces the texel box its in-face lookups touch on
 // the face of the tile's first pixel; when that box fits in shared memory the contributions are accumulated there and
 // each touched texel is flushed with one global RED.  Contributions of other faces, wrapped edges and corners, or of a
-// tile whose box is too large, go straight to global REDs.  Float atomics: the gradient is not bit-reproducible.
+// tile whose box is too large, go straight to global REDs.  Float atomics: this gradient is not bit-reproducible.
+//
+// Deterministic backward (sgn_sky_bwd_det / sgn_cube_texture_bwd_det, cube_bwd_kernel<CAM, true>): the same tiles and
+// boxes, but every addend is rounded once to 64-bit fixed point and added as an integer, in the shared box and on the
+// global path alike.  Integer addition is associative, so the sums are bit-identical whatever the order in which blocks,
+// warps and atomics run; one conversion kernel then adds them to v_tex.  The grid is 2^32 units per unit of max|v_out|
+// (cot_max_kernel + fixed_scale_kernel, sgn_fixed.cuh: a power of two, so scaling an addend is exact).  A lookup gives a
+// texel at most one addend (its taps are four distinct texels, the missing corner tap's share folded into the other three),
+// of |w v| <= 4/3 max|v_out|, i.e. at most 4/3 2^32 units; an int64 holds 2^30 such addends, while a camera of 32-bit
+// indexable size has fewer than 2^30 pixels (1920 x 1280: 2^21.2) and a uv array fewer than 2^29.5 lookups (3 P <= INT_MAX).
+// So, unlike the blend's conic components, no texel needs a coarser grid.  Halving the box capacity keeps the int64 box at
+// the float box's 24 KB of static shared memory.
 #include <limits.h>
 
+#include <type_traits>
+
 #include "sgn_common.cuh"
+#include "sgn_fixed.cuh"
 
 #define SKY_THREADS 256
 #define SKY_TILE 32                                   // backward tile: 32 x 32 pixels (camera) or 1024 items (uv array)
 #define SKY_ITEMS (SKY_TILE * SKY_TILE / SKY_THREADS) // items per thread in the backward
 #define SKY_BOX_TEXELS 2048                           // shared-memory box capacity (x 3 channels: 24 KB)
+#define SKY_DET_BOX_TEXELS 1024                       // the deterministic backward's int64 box (x 3 channels: 24 KB)
+
+// gradient accumulator of the backward: float (atomics in any order) or fixed point (deterministic)
+template <bool DET>
+using SkyAcc = typename std::conditional<DET, unsigned long long, float>::type;
 
 // face basis (N, U, V) of faces 0..5 = +x, -x, +y, -y, +z, -z: direction = N + a U + b V with a = 2s - 1, b = 2t - 1
 __constant__ int8_t kCubeBasis[6][3][3] = {
@@ -169,6 +188,20 @@ static __device__ __forceinline__ void quad_weights(const Quad& q, float w[4]) {
     w[0] = 1.f - q.fu - w[2];
 }
 
+// the same weights with every operation rounded on its own (no contraction): the deterministic backward forms each
+// addend by one fixed sequence of roundings wherever the lookup is accumulated (shared box or global path)
+static __device__ __forceinline__ void quad_weights_rn(const Quad& q, float w[4]) {
+    w[3] = __fmul_rn(q.fu, q.fv);
+    w[2] = __fsub_rn(q.fv, w[3]);
+    w[1] = __fsub_rn(q.fu, w[3]);
+    w[0] = __fsub_rn(__fsub_rn(1.f, q.fu), w[2]);
+}
+
+// an addend on the fixed-point grid: the scale is a power of two (the product is exact), then one rounding to an integer
+static __device__ __forceinline__ unsigned long long to_fixed(float a, float fscale) {
+    return (unsigned long long)__float2ll_rn(__fmul_rn(a, fscale));
+}
+
 // every tap of the lookup straight to global memory, with the corner rule
 static __device__ __forceinline__ void quad_red_global(const Quad& q, const float vy[3], float* __restrict__ v_tex) {
     float w[4];
@@ -186,6 +219,28 @@ static __device__ __forceinline__ void quad_red_global(const Quad& q, const floa
 #pragma unroll
         for (int k = 0; k < 4; ++k)
             if (q.idx[k] >= 0) atomicAdd(v_tex + 3 * q.idx[k] + ch, corner ? cw[k] + cb : cw[k]);
+    }
+}
+
+// the deterministic form: the same addends w v and, at a corner, w v + (w_missing v) kThird, each rounded on its own and
+// then once to fixed point
+static __device__ __forceinline__ void quad_red_global(const Quad& q, const float vy[3], unsigned long long* __restrict__ v_fx,
+                                                       float fscale) {
+    float w[4];
+    quad_weights_rn(q, w);
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+        float cw[4], cb = 0.f;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            cw[k] = __fmul_rn(w[k], vy[ch]);
+            if (q.idx[k] < 0) cb = cw[k];
+        }
+        const bool corner = quad_corner(q);
+        if (corner) cb = __fmul_rn(cb, kThird);
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+            if (q.idx[k] >= 0) atomicAdd(v_fx + 3 * q.idx[k] + ch, to_fixed(corner ? __fadd_rn(cw[k], cb) : cw[k], fscale));
     }
 }
 
@@ -232,12 +287,17 @@ __global__ void __launch_bounds__(SKY_THREADS) cube_fwd_kernel(const SkyCam c, c
     out[3 * p + 2] = o[2];
 }
 
-template <bool CAM>
+// DET = false: float atomics into v_tex.  DET = true: v_tex is the fixed-point scratch, int64 [6,R,R,3] followed by the
+// grid scale (one float), and the box holds int64 (SKY_DET_BOX_TEXELS).  The float instantiations carry no fixed-point code.
+template <bool CAM, bool DET>
 __global__ void __launch_bounds__(SKY_THREADS) cube_bwd_kernel(const SkyCam c, const float* __restrict__ ju, const float* __restrict__ jv,
                                                                const float* __restrict__ uv, int P, int R, const float* __restrict__ v_out,
-                                                               float* __restrict__ v_tex) {
-    __shared__ float box[SKY_BOX_TEXELS * 3];
+                                                               SkyAcc<DET>* __restrict__ v_tex) {
+    constexpr int BOX_TEXELS = DET ? SKY_DET_BOX_TEXELS : SKY_BOX_TEXELS;
+    __shared__ SkyAcc<DET> box[BOX_TEXELS * 3];
     __shared__ int s_dom, s_lo[2], s_hi[2];
+    float fscale = 0.f;
+    if constexpr (DET) fscale = __ldg(reinterpret_cast<const float*>(v_tex + 18LL * R * R));
     const int tid = threadIdx.x;
     if (tid == 0) {
         s_dom = -1;
@@ -288,9 +348,9 @@ __global__ void __launch_bounds__(SKY_THREADS) cube_bwd_kernel(const SkyCam c, c
     const int bi0 = s_lo[0], bj0 = s_lo[1];
     const bool some = dom >= 0 && s_hi[0] >= bi0;  // block-uniform: some lookup lies on the privatised face
     const int bw = some ? s_hi[0] - bi0 + 2 : 0, bh = some ? s_hi[1] - bj0 + 2 : 0;  // a quad spans two texels per axis
-    const bool priv = some && bw * bh <= SKY_BOX_TEXELS;
+    const bool priv = some && bw * bh <= BOX_TEXELS;
     if (priv) {
-        for (int e = tid; e < bw * bh * 3; e += SKY_THREADS) box[e] = 0.f;
+        for (int e = tid; e < bw * bh * 3; e += SKY_THREADS) box[e] = 0;
         __syncthreads();
     }
 #pragma unroll
@@ -300,25 +360,39 @@ __global__ void __launch_bounds__(SKY_THREADS) cube_bwd_kernel(const SkyCam c, c
         const float vy[3] = {v_out[3 * p], v_out[3 * p + 1], v_out[3 * p + 2]};
         if (vy[0] == 0.f && vy[1] == 0.f && vy[2] == 0.f) continue;
         if (priv && q[k].own_face == dom) {
-            float w[4];
-            quad_weights(q[k], w);
-            float* b = box + 3 * ((q[k].j0 - bj0) * bw + (q[k].i0 - bi0));
+            if constexpr (DET) {
+                float w[4];
+                quad_weights_rn(q[k], w);
+                unsigned long long* b = box + 3 * ((q[k].j0 - bj0) * bw + (q[k].i0 - bi0));
 #pragma unroll
-            for (int ch = 0; ch < 3; ++ch) {
-                atomicAdd(b + ch, w[0] * vy[ch]);
-                atomicAdd(b + 3 + ch, w[1] * vy[ch]);
-                atomicAdd(b + 3 * bw + ch, w[2] * vy[ch]);
-                atomicAdd(b + 3 * bw + 3 + ch, w[3] * vy[ch]);
+                for (int ch = 0; ch < 3; ++ch) {
+                    atomicAdd(b + ch, to_fixed(__fmul_rn(w[0], vy[ch]), fscale));
+                    atomicAdd(b + 3 + ch, to_fixed(__fmul_rn(w[1], vy[ch]), fscale));
+                    atomicAdd(b + 3 * bw + ch, to_fixed(__fmul_rn(w[2], vy[ch]), fscale));
+                    atomicAdd(b + 3 * bw + 3 + ch, to_fixed(__fmul_rn(w[3], vy[ch]), fscale));
+                }
+            } else {
+                float w[4];
+                quad_weights(q[k], w);
+                float* b = box + 3 * ((q[k].j0 - bj0) * bw + (q[k].i0 - bi0));
+#pragma unroll
+                for (int ch = 0; ch < 3; ++ch) {
+                    atomicAdd(b + ch, w[0] * vy[ch]);
+                    atomicAdd(b + 3 + ch, w[1] * vy[ch]);
+                    atomicAdd(b + 3 * bw + ch, w[2] * vy[ch]);
+                    atomicAdd(b + 3 * bw + 3 + ch, w[3] * vy[ch]);
+                }
             }
         } else {
-            quad_red_global(q[k], vy, v_tex);
+            if constexpr (DET) quad_red_global(q[k], vy, v_tex, fscale);
+            else quad_red_global(q[k], vy, v_tex);
         }
     }
     if (priv) {
         __syncthreads();
         for (int e = tid; e < bw * bh * 3; e += SKY_THREADS) {
-            const float g = box[e];
-            if (g != 0.f) {
+            const SkyAcc<DET> g = box[e];
+            if (g != 0) {
                 const int t = e / 3, ch = e - 3 * t;
                 const int jj = t / bw, ii = t - jj * bw;
                 atomicAdd(v_tex + 3 * ((dom * R + bj0 + jj) * R + bi0 + ii) + ch, g);
@@ -379,9 +453,60 @@ extern "C" int sgn_sky_bwd(const sgn_camera* cam, const float* jitter_u, const f
     if (int rc = check_jitter(jitter_u, jitter_v, "sgn_sky_bwd")) return rc;
     SGN_REQUIRE(v_sky && v_tex, "sgn_sky_bwd: null v_sky or v_tex");
     const dim3 grid((c.W + SKY_TILE - 1) / SKY_TILE, (c.H + SKY_TILE - 1) / SKY_TILE);
-    cube_bwd_kernel<true><<<grid, SKY_THREADS, 0, (cudaStream_t)stream>>>(c, jitter_u, jitter_v, nullptr, c.W * c.H, R, v_sky, v_tex);
+    cube_bwd_kernel<true, false><<<grid, SKY_THREADS, 0, (cudaStream_t)stream>>>(c, jitter_u, jitter_v, nullptr, c.W * c.H, R, v_sky, v_tex);
     SGN_CHECK_LAUNCH("cube_bwd_kernel<camera>");
     return SGN_OK;
+}
+
+// ---- deterministic backward: zero the scratch, the grid from max|v_out|, the kernel into the int64 sums, then v_tex += sums
+__global__ void __launch_bounds__(256)
+sky_fixed_add_kernel(const long long* __restrict__ fx, const float* __restrict__ scale, float* __restrict__ v_tex, long long n) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) v_tex[i] += (float)((double)fx[i] / (double)scale[0]);
+}
+
+extern "C" size_t sgn_sky_det_scratch_bytes(int R) {
+    if (R < 1 || 18LL * R * R > INT_MAX) return 0;
+    return (size_t)18 * R * R * sizeof(long long) + 16;  // the int64 sums, then the grid scale (one float, padded)
+}
+
+static int check_det_scratch(const void* scratch, size_t scratch_bytes, int R, const char* who) {
+    SGN_REQUIRE(scratch, "%s: null scratch", who);
+    SGN_REQUIRE((reinterpret_cast<uintptr_t>(scratch) & 7) == 0, "%s: scratch must be 8-byte aligned", who);
+    const size_t need = sgn_sky_det_scratch_bytes(R);
+    SGN_REQUIRE(scratch_bytes >= need, "%s: scratch of %zu bytes, sgn_sky_det_scratch_bytes(%d) = %zu", who, scratch_bytes, R, need);
+    return SGN_OK;
+}
+
+template <bool CAM>
+static int launch_bwd_det(const SkyCam& c, const float* ju, const float* jv, const float* uv, int P, int R, const float* v_out,
+                          float* v_tex, void* scratch, dim3 grid, cudaStream_t stream) {
+    const long long n = 18LL * R * R;
+    unsigned long long* fx = reinterpret_cast<unsigned long long*>(scratch);
+    float* scale = reinterpret_cast<float*>(fx + n);
+    SGN_CHECK_CUDA(cudaMemsetAsync(scratch, 0, (size_t)n * sizeof(long long) + sizeof(float), stream));
+    cot_max_kernel<<<296, 256, 0, stream>>>(v_out, 3LL * P, reinterpret_cast<unsigned*>(scale));
+    SGN_CHECK_LAUNCH("cot_max_kernel");
+    fixed_scale_kernel<<<1, 1, 0, stream>>>(scale);
+    SGN_CHECK_LAUNCH("fixed_scale_kernel");
+    cube_bwd_kernel<CAM, true><<<grid, SKY_THREADS, 0, stream>>>(c, ju, jv, uv, P, R, v_out, fx);
+    SGN_CHECK_LAUNCH(CAM ? "cube_bwd_kernel<camera, det>" : "cube_bwd_kernel<uv, det>");
+    sky_fixed_add_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const long long*>(fx), scale, v_tex, n);
+    SGN_CHECK_LAUNCH("sky_fixed_add_kernel");
+    return SGN_OK;
+}
+
+extern "C" int sgn_sky_bwd_det(const sgn_camera* cam, const float* jitter_u, const float* jitter_v, int R, const float* v_sky, float* v_tex,
+                               void* scratch, size_t scratch_bytes, void* stream) {
+    SGN_RANGE("sgn_sky_bwd_det");
+    SkyCam c;
+    if (int rc = sky_cam(c, cam, "sgn_sky_bwd_det")) return rc;
+    if (int rc = check_res(R, "sgn_sky_bwd_det")) return rc;
+    if (int rc = check_jitter(jitter_u, jitter_v, "sgn_sky_bwd_det")) return rc;
+    SGN_REQUIRE(v_sky && v_tex, "sgn_sky_bwd_det: null v_sky or v_tex");
+    if (int rc = check_det_scratch(scratch, scratch_bytes, R, "sgn_sky_bwd_det")) return rc;
+    const dim3 grid((c.W + SKY_TILE - 1) / SKY_TILE, (c.H + SKY_TILE - 1) / SKY_TILE);
+    return launch_bwd_det<true>(c, jitter_u, jitter_v, nullptr, c.W * c.H, R, v_sky, v_tex, scratch, grid, (cudaStream_t)stream);
 }
 
 static int check_items(int P, const char* who) {
@@ -410,7 +535,20 @@ extern "C" int sgn_cube_texture_bwd(int P, const float* uv, int R, const float* 
     if (P == 0) return SGN_OK;
     const SkyCam c{};
     const int tile = SKY_TILE * SKY_TILE;
-    cube_bwd_kernel<false><<<(P + tile - 1) / tile, SKY_THREADS, 0, (cudaStream_t)stream>>>(c, nullptr, nullptr, uv, P, R, v_out, v_tex);
+    cube_bwd_kernel<false, false><<<(P + tile - 1) / tile, SKY_THREADS, 0, (cudaStream_t)stream>>>(c, nullptr, nullptr, uv, P, R, v_out, v_tex);
     SGN_CHECK_LAUNCH("cube_bwd_kernel<uv>");
     return SGN_OK;
+}
+
+extern "C" int sgn_cube_texture_bwd_det(int P, const float* uv, int R, const float* v_out, float* v_tex, void* scratch, size_t scratch_bytes,
+                                        void* stream) {
+    SGN_RANGE("sgn_cube_texture_bwd_det");
+    if (int rc = check_items(P, "sgn_cube_texture_bwd_det")) return rc;
+    if (int rc = check_res(R, "sgn_cube_texture_bwd_det")) return rc;
+    SGN_REQUIRE(uv && v_out && v_tex, "sgn_cube_texture_bwd_det: null uv, v_out or v_tex");
+    if (int rc = check_det_scratch(scratch, scratch_bytes, R, "sgn_cube_texture_bwd_det")) return rc;
+    if (P == 0) return SGN_OK;
+    const SkyCam c{};
+    const int tile = SKY_TILE * SKY_TILE;
+    return launch_bwd_det<false>(c, nullptr, nullptr, uv, P, R, v_out, v_tex, scratch, dim3((P + tile - 1) / tile), (cudaStream_t)stream);
 }
