@@ -347,6 +347,22 @@ int sgn_ssim_fwd(int H, int W, const sgn_loss_in* in, float weight, float* loss,
 int sgn_ssim_bwd(int H, int W, const sgn_loss_in* in, float weight, const float* grad_loss, const void* workspace, float* v_rgb,
                  void* stream);
 
+/* ---- per-step metrics (get_metrics_dict, sgn_splatfacto.py:1015-1040; eval psnr of :1109-1187) ---------------
+ * One HBM-bound pass over the image and the frame's parameters, through the device segment table of sgn_project_fwd (no copy):
+ *   out[0] psnr            = 10 log10(1 / mean((gt*mask - rgb*mask)^2)) over H*W*3 (torchmetrics PeakSignalNoiseRatio,
+ *                            data_range 1); +inf for equal images.  Uses image->rgb, image->gt_u8 | image->gt_f32, image->mask;
+ *                            image == NULL or image->rgb == NULL: no psnr (NaN).
+ *   out[1] scale_mean      = mean(exp(scales)) over the N rows of the table x 3
+ *   out[2] log_scale_mean  = mean(scales)
+ *   out[3] sigmoid_opacity = mean(sigmoid(opacities))   (table_dev == NULL: out[1..3] are NaN)
+ *   out[4] radii_mean      = mean(radii[0..N))          (radii == NULL: NaN)
+ * Sums in fp64 in a fixed order (bit-identical run to run), results rounded once to fp32; means over zero rows are NaN.  No
+ * host synchronisation.  A null table with nseg > 0, both or neither gt pointer with rgb, a null out / scratch (SGN_ERR_INVALID)
+ * or a short scratch (SGN_ERR_WORKSPACE) launch nothing. */
+size_t sgn_metrics_scratch_bytes(void);
+int sgn_metrics(int H, int W, const sgn_loss_in* image, const sgn_segment* table_dev, int nseg, int N, int num_chunks,
+                const int32_t* radii, float* out, void* scratch, size_t scratch_bytes, void* stream);
+
 /* ---- sky cube map (EnvLight, sgn_splatfacto.py:109-150; use_sky_sphere = True) ------------------------------
  * nvdiffrast dr.texture(tex[None], l, filter_mode='linear', boundary_mode='cube') on a learnable [6,R,R,3] map, and its
  * gradient for the map (no gradient for the directions).  The camera path generates the reference's per-pixel world

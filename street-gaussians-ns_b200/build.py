@@ -24,6 +24,7 @@ SOURCES = {
     "blend.cu": ["--use_fast_math"],
     "loss.cu": [],
     "ssim.cu": [],  # IEEE divisions (no fast math); contraction allowed
+    "metrics.cu": [],  # IEEE expf / division; the squared differences use explicit _rn intrinsics
     "sky.cu": [],  # IEEE divisions / square root and denormals, as the directions and the sampler it stands in for use
     "densify.cu": ["--fmad=false"],
     "adam.cu": ["--fmad=false"],  # keep torch.optim.Adam's rounding sequence (no contraction)

@@ -2,7 +2,8 @@
 (street_gaussians_ns/sgn_splatfacto.py:1042-1094, sgn_splatfacto_scene_graph.py:376-391) that re-read the
 rasterizer's outputs -- L1, sky accumulation, object-accumulation entropy -- as two HBM-bound kernels of
 libsgn_raster.so (forward sums, backward cotangents) behind one autograd node; and the SSIM term
-(sgn_splatfacto.py:1085-1087) as its own forward / backward pair (csrc/ssim.cu) behind a second one."""
+(sgn_splatfacto.py:1085-1087) as its own forward / backward pair (csrc/ssim.cu) behind a second one.  The per-step metrics
+of ``get_metrics_dict`` (sgn_splatfacto.py:1015-1040) are one reduction kernel (csrc/metrics.cu, ``fused_metrics``)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -122,3 +123,44 @@ def fused_ssim_loss(rgb: torch.Tensor, gt: torch.Tensor, mask: Optional[torch.Te
     if float(weight) == 0.0:
         return torch.zeros((), device=rgb.device)
     return _FusedSSIM.apply(rgb, gt, mask, float(weight))
+
+
+METRIC_NAMES = ("psnr", "scale_mean", "log_scale_mean", "sigmoid_opacity", "radii_mean")
+
+
+def fused_metrics(rgb: Optional[torch.Tensor] = None, gt: Optional[torch.Tensor] = None, mask: Optional[torch.Tensor] = None,
+                  table=None, radii: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The per-step metrics of the reference's ``get_metrics_dict`` (sgn_splatfacto.py:1015-1040) from one ``sgn_metrics``
+    call (csrc/metrics.cu): a float32 device tensor [5] = ``METRIC_NAMES``.
+
+    * psnr: ``10 log10(1 / mean((gt*mask - rgb*mask)^2))`` over H*W*3 (torchmetrics PeakSignalNoiseRatio, data_range 1), +inf
+      for equal images; ``rgb`` [H,W,3] float32, ``gt`` [H,W,3] float32 or uint8 (gt/255), ``mask`` [H,W,1] or None.
+    * scale_mean, log_scale_mean, sigmoid_opacity: means of exp(scales), scales and sigmoid(opacities) over the rows of
+      ``table`` (a ``raster.SegmentTable`` with its device rows: the frame's visible sub-models, read in place).
+    * radii_mean: mean of ``radii`` [N] int32.
+    A term without its inputs is NaN, as is a mean over zero rows.  Nothing is read back to the host."""
+    L = _lib.load()
+    ref = rgb if rgb is not None else radii
+    dev = ref.device if ref is not None else table.dev.device
+    if dev.type != "cuda":
+        raise _lib.SgnError("the fused metrics have no CPU path")
+    li, keep, H, W = None, [], 0, 0
+    if rgb is not None:
+        H, W = rgb.shape[0], rgb.shape[1]
+        li, keep = _loss_in(rgb, gt, mask, None, None, None, (0.0, 0.0, 0.0))
+    if radii is not None:
+        assert radii.dtype == torch.int32
+        radii = radii.contiguous()
+    tab, nseg, N, chunks = None, 0, 0, 0
+    if table is not None:
+        tab, nseg, N, chunks = table.dev, table.nseg, table.N, table.num_chunks
+    elif radii is not None:
+        N = radii.shape[0]
+    if radii is not None:
+        assert radii.shape[0] == N, "radii must have one entry per row of the table"
+    out = torch.empty(5, device=dev, dtype=torch.float32)
+    sb = L.sgn_metrics_scratch_bytes()
+    scratch = torch.empty(sb, device=dev, dtype=torch.uint8)
+    _lib.check(L.sgn_metrics(H, W, C.byref(li) if li is not None else None, _ptr(tab), nseg, N, chunks, _ptr(radii), _ptr(out),
+                             _ptr(scratch), sb, _stream()), "sgn_metrics")
+    return out

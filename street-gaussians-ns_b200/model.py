@@ -11,7 +11,9 @@ parts of ``SplatfactoModel`` it inherits (street_gaussians_ns/sgn_splatfacto.py:
   * side-effect attributes ``xys`` (with ``.grad`` = pixel-space mean gradient after backward),
     ``depths, radii, conics, num_tiles_hit, last_size`` on the model and split per sub-model
     (``SplatfactoModel.after_train`` reads ``self.xys.grad`` and ``self.radii``, :513-541);
-  * ``get_loss_dict`` (L1 + SSIM + sky accumulation + object-accumulation entropy).
+  * ``get_loss_dict`` (L1 + SSIM + sky accumulation + object-accumulation entropy);
+  * ``get_metrics_dict`` (per-step psnr, Gaussian count, scale / opacity / radii means: one reduction kernel),
+    ``get_image_metrics_and_images`` and ``get_outputs_for_camera`` (eval).
 
 nerfstudio is not a dependency here: ``camera`` is any object with the fields of
 ``street_gaussians_ns_b200.scene.Camera`` (SURVEY.md 8b lists what the path reads from ``Cameras``).
@@ -320,6 +322,9 @@ class SceneGraphRasterModel(torch.nn.Module):
         self.__dict__["_serial"] = next(_MODEL_SERIAL)  # names this model in raster's static segment-table cache (ids are recycled)
         self._grad_sink = _FullArenaSink() if self.config.full_gradient_arena else _GradSink()
         self._anchor = None
+        # eval's LPIPS (torchmetrics LearnedPerceptualImagePatchSimilarity(normalize=True), sgn_splatfacto.py:331): its AlexNet
+        # weights are not part of this library; an integration that has them sets a callable (gt, rgb) -> score here
+        self.lpips = None
 
     @staticmethod
     def get_object_model_name(object_id) -> str:
@@ -776,6 +781,89 @@ class SceneGraphRasterModel(torch.nn.Module):
                 losses["object_acc_entropy_loss"] = c.object_acc_entropy_loss_mult * -(
                     oa * torch.log(oa) + (1.0 - oa) * torch.log(1.0 - oa)).mean()
         return losses
+
+    def _fused_metrics_ok(self, rgb: torch.Tensor) -> bool:
+        return self.config.fused_loss and rgb.is_cuda
+
+    def get_metrics_dict(self, outputs, batch) -> Dict[str, object]:
+        """``SplatfactoModel.get_metrics_dict`` as the scene graph inherits it (sgn_splatfacto.py:1015-1040; num_downscales = 0):
+        psnr of ``outputs["rgb"]`` against ``batch["image"]`` (no mask), ``gaussian_count`` (host int: rows of the visible
+        sub-models), the scene graph's own refine counters (always empty: refinement runs on the sub-models), then the means of
+        exp(scales), scales, sigmoid(opacities) and radii over the visible rows, under the reference's key names.
+
+        Fused path: the five values are 0-d device tensors of ONE ``sgn_metrics`` launch that reads the parameters through the
+        frame's device segment table -- no concatenation, no read-back.  ``fused_loss=False`` or CPU tensors: the reference's
+        torch expressions over ``torch.cat`` of the visible sub-models."""
+        rgb, gt = outputs["rgb"], batch["image"]
+        h = self._holder
+        d: Dict[str, object] = {}
+        if self._fused_metrics_ok(rgb) and h is not None and h.table is not None:
+            from .loss import fused_metrics
+            psnr, scale_mean, log_scale_mean, sig, radii_mean = fused_metrics(rgb, gt, table=h.table, radii=h.radii).unbind()
+            d["psnr"] = psnr
+            d["gaussian_count"] = int(h.table.N)
+        else:
+            visible = [self.all_models._modules[n] for n in self.visible_model_names]
+            with torch.no_grad():
+                g = gt.float() / 255.0 if gt.dtype == torch.uint8 else gt
+                d["psnr"] = _psnr(rgb.detach(), g)
+                d["gaussian_count"] = sum(sub.num_points for sub in visible)
+                scales = torch.cat([sub.gauss_params["scales"] for sub in visible])
+                opacities = torch.cat([sub.gauss_params["opacities"] for sub in visible])
+                scale_mean, log_scale_mean = torch.exp(scales).mean(), scales.mean()
+                sig = torch.sigmoid(opacities).mean()
+                radii_mean = self.radii.float().mean()
+        d["scale_mean"] = scale_mean
+        d["log_scale_mean"] = log_scale_mean
+        d["sigmoid_opacity"] = sig
+        d["self.radii"] = radii_mean  # sic: the reference's key
+        return d
+
+    def get_image_metrics_and_images(self, outputs, batch):
+        """``SplatfactoModel.get_image_metrics_and_images`` (sgn_splatfacto.py:1109-1187; num_downscales = 0).
+
+        Metrics (Python floats): ``psnr`` and ``ssim`` of gt*mask against rgb*mask (no mask: the images as they are), and
+        ``lpips`` when ``self.lpips`` is a callable (it receives the masked [1,3,H,W] gt and rgb, in that order).  Fused path:
+        psnr from ``sgn_metrics``, ssim = 1 - the SSIM loss kernel at weight 1.  Images: ``img`` = cat([gt, rgb], dim=1), built
+        before masking as the reference does; ``accumulation`` and ``depth`` as the model's [H,W,1] maps, not colour-mapped.
+        Unlike the reference, ``outputs["rgb"]`` and ``batch["image"]`` are not multiplied by the mask in place."""
+        rgb, gt = outputs["rgb"], batch["image"]
+        gt_f = gt.float() / 255.0 if gt.dtype == torch.uint8 else gt
+        mask = batch.get("mask")
+        if mask is not None:
+            mask = mask.to(rgb.device).float()
+        with torch.no_grad():
+            img = torch.cat([gt_f, rgb], dim=1)
+            masked = None
+            if self._fused_metrics_ok(rgb):
+                from .loss import fused_metrics, fused_ssim_loss
+                psnr = fused_metrics(rgb, gt, mask)[0]
+                ssim_v = 1.0 - fused_ssim_loss(rgb, gt, mask, weight=1.0)
+            else:
+                masked = (gt_f * mask, rgb * mask) if mask is not None else (gt_f, rgb)
+                psnr = _psnr(masked[1], masked[0])
+                ssim_v = ssim(masked[0].permute(2, 0, 1)[None], masked[1].permute(2, 0, 1)[None])
+            metrics = {"psnr": float(psnr.item()), "ssim": float(ssim_v)}
+            if callable(self.lpips):
+                if masked is None:
+                    masked = (gt_f * mask, rgb * mask) if mask is not None else (gt_f, rgb)
+                metrics["lpips"] = float(self.lpips(torch.moveaxis(masked[0], -1, 0)[None], torch.moveaxis(masked[1], -1, 0)[None]))
+        images = {"img": img, "accumulation": outputs["accumulation"], "depth": outputs["depth"]}
+        return metrics, images
+
+    def get_outputs_for_camera(self, camera: Camera, obb_box=None) -> Dict[str, torch.Tensor]:
+        """``SplatfactoModel.get_outputs_for_camera`` (sgn_splatfacto.py:1096-1107): ``get_outputs`` under ``no_grad``.  The
+        scene graph supports no crop box outside training (scene graph :361): a box raises."""
+        if obb_box is not None:
+            raise ValueError("crop boxes are not supported by the scene-graph model")
+        with torch.no_grad():
+            return self.get_outputs(camera)
+
+
+def _psnr(preds: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
+    """torchmetrics PeakSignalNoiseRatio(data_range=1.0) on one pair: 10 log10(1 / mean((preds - target)^2)), +inf when equal."""
+    mse = torch.sum((preds - target) ** 2) / target.numel()
+    return 10.0 * torch.log10(1.0 / mse)
 
 
 class _NoOptimizer:

@@ -620,6 +620,7 @@ class _Holder:
         self.v_sky = None
         self.M = 0
         self.tile_bins = self.tile_depth = None
+        self.table = None  # the frame's SegmentTable: its device rows are what sgn_metrics reads the parameters through
         self.post_backward = None
         # model path: an object with target(static) -> arena-or-None and publish(arena, static); the parameter
         # gradients are then delivered through it instead of through 6 x segments autograd leaves
@@ -660,6 +661,7 @@ class _SceneGraphRasterize(torch.autograd.Function):
         out = blend_fwd(cs, bo, records, sorted_ids, tile_bins, sky, obj_ids, obj_bins)
         holder.records, holder.radii, holder.num_tiles_hit, holder.M = records, radii, tiles_hit, M
         holder.xys, holder.conics, holder.depths = records[:, 0:2], records[:, 2:5], records[:, 9]
+        holder.table = table
         ctx.frame, ctx.settings, ctx.holder = frame, settings, holder
         ctx.cs, ctx.bo, ctx.table, ctx.params = cs, bo, table, params
         ctx.saved = dict(raw=out["raw"], final_T=out["final_T"], final_idx=out["final_idx"], tile_depth=out["tile_depth"])
@@ -754,6 +756,7 @@ def forward_backward(frame: Frame, settings: RenderSettings, cotangents: Dict[st
     holder = _Holder()
     holder.records, holder.radii, holder.num_tiles_hit, holder.M = records, radii, tiles_hit, M
     holder.xys, holder.conics, holder.depths = records[:, 0:2], records[:, 2:5], records[:, 9]
+    holder.table = table
     holder.v_records, holder.grad_arena, holder.v_sky = v_records, arena, v_sky
     holder.param_grads = flat
     holder.tile_bins, holder.tile_depth = tile_bins, out["tile_depth"]  # diagnostics (tools/depth_stats.py)

@@ -30,10 +30,13 @@ from .scene import Camera
 class TrainStep:
     def __init__(self, model: SceneGraphRasterModel, optimizer: FusedAdam, refine_every: Optional[int] = None,
                  group: Optional[dist.ProcessGroup] = None, pipeline_chunks: int = 0, refine_seed: int = 0,
-                 check_replicas: bool = True, overlap: bool = False, exchange: str = "auto"):
+                 check_replicas: bool = True, overlap: bool = False, exchange: str = "auto", metrics: bool = False):
         """``pipeline_chunks`` > 0 (data parallel only): all-reduce and Adam are pipelined over that many ranges of the
-        arena (dp.allreduce_and_step) instead of running one after the other."""
+        arena (dp.allreduce_and_step) instead of running one after the other.  ``metrics``: every step calls
+        ``model.get_metrics_dict`` between ``get_outputs`` and ``get_loss_dict`` (nerfstudio's order,
+        ``VanillaPipeline.get_train_loss_dict``) and keeps its result on ``self.metrics`` (device tensors, no read-back)."""
         self.model, self.optimizer, self.group = model, optimizer, group
+        self.want_metrics, self.metrics = metrics, None
         self.pipeline_chunks = pipeline_chunks if pipeline_chunks > 0 or not overlap else 4
         self.refine_seed, self.check_replicas, self._gen = refine_seed, check_replicas, None
         # how the gradient arena is exchanged: "sym" = this library's kernel over symmetric memory (csrc/collective.cu),
@@ -90,6 +93,8 @@ class TrainStep:
                 self._exchange.flags.zero_()
                 self._exchange._union_fresh = False
                 self._exchange._union_rows = n_bg
+        if self.want_metrics:
+            self.metrics = m.get_metrics_dict(out, batch)
         losses = m.get_loss_dict(out, batch)
         total = sum(losses.values())
         rendered = isinstance(total, torch.Tensor) and total.requires_grad

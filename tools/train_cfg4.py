@@ -25,10 +25,11 @@ sys.path.insert(0, ROOT)
 
 def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int = 100, start_step: int = 600,
         actor_range: float = 45.0, pipeline_chunks: int = 0, overlap: bool = False, resident_table: bool = True,
-        async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True, sky: bool = False) -> dict:
+        async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True, sky: bool = False, metrics: bool = False) -> dict:
     """One measurement.  torch.distributed must already be initialised when WORLD_SIZE > 1.  Returns the result dict on
     rank 0 (None elsewhere).  ``sky``: the reference's default learnable sky (use_sky_sphere, a 1024^2 cube map stepped by
-    the same Adam launch at the ``sky_sphere`` group's lr 0.005, sgn_config.py:72-75)."""
+    the same Adam launch at the ``sky_sphere`` group's lr 0.005, sgn_config.py:72-75).  ``metrics``: every step also computes
+    ``get_metrics_dict`` (psnr, gaussian_count, scale / opacity / radii means), as nerfstudio's training pipeline does."""
     import torch
     import torch.distributed as dist
 
@@ -65,7 +66,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     model.train()
     extra = {"sky": (model.env_map.base, 0.005)} if sky else None
     opt = FusedAdam(model.optimizer_params(), extra=extra, reserve_spare=True)  # no cudaMalloc of moment arenas inside the training loop
-    step_fn = TrainStep(model, opt, refine_every=refine_every, pipeline_chunks=pipeline_chunks, overlap=overlap)
+    step_fn = TrainStep(model, opt, refine_every=refine_every, pipeline_chunks=pipeline_chunks, overlap=overlap, metrics=metrics)
     g = torch.Generator().manual_seed(5)
     gt = (torch.rand(H, W, 3, generator=g) * 255).to(torch.uint8).to(dev)  # get_loss_dict consumes uint8 directly
     counts0 = [sub.num_points for sub in model.all_models.values()]
@@ -172,7 +173,8 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                                f"{W}x{H}; rank r renders camera (step*g + r) mod 425; actors have a box within {actor_range} m of the ego vehicle",
                    "parallelism": f"camera-sharded dp{world}", "ssim_lambda": ssim_lambda,
                    **({"sky": "CubeMapSky(1024), Adam lr 0.005"} if sky else {}),
-                   "loss": "fused kernels" if fused_loss else "torch ops", "start_step": start_step, "refine_every": refine_every,
+                   "loss": "fused kernels" if fused_loss else "torch ops", "metrics": "get_metrics_dict every step" if metrics else "none",
+                   "start_step": start_step, "refine_every": refine_every,
                    "refinement_kernels_loaded_before_timing": refine_warm,
                    "binning": "no host read-back of the intersection count" if async_binning else "one read-back per frame",
                    "segment_table": "device-resident (staged up front; re-staged per timestamp on first use after a refinement)" if resident_table else "host build per frame",
@@ -182,6 +184,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         "gaussians_before": int(sum(counts0)), "gaussians_after": int(sum(counts1)),
         "submodels_changed": int(sum(a != b for a, b in zip(counts0, counts1))),
         "loss_first": first, "loss_last": last, "replicas_identical": replicas_identical,
+        **({"metrics_last": {k: (v if isinstance(v, int) else float(v)) for k, v in step_fn.metrics.items()}} if metrics else {}),
         "step_ms_rank0": step_ms, "host_ms_rank0": [round(x, 3) for x in host_ms]}
 
 
@@ -199,6 +202,7 @@ def main():
     ap.add_argument("--ssim-lambda", type=float, default=0.0, help="weight of the SSIM term (the reference trains with 0.2)")
     ap.add_argument("--torch-loss", action="store_true", help="loss terms as torch ops (SceneGraphConfig.fused_loss = False)")
     ap.add_argument("--sky", action="store_true", help="train the learnable sky cube map (the reference's use_sky_sphere = True)")
+    ap.add_argument("--metrics", action="store_true", help="get_metrics_dict every step, between get_outputs and get_loss_dict")
     args = ap.parse_args()
 
     import torch
@@ -210,7 +214,8 @@ def main():
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     res = run(args.steps, args.warmup, args.scale, args.refine_every, args.start_step, args.actor_range, args.pipeline_chunks,
-              args.overlap, not args.host_table, ssim_lambda=args.ssim_lambda, fused_loss=not args.torch_loss, sky=args.sky)
+              args.overlap, not args.host_table, ssim_lambda=args.ssim_lambda, fused_loss=not args.torch_loss, sky=args.sky,
+              metrics=args.metrics)
     if res is not None:
         print(json.dumps(res))
     if world > 1:
