@@ -165,6 +165,20 @@ int sgn_project_bwd_range(const sgn_segment* segs_dev, const sgn_segment_grads* 
                           const sgn_camera* cam, const float* records, const int32_t* radii, const float* v_records,
                           int chunk_begin, int chunk_end, void* stream);
 
+/* The range backward that ALSO yields the cotangents of the segments' object->world poses: every 128-row chunk of a
+ * segment with has_pose stores the sums over its rows of (v_R[9] row-major, v_t[3], v_q[4]) -- means_w = R m + t gives
+ * v_t = sum vmw and v_R[r][c] = sum vmw[r] m[c]; q_w = q_box (x) q gives v_q = sum vqr (x) conj(q), q un-normalised -- to
+ * pose_partials[num_chunks, SGN_POSE_FLOATS] (chunks of other segments are not written).  The parameter gradients are
+ * bit-identical to sgn_project_bwd_range's.  sgn_pose_grad_reduce, called after the last range, sums a segment's chunks
+ * into v_pose[nseg, SGN_POSE_FLOATS] (zero rows for segments without a pose).  Neither stage uses atomics: v_pose is the
+ * same bits on every run over the same v_records. */
+#define SGN_POSE_FLOATS 16
+int sgn_project_bwd_pose(const sgn_segment* segs_dev, const sgn_segment_grads* grads_dev, int nseg, int N, int num_chunks,
+                         const sgn_camera* cam, const float* records, const int32_t* radii, const float* v_records,
+                         int chunk_begin, int chunk_end, float* pose_partials, void* stream);
+int sgn_pose_grad_reduce(const sgn_segment* segs_dev, int nseg, int num_chunks, const float* pose_partials, float* v_pose,
+                         void* stream);
+
 /* ---- Level-1: gsplat 0.1.x function API on plain tensors (sgn_splatfacto.py:11-14) -------------------
  * gsplat.project_gaussians(means3d, scales, glob_scale, quats, viewmat, fx, fy, cx, cy, H, W, block_width,
  * clip_thresh) -> xys[N,2], depths[N], radii[N] i32, conics[N,3], compensation[N], num_tiles_hit[N] i32,

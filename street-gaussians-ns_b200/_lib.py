@@ -134,8 +134,9 @@ EXPORTS = [
     "sgn_sizeof_refine_config", "sgn_sizeof_refine_tensors", "sgn_refine_decide", "sgn_refine_apply",
     "sgn_bin_local_cap", "sgn_bin_local_scratch_bytes", "sgn_bin_local_count", "sgn_bin_local_sort",
     "sgn_project_bwd_range", "sgn_allreduce_sym", "sgn_blend_extra_fwd", "sgn_blend_extra_bwd", "sgn_blend_extra_bwd_det",
-    "sgn_bin_sort_capped", "sgn_visible_flags", "sgn_visible_union",
+    "sgn_bin_sort_capped", "sgn_visible_flags", "sgn_visible_union", "sgn_project_bwd_pose", "sgn_pose_grad_reduce",
 ]
+POSE_FLOATS = 16  # SGN_POSE_FLOATS: a segment's pose (and its cotangent) as R[9] row-major, t[3], q[4]
 AR_MAX_SLICES = 48  # SGN_AR_MAX_SLICES
 
 
@@ -161,6 +162,9 @@ def load():
     L.sgn_project_bwd.argtypes = [vp, vp, i32, i32, i32, C.POINTER(CameraStruct), vp, vp, vp, vp]
     L.sgn_project_bwd_range.argtypes = [vp, vp, i32, i32, i32, C.POINTER(CameraStruct), vp, vp, vp, i32, i32, vp]
     L.sgn_project_bwd_range.restype = C.c_int
+    L.sgn_project_bwd_pose.argtypes = [vp, vp, i32, i32, i32, C.POINTER(CameraStruct), vp, vp, vp, i32, i32, vp, vp]
+    L.sgn_pose_grad_reduce.argtypes = [vp, i32, i32, vp, vp, vp]
+    L.sgn_project_bwd_pose.restype = L.sgn_pose_grad_reduce.restype = C.c_int
     L.sgn_allreduce_sym.argtypes = [vp, vp, vp, i32, i32, i32, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int32),
                                     C.POINTER(C.c_int64), C.POINTER(C.c_int64), vp, C.c_float, i32, vp]
     L.sgn_visible_flags.argtypes = [vp, i64, vp, vp]

@@ -461,10 +461,15 @@ __device__ __forceinline__ void sgn_project_vjp(const sgn_camera& cam, const Sgn
 // ------------------------------------------------------------------------------------------------
 // backward
 // ------------------------------------------------------------------------------------------------
+// POSE: a block whose segment has an object->world pose also reduces the cotangents of that pose over its rows --
+// v_R[r][c] = sum vmw[r] m[c] (means_w = R m + t), v_t = sum vmw, v_a = sum vqr (x) conj(q) (q_w = a (x) q, q un-normalised) --
+// and stores the 16 sums to pose_partials[chunk]: warp shuffles, then the four warps in fixed order; no atomics, so the
+// sums do not depend on the run.  Colour contributes nothing (the SH view direction is taken from detached means).
+template <bool POSE>
 __global__ void __launch_bounds__(CH)
 project_bwd_kernel(const sgn_segment* __restrict__ segs, const sgn_segment_grads* __restrict__ grads, int nseg,
                    const sgn_camera cam, const float4* __restrict__ records, const int32_t* __restrict__ radii,
-                   const float4* __restrict__ v_records, const int chunk_begin) {
+                   const float4* __restrict__ v_records, const int chunk_begin, float* __restrict__ pose_partials) {
     extern __shared__ int s_chunk0[];
     __shared__ __align__(16) float s_rest[CH * MAX_REST];   // out: features_rest gradient rows
     __shared__ __align__(16) float s_dc[CH * MAX_DC];       // out: features_dc gradient rows
@@ -485,6 +490,7 @@ project_bwd_kernel(const sgn_segment* __restrict__ segs, const sgn_segment_grads
     __syncthreads();
     const int tid = threadIdx.x;
     float gm[3] = {0.f, 0.f, 0.f}, gs[3] = {0.f, 0.f, 0.f}, gq[4] = {0.f, 0.f, 0.f, 0.f};
+    float vp[POSE ? SGN_POSE_FLOATS : 1] = {};  // this row's share of (v_R 9, v_t 3, v_a 4)
     const bool row_vis = (tid < rows) && radii[(size_t)sg.row0 + r0 + tid] > 0;
     if (tid < rows && !row_vis) {
         // the rasterizer never touched this Gaussian: every cotangent is zero, so is every gradient
@@ -567,6 +573,18 @@ project_bwd_kernel(const sgn_segment* __restrict__ segs, const sgn_segment_grads
                 gq[1] = -ax * vqr[0] + aw * vqr[1] + az * vqr[2] - ay * vqr[3];
                 gq[2] = -ay * vqr[0] - az * vqr[1] + aw * vqr[2] + ax * vqr[3];
                 gq[3] = -az * vqr[0] + ay * vqr[1] - ax * vqr[2] + aw * vqr[3];
+                if constexpr (POSE) {
+#pragma unroll
+                    for (int r = 0; r < 3; ++r) {
+#pragma unroll
+                        for (int c = 0; c < 3; ++c) vp[3 * r + c] = vmw[r] * m[c];
+                        vp[9 + r] = vmw[r];
+                    }
+                    vp[12] = vqr[0] * q[0] + vqr[1] * q[1] + vqr[2] * q[2] + vqr[3] * q[3];
+                    vp[13] = -vqr[0] * q[1] + vqr[1] * q[0] - vqr[2] * q[3] + vqr[3] * q[2];
+                    vp[14] = -vqr[0] * q[2] + vqr[1] * q[3] + vqr[2] * q[0] - vqr[3] * q[1];
+                    vp[15] = -vqr[0] * q[3] - vqr[1] * q[2] + vqr[2] * q[1] + vqr[3] * q[0];
+                }
             } else {
 #pragma unroll
                 for (int c = 0; c < 3; ++c) gm[c] = vmw[c];
@@ -575,6 +593,25 @@ project_bwd_kernel(const sgn_segment* __restrict__ segs, const sgn_segment_grads
             }
         }
         reinterpret_cast<float4*>(gr.quats)[i] = make_float4(gq[0], gq[1], gq[2], gq[3]);
+    }
+    if constexpr (POSE) {
+        __shared__ float s_pose[(CH / 32) * SGN_POSE_FLOATS];
+        if (sg.has_pose) {  // block-uniform: a chunk never straddles segments
+#pragma unroll
+            for (int k = 0; k < SGN_POSE_FLOATS; ++k) {
+                float x = vp[k];
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) x += __shfl_down_sync(0xffffffffu, x, o);
+                if ((tid & 31) == 0) s_pose[(tid >> 5) * SGN_POSE_FLOATS + k] = x;
+            }
+            __syncthreads();
+            if (tid < SGN_POSE_FLOATS) {
+                float x = s_pose[tid];
+#pragma unroll
+                for (int w = 1; w < CH / 32; ++w) x += s_pose[w * SGN_POSE_FLOATS + tid];
+                pose_partials[(size_t)chunk * SGN_POSE_FLOATS + tid] = x;
+            }
+        }
     }
     __syncthreads();  // every thread has consumed its means / scales inputs
     if (tid < rows) {
@@ -588,27 +625,71 @@ project_bwd_kernel(const sgn_segment* __restrict__ segs, const sgn_segment_grads
     if (nrest > 0) coop_store(gr.features_rest + (size_t)r0 * nrest, s_rest, rows * nrest);
 }
 
+static int project_bwd_launch(const char* what, const sgn_segment* segs_dev, const sgn_segment_grads* grads_dev, int nseg, int N, int num_chunks,
+                              const sgn_camera* cam, const float* records, const int32_t* radii, const float* v_records,
+                              int chunk_begin, int chunk_end, float* pose_partials, bool pose, void* stream) {
+    SGN_REQUIRE(segs_dev && grads_dev && cam && records && radii && v_records, "%s: null pointer", what);
+    SGN_REQUIRE(!pose || pose_partials, "%s: null pose_partials", what);
+    SGN_REQUIRE(nseg >= 1 && nseg <= SGN_MAX_SEGMENTS, "%s: nseg=%d out of range", what, nseg);
+    SGN_REQUIRE(sgn_aligned16(records) && sgn_aligned16(v_records), "records / v_records must be 16-byte aligned");
+    SGN_REQUIRE(chunk_begin >= 0 && chunk_begin <= chunk_end && chunk_end <= num_chunks, "%s: chunk range [%d, %d) outside [0, %d)",
+                what, chunk_begin, chunk_end, num_chunks);
+    if (N == 0 || chunk_end == chunk_begin) return SGN_OK;
+    auto kernel = pose ? project_bwd_kernel<true> : project_bwd_kernel<false>;
+    kernel<<<chunk_end - chunk_begin, CH, nseg * sizeof(int), (cudaStream_t)stream>>>(
+        segs_dev, grads_dev, nseg, *cam, reinterpret_cast<const float4*>(records), radii,
+        reinterpret_cast<const float4*>(v_records), chunk_begin, pose_partials);
+    SGN_CHECK_LAUNCH("project_bwd_kernel");
+    return SGN_OK;
+}
+
 extern "C" int sgn_project_bwd_range(const sgn_segment* segs_dev, const sgn_segment_grads* grads_dev, int nseg, int N, int num_chunks,
                                      const sgn_camera* cam, const float* records, const int32_t* radii,
                                      const float* v_records, int chunk_begin, int chunk_end, void* stream) {
     SGN_RANGE("sgn_project_bwd");
-    SGN_REQUIRE(segs_dev && grads_dev && cam && records && radii && v_records, "sgn_project_bwd: null pointer");
-    SGN_REQUIRE(nseg >= 1 && nseg <= SGN_MAX_SEGMENTS, "sgn_project_bwd: nseg=%d out of range", nseg);
-    SGN_REQUIRE(sgn_aligned16(records) && sgn_aligned16(v_records), "records / v_records must be 16-byte aligned");
-    SGN_REQUIRE(chunk_begin >= 0 && chunk_begin <= chunk_end && chunk_end <= num_chunks, "sgn_project_bwd: chunk range [%d, %d) outside [0, %d)",
-                chunk_begin, chunk_end, num_chunks);
-    if (N == 0 || chunk_end == chunk_begin) return SGN_OK;
-    project_bwd_kernel<<<chunk_end - chunk_begin, CH, nseg * sizeof(int), (cudaStream_t)stream>>>(
-        segs_dev, grads_dev, nseg, *cam, reinterpret_cast<const float4*>(records), radii,
-        reinterpret_cast<const float4*>(v_records), chunk_begin);
-    SGN_CHECK_LAUNCH("project_bwd_kernel");
-    return SGN_OK;
+    return project_bwd_launch("sgn_project_bwd", segs_dev, grads_dev, nseg, N, num_chunks, cam, records, radii, v_records, chunk_begin,
+                              chunk_end, nullptr, false, stream);
 }
 
 extern "C" int sgn_project_bwd(const sgn_segment* segs_dev, const sgn_segment_grads* grads_dev, int nseg, int N, int num_chunks,
                                const sgn_camera* cam, const float* records, const int32_t* radii,
                                const float* v_records, void* stream) {
     return sgn_project_bwd_range(segs_dev, grads_dev, nseg, N, num_chunks, cam, records, radii, v_records, 0, num_chunks > 0 ? num_chunks : 0, stream);
+}
+
+extern "C" int sgn_project_bwd_pose(const sgn_segment* segs_dev, const sgn_segment_grads* grads_dev, int nseg, int N, int num_chunks,
+                                    const sgn_camera* cam, const float* records, const int32_t* radii, const float* v_records,
+                                    int chunk_begin, int chunk_end, float* pose_partials, void* stream) {
+    SGN_RANGE("sgn_project_bwd_pose");
+    return project_bwd_launch("sgn_project_bwd_pose", segs_dev, grads_dev, nseg, N, num_chunks, cam, records, radii, v_records,
+                              chunk_begin, chunk_end, pose_partials, true, stream);
+}
+
+// One warp per segment: the sums of pose_partials over the segment's chunks, in a fixed order (lane = value + 16 x chunk
+// parity, chunks ascending, then the two parities) -> v_pose[segment]; zeros for a segment without a pose.
+__global__ void __launch_bounds__(CH)
+pose_reduce_kernel(const sgn_segment* __restrict__ segs, int nseg, const float* __restrict__ pose_partials, float* __restrict__ v_pose) {
+    const int si = blockIdx.x * (CH / 32) + (threadIdx.x >> 5);
+    if (si >= nseg) return;
+    const int lane = threadIdx.x & 31, k = lane & (SGN_POSE_FLOATS - 1);
+    float x = 0.f;
+    if (segs[si].has_pose) {
+        const int chunk0 = segs[si].chunk0, n = (segs[si].count + CH - 1) / CH;
+        for (int c = lane >> 4; c < n; c += 2) x += pose_partials[(size_t)(chunk0 + c) * SGN_POSE_FLOATS + k];
+    }
+    x += __shfl_down_sync(0xffffffffu, x, 16);
+    if (lane < SGN_POSE_FLOATS) v_pose[(size_t)si * SGN_POSE_FLOATS + lane] = x;
+}
+
+extern "C" int sgn_pose_grad_reduce(const sgn_segment* segs_dev, int nseg, int num_chunks, const float* pose_partials, float* v_pose,
+                                    void* stream) {
+    SGN_RANGE("sgn_pose_grad_reduce");
+    SGN_REQUIRE(segs_dev && v_pose, "sgn_pose_grad_reduce: null pointer");
+    SGN_REQUIRE(nseg >= 1 && nseg <= SGN_MAX_SEGMENTS, "sgn_pose_grad_reduce: nseg=%d out of range", nseg);
+    SGN_REQUIRE(num_chunks >= 0 && (num_chunks == 0 || pose_partials), "sgn_pose_grad_reduce: null pose_partials for %d chunks", num_chunks);
+    pose_reduce_kernel<<<(nseg + CH / 32 - 1) / (CH / 32), CH, 0, (cudaStream_t)stream>>>(segs_dev, nseg, pose_partials, v_pose);
+    SGN_CHECK_LAUNCH("pose_reduce_kernel");
+    return SGN_OK;
 }
 
 // ================================================================================================

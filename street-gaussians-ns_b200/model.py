@@ -36,13 +36,16 @@ from .scene import PARAM_NAMES, CLS_BACKGROUND, CLS_OBJECT, Camera, Frame, Gauss
 @dataclass
 class ActorPose:
     """What the path needs from a reference ``Box`` (data/utils/dynamic_annotation.py): trackId,
-    center, rot, frame; plus the actor's frame list for the Fourier time (scene graph :239-245)."""
+    center, rot, frame; plus the actor's frame list for the Fourier time (scene graph :239-245).  ``frame_id``: the integer
+    timestamp of the box's annotated frame (``Box.frame_id``), which names its row of the box corrections
+    (box_pose.BoxPoseOptimizer); None -- the default -- for a box that is not corrected."""
 
     track_id: str
     rot: np.ndarray
     center: np.ndarray
     frame: int
     frame_list: Sequence[int]
+    frame_id: Optional[int] = None
 
 
 @dataclass
@@ -302,9 +305,12 @@ _MODEL_SERIAL = itertools.count()
 class SceneGraphRasterModel(torch.nn.Module):
     def __init__(self, background: GaussianSet, actors: Dict[str, GaussianSet], config: Optional[SceneGraphConfig] = None,
                  poses_at: Optional[Callable[[float], List[ActorPose]]] = None,
-                 sky: Optional[Callable[[Camera, bool], torch.Tensor]] = None):
+                 sky: Optional[Callable[[Camera, bool], torch.Tensor]] = None, bbox_optimizer: Optional[torch.nn.Module] = None):
         super().__init__()
         self.config = config or SceneGraphConfig()
+        # trainable corrections of the actor boxes (box_pose.BoxPoseOptimizer; the reference's attribute name, scene graph
+        # :91).  None, or one in mode "off": the boxes are rendered as annotated, by the same calls as without it
+        self.bbox_optimizer = bbox_optimizer
         self.all_models = torch.nn.ModuleDict()
         self.all_models["background"] = GaussianSubModel(background)
         for obj_id, ps in actors.items():
@@ -371,7 +377,7 @@ class SceneGraphRasterModel(torch.nn.Module):
         if hit is not None and hit["digest"] == digest and hit["ptr0"] == self.all_models._modules["background"].gauss_params._parameters["means"].data_ptr():
             self.visible_model_names = hit["names"]
             frame = Frame(camera, hit["segments"])
-            frame._prebuilt, frame._table_slot = hit["table"], hit
+            frame._prebuilt, frame._table_slot, frame._actor_poses = hit["table"], hit, hit["actor_poses"]
             frame._static_key = ("model", self.__dict__["_serial"], self.__dict__.get("_param_epoch", 0), tuple(hit["names"]), str(self.device))
             return frame
         frame = self._build_frame(camera, poses)
@@ -391,6 +397,7 @@ class SceneGraphRasterModel(torch.nn.Module):
             self._frame_cache.clear()
         slot = self._frame_cache[time] = dict(
             digest=digest, segments=frame.segments, names=list(self.visible_model_names), table=table,
+            actor_poses=frame._actor_poses,
             ptr0=self.all_models._modules["background"].gauss_params._parameters["means"].data_ptr())
         return slot
 
@@ -434,6 +441,7 @@ class SceneGraphRasterModel(torch.nn.Module):
     def _build_frame(self, camera: Camera, poses) -> Frame:
         segs = [Segment(self._set_of("background"), CLS_BACKGROUND, name="background")]
         names = ["background"]
+        kept = []
         for pose in poses:
             name = self.get_object_model_name(pose.track_id)
             assert name not in names
@@ -447,8 +455,10 @@ class SceneGraphRasterModel(torch.nn.Module):
                 basis = idft_basis(t, F)
             segs.append(Segment(ps, CLS_OBJECT, rot=pose.rot, center=pose.center, idft=basis, name=name))
             names.append(name)
+            kept.append(pose)
         self.visible_model_names = names
         frame = Frame(camera, segs)
+        frame._actor_poses = kept
         frame._static_key = ("model", self.__dict__["_serial"], self.__dict__.get("_param_epoch", 0), tuple(names), str(self.device))
         return frame
 
@@ -458,6 +468,23 @@ class SceneGraphRasterModel(torch.nn.Module):
         return raster.RenderSettings(sh_degree=c.sh_degree, sh_degree_to_use=n, block_width=c.block_width,
                                      alpha_clamp_fwd=c.alpha_clamp_fwd, alpha_clamp_bwd=c.alpha_clamp_bwd,
                                      class_streams=class_streams, training=self.training, async_binning=c.async_binning)
+
+    def _box_poses(self, frame: Frame) -> Optional[torch.Tensor]:
+        """The corrected poses of the frame's actors, [actors, 16], from ``bbox_optimizer`` -- in training and in eval alike,
+        as the reference applies the correction whenever the box has an annotated frame (scene graph :340-341).  The
+        annotated poses and parameter rows of a timestamp are staged on the device once and kept with its segment rows."""
+        bo = self.bbox_optimizer
+        boxes = frame._actor_poses
+        if bo is None or bo.mode == "off" or not boxes:
+            return None
+        slot = getattr(frame, "_table_slot", None)
+        staged = slot.get("box_stage") if slot is not None else None
+        if staged is None:
+            fi, bi = bo.indices(boxes)
+            staged = bo.stage(fi, bi, [b.rot for b in boxes], [b.center for b in boxes], device=self.device)
+            if slot is not None:
+                slot["box_stage"] = staged
+        return bo(staged)
 
     def get_outputs(self, camera: Camera) -> Dict[str, torch.Tensor]:
         """``SplatfactoSceneGraphModel.get_outputs`` (scene graph :305-374)."""
@@ -478,7 +505,8 @@ class SceneGraphRasterModel(torch.nn.Module):
                 if self._anchor is None or self._anchor.device != flat[0].device:
                     self._anchor = torch.zeros(1, device=flat[0].device, requires_grad=True)
                 anchor = self._anchor
-        out, holder = raster.render_frame(frame, self._settings(class_streams=True), sky=sky, grad_sink=sink, anchor=anchor)
+        pose = self._box_poses(frame)
+        out, holder = raster.render_frame(frame, self._settings(class_streams=True), sky=sky, grad_sink=sink, anchor=anchor, pose=pose)
         self._holder = holder
         self._publish_side_effects(frame, holder)
         if isinstance(holder.M, raster.LazyCount):
@@ -500,19 +528,19 @@ class SceneGraphRasterModel(torch.nn.Module):
             # eval-only extra renders (scene graph :367-372): per-class rgb
             with torch.no_grad():
                 out["background_rgb"] = self._class_rgb(frame, CLS_BACKGROUND, sky)
-                out["object_rgb"] = self._class_rgb(frame, CLS_OBJECT, None)
+                out["object_rgb"] = self._class_rgb(frame, CLS_OBJECT, None, pose)
                 if not any(s.cls == CLS_OBJECT for s in frame.segments):
                     # without actors the reference's objects-only render returns {'rgb': zeros[H,W,1], 'depth': zeros[H,W,1]}
                     # (scene graph :264-267), which get_outputs publishes as object_rgb AND object_depth (:371-372)
                     out["object_depth"] = torch.zeros(H, W, 1, device=self.device)
         return out
 
-    def _class_rgb(self, frame: Frame, cls: int, sky):
+    def _class_rgb(self, frame: Frame, cls: int, sky, pose=None):
         segs = [s for s in frame.segments if s.cls == cls]
         H, W = frame.camera.height, frame.camera.width
         if not segs:
             return torch.zeros(H, W, 1, device=self.device) if sky is None else sky
-        sub, _ = raster.render_frame(Frame(frame.camera, segs), self._settings(class_streams=False), sky=sky)
+        sub, _ = raster.render_frame(Frame(frame.camera, segs), self._settings(class_streams=False), sky=sky, pose=pose)
         return sub["rgb"]
 
     def _refine_settings_of(self, sub) -> RefineSettings:

@@ -190,6 +190,13 @@ class PoseTable:
     def poses_at(self, time) -> list:
         """Boxes at a camera time as the ``ActorPose`` records SceneGraphRasterModel consumes.  ``frame`` is the box's
         annotated-frame index (-1 for interpolated boxes, which is what the reference's Fourier time then uses,
-        sgn_splatfacto_scene_graph.py:239-245) and ``frame_list`` the track's annotated frames."""
+        sgn_splatfacto_scene_graph.py:239-245), ``frame_list`` the track's annotated frames and ``frame_id`` the annotated
+        frame's timestamp (None for interpolated boxes: the box corrections skip them, :340-341)."""
         from .model import ActorPose
-        return [ActorPose(b.track_id, b.rot, b.center, b.frame, self.objects_frames[b.track_id]) for b in self[time]]
+        return [ActorPose(b.track_id, b.rot, b.center, b.frame, self.objects_frames[b.track_id],
+                          frame_id=b.frame_id if b.frame != -1 else None) for b in self[time]]
+
+    def frame_idx_map(self) -> Dict[int, int]:
+        """Integer timestamp of every annotated frame -> its index (``build_frame_idx_map``, scene graph :101-105): what
+        ``box_pose.BoxPoseOptimizer(len(table), table.unique_track_ids, table.frame_idx_map())`` indexes its rows by."""
+        return {int(ts): i for i, ts in enumerate(self.all_names)}

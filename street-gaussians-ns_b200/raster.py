@@ -11,6 +11,7 @@ CUDA library.  There is no CPU fallback.
 """
 from __future__ import annotations
 
+import copy
 import ctypes as C
 import os
 from dataclasses import dataclass
@@ -218,6 +219,34 @@ def _grads_table(arena: torch.Tensor, static: dict, device) -> torch.Tensor:
         off = static["grad_offsets"] = (np.concatenate([[0], np.cumsum(flat)[:-1]]) * 4).astype(np.uint64)
     tab = (np.uint64(arena.data_ptr()) + off).view(np.uint8)
     return torch.from_numpy(tab).to(device, non_blocking=True)
+
+
+SEG_FLOATS = SEG_DTYPE.itemsize // 4
+POSE_OFFSET = SEG_DTYPE.fields["R"][1] // 4  # R[9], t[3], q[4] are contiguous floats of a row
+assert SEG_DTYPE.fields["t"][1] == 4 * (POSE_OFFSET + 9) and SEG_DTYPE.fields["q"][1] == 4 * (POSE_OFFSET + 12)
+
+
+def posed_rows(table: SegmentTable):
+    """Indices of the table's segments that carry a pose, as a slice when they are adjacent (background first, then the
+    actors: the usual frame) and as a list otherwise."""
+    idx = np.nonzero(table.host["has_pose"])[0]
+    if idx.size and idx[-1] - idx[0] + 1 == idx.size:
+        return slice(int(idx[0]), int(idx[-1]) + 1), int(idx.size)
+    return [int(i) for i in idx], int(idx.size)
+
+
+def with_poses(table: SegmentTable, pose: torch.Tensor) -> SegmentTable:
+    """A copy of ``table`` whose device rows carry ``pose`` [n_posed, 16] (R 9 row-major, t 3, q 4; float32, in the order of
+    the posed segments) instead of the poses it was built with.  The rows ``table`` holds -- which may be a timestamp's
+    resident rows (model.prepare_frames) -- are not written: one device copy of nseg x 168 bytes, one assignment."""
+    rows, n = posed_rows(table)
+    if not (pose.is_cuda and pose.device == table.dev.device and pose.dtype == torch.float32 and tuple(pose.shape) == (n, _lib.POSE_FLOATS)):
+        raise _lib.SgnError(f"pose must be a float32 [{n}, {_lib.POSE_FLOATS}] tensor on {table.dev.device} (one row per posed segment); "
+                            f"got {pose.dtype} {tuple(pose.shape)} on {pose.device}")
+    out = copy.copy(table)
+    out.dev = table.dev.clone()
+    out.dev.view(torch.float32).view(table.nseg, SEG_FLOATS)[rows, POSE_OFFSET:POSE_OFFSET + _lib.POSE_FLOATS] = pose.detach()
+    return out
 
 
 # --------------------------------------------------------------------------------------------------
@@ -570,10 +599,13 @@ def arena_views(arena: torch.Tensor, static: dict) -> List[torch.Tensor]:
 
 
 def project_bwd(table: SegmentTable, params: List[List[torch.Tensor]], cs, records, radii, v_records, make_views: bool = True,
-                out: Optional[torch.Tensor] = None, out_offsets: Optional[np.ndarray] = None, chunk_ranges=None, after_range=None):
+                out: Optional[torch.Tensor] = None, out_offsets: Optional[np.ndarray] = None, chunk_ranges=None, after_range=None,
+                v_pose: Optional[torch.Tensor] = None):
     """Dense parameter gradients, one flat arena (a single allocation, 16-byte aligned slices; ``out`` reuses one).
     ``out_offsets`` (floats, one per parameter tensor of the frame, multiples of 4) places the slices inside a larger
-    ``out`` -- the data-parallel arena that has the layout of ALL sub-models (model._FullArenaSink)."""
+    ``out`` -- the data-parallel arena that has the layout of ALL sub-models (model._FullArenaSink).
+    ``v_pose`` [nseg, 16] float32: also filled with the cotangents of the segments' poses (R 9, t 3, q 4; zero rows for
+    segments without one) -- sgn_project_bwd_pose for every range, then sgn_pose_grad_reduce.  The arena is the same bits."""
     L = _lib.load()
     device = records.device
     st = table.static
@@ -589,6 +621,12 @@ def project_bwd(table: SegmentTable, params: List[List[torch.Tensor]], cs, recor
         assert arena.numel() == sum(flat_sizes)
         gt = _grads_table(arena, st, device)
     flat = arena_views(arena, st) if make_views else None
+    partials = None
+    if v_pose is not None:
+        assert v_pose.shape == (table.nseg, _lib.POSE_FLOATS) and v_pose.dtype == torch.float32 and v_pose.is_contiguous() and v_pose.device == device
+        partials = torch.empty(max(table.num_chunks, 1), _lib.POSE_FLOATS, device=device, dtype=torch.float32)
+        if chunk_ranges is None:
+            chunk_ranges = [(0, table.num_chunks)]
     with _timed("project_bwd"):
         if chunk_ranges is None:
             _lib.check(L.sgn_project_bwd(_ptr(table.dev), _ptr(gt), table.nseg, table.N, table.num_chunks, C.byref(cs), _ptr(records),
@@ -597,11 +635,19 @@ def project_bwd(table: SegmentTable, params: List[List[torch.Tensor]], cs, recor
             # range by range (data parallel): ``after_range(k)`` is called once range k's launch is enqueued -- the exchange of
             # that range's slices starts there and overlaps the production of the next range (dp.SymmetricExchange)
             for k, (c0, c1) in enumerate(chunk_ranges):
-                _lib.check(L.sgn_project_bwd_range(_ptr(table.dev), _ptr(gt), table.nseg, table.N, table.num_chunks, C.byref(cs),
-                                                   _ptr(records), _ptr(radii), _ptr(v_records), int(c0), int(c1), _stream()),
-                           "sgn_project_bwd_range")
+                if partials is not None:
+                    _lib.check(L.sgn_project_bwd_pose(_ptr(table.dev), _ptr(gt), table.nseg, table.N, table.num_chunks, C.byref(cs),
+                                                      _ptr(records), _ptr(radii), _ptr(v_records), int(c0), int(c1), _ptr(partials),
+                                                      _stream()), "sgn_project_bwd_pose")
+                else:
+                    _lib.check(L.sgn_project_bwd_range(_ptr(table.dev), _ptr(gt), table.nseg, table.N, table.num_chunks, C.byref(cs),
+                                                       _ptr(records), _ptr(radii), _ptr(v_records), int(c0), int(c1), _stream()),
+                               "sgn_project_bwd_range")
                 if after_range is not None:
                     after_range(k)
+        if partials is not None:
+            _lib.check(L.sgn_pose_grad_reduce(_ptr(table.dev), table.nseg, table.num_chunks, _ptr(partials), _ptr(v_pose), _stream()),
+                       "sgn_pose_grad_reduce")
     return flat, arena
 
 
@@ -618,6 +664,7 @@ class _Holder:
         self.grad_arena = None
         self.param_grads = None
         self.v_sky = None
+        self.v_pose = None  # [nseg, 16] after a backward through a render whose ``pose`` required grad
         self.M = 0
         self.tile_bins = self.tile_depth = None
         self.table = None  # the frame's SegmentTable: its device rows are what sgn_metrics reads the parameters through
@@ -630,7 +677,7 @@ class _Holder:
 class _SceneGraphRasterize(torch.autograd.Function):
     @staticmethod
     def forward(ctx, frame: Frame, settings: RenderSettings, holder: _Holder, sky: Optional[torch.Tensor],
-                extra: Optional[torch.Tensor], *flat):
+                extra: Optional[torch.Tensor], pose: Optional[torch.Tensor], *flat):
         # unused outputs must reach backward as None, not as zero tensors: the kernels specialise on
         # which cotangents exist (depth / background_acc have none in training)
         ctx.set_materialize_grads(False)
@@ -652,6 +699,9 @@ class _SceneGraphRasterize(torch.autograd.Function):
             assert sky.shape == (cs.height, cs.width, 3)
         bo = blend_opts(settings, sky is not None)
         table = SegmentTable(frame, params, device)
+        if pose is not None:
+            table = with_poses(table, pose)
+        ctx.pose_needs_grad = pose is not None and pose.requires_grad
         proj = project_fwd(table, cs, device)
         records, radii, tiles_hit, bbox = proj
         M, sorted_ids, tile_bins = bin_and_sort(cs, records, radii, proj=proj, async_binning=settings.async_binning)
@@ -697,6 +747,9 @@ class _SceneGraphRasterize(torch.autograd.Function):
                                       deterministic=ctx.settings.deterministic)
         h = ctx.holder
         sink = h.grad_sink
+        v_pose = g_pose = None
+        if ctx.pose_needs_grad:
+            v_pose = torch.empty(ctx.table.nseg, _lib.POSE_FLOATS, device=v_records.device, dtype=torch.float32)
         if sink is not None:
             target = sink.target(ctx.table.static, v_records.device)
             offsets = sink.grad_offsets(ctx.table.static) if target is not None else None  # None: the frame's own layout
@@ -705,18 +758,20 @@ class _SceneGraphRasterize(torch.autograd.Function):
             if plan is not None and target is not None:
                 chunk_ranges, after_range = plan(ctx.table)
             _, arena = project_bwd(ctx.table, ctx.params, ctx.cs, ctx.records, ctx.radii, v_records, make_views=False,
-                                   out=target, out_offsets=offsets, chunk_ranges=chunk_ranges, after_range=after_range)
+                                   out=target, out_offsets=offsets, chunk_ranges=chunk_ranges, after_range=after_range, v_pose=v_pose)
             sink.publish(arena, ctx.table.static)
             flat = (None,)
         else:
-            flat, arena = project_bwd(ctx.table, ctx.params, ctx.cs, ctx.records, ctx.radii, v_records)
-        h.v_records, h.grad_arena = v_records, arena
+            flat, arena = project_bwd(ctx.table, ctx.params, ctx.cs, ctx.records, ctx.radii, v_records, v_pose=v_pose)
+        h.v_records, h.grad_arena, h.v_pose = v_records, arena, v_pose
+        if v_pose is not None:
+            g_pose = v_pose[posed_rows(ctx.table)[0]]
         # the reference reads ``self.xys.grad`` after backward (densification statistics,
         # sgn_splatfacto.py:520-524): xys is a view of the record array, its gradient a view of v_records
         h.xys.grad = v_records[:, 0:2]
         if h.post_backward is not None:
             h.post_backward(h)
-        return (None, None, None, v_sky, v_extra, *flat)
+        return (None, None, None, v_sky, v_extra, g_pose, *flat)
 
 
 def forward_backward(frame: Frame, settings: RenderSettings, cotangents: Dict[str, Optional[torch.Tensor]],
@@ -801,8 +856,17 @@ def blend_extra_bwd(cs, bo, records, sorted_ids, tile_bins, final_T, final_idx, 
 
 
 def render_frame(frame: Frame, settings: Optional[RenderSettings] = None, sky: Optional[torch.Tensor] = None,
-                 grad_sink=None, anchor: Optional[torch.Tensor] = None, extra: Optional[torch.Tensor] = None):
+                 grad_sink=None, anchor: Optional[torch.Tensor] = None, extra: Optional[torch.Tensor] = None,
+                 pose: Optional[torch.Tensor] = None):
     """Render one camera.  Returns (outputs dict, holder).  Segment parameters must be CUDA tensors.
+
+    ``pose`` [n_posed, 16] (float32, on the device; one row per posed segment in the frame's order: R 9 row-major, t 3,
+    q 4 -- the unit quaternion of R with w >= 0, as ``object2world_gs`` hands it on): the object->world poses to render
+    with, in place of the ones the frame's segments carry.  Differentiable: when it requires grad, backward reduces its
+    cotangent inside the projection backward (sgn_project_bwd_pose + sgn_pose_grad_reduce; no atomics, so the gradient
+    is the same bits on every run over the same image cotangents in deterministic mode).  R enters through the means and
+    q through the covariances only, exactly as the kernels use them; nothing ties the two together here, that is the
+    caller's parametrisation (box_pose.BoxPoseOptimizer).  Without ``pose`` the call sequence is unchanged.
 
     ``extra`` [N, C] (rows in the frame's concatenated order, float32): generic per-Gaussian channels -- e.g. semantic
     logits -- composited with the weights of the main render into ``out["extra"]`` [H, W, C], 8 channels per traversal,
@@ -814,7 +878,7 @@ def render_frame(frame: Frame, settings: Optional[RenderSettings] = None, sky: O
     holder = _Holder()
     holder.grad_sink = grad_sink
     flat = [anchor] if grad_sink is not None else [t for seg in frame.segments for t in seg.params.tensors()]
-    outs = _SceneGraphRasterize.apply(frame, settings, holder, sky, extra, *flat)
+    outs = _SceneGraphRasterize.apply(frame, settings, holder, sky, extra, pose, *flat)
     extra_img = None
     if extra is not None:
         outs, extra_img = outs[:-1], outs[-1]

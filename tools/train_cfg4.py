@@ -25,11 +25,14 @@ sys.path.insert(0, ROOT)
 
 def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int = 100, start_step: int = 600,
         actor_range: float = 45.0, pipeline_chunks: int = 0, overlap: bool = False, resident_table: bool = True,
-        async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True, sky: bool = False, metrics: bool = False) -> dict:
+        async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True, sky: bool = False, metrics: bool = False,
+        bbox_opt: bool = False) -> dict:
     """One measurement.  torch.distributed must already be initialised when WORLD_SIZE > 1.  Returns the result dict on
     rank 0 (None elsewhere).  ``sky``: the reference's default learnable sky (use_sky_sphere, a 1024^2 cube map stepped by
     the same Adam launch at the ``sky_sphere`` group's lr 0.005, sgn_config.py:72-75).  ``metrics``: every step also computes
-    ``get_metrics_dict`` (psnr, gaussian_count, scale / opacity / radii means), as nerfstudio's training pipeline does."""
+    ``get_metrics_dict`` (psnr, gaussian_count, scale / opacity / radii means), as nerfstudio's training pipeline does.
+    ``bbox_opt``: the reference's default box corrections (``bbox_optimizer`` mode "simple": delta_center / delta_yaw per
+    (frame, box), stepped by the same Adam launch at the ``bbox_opt`` group's lr 1e-3, sgn_config.py:80-83)."""
     import torch
     import torch.distributed as dist
 
@@ -51,7 +54,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
 
     def poses_at(t):  # fresh objects per call, as a data manager hands them out
         f = int(t)
-        return [ActorPose(str(a), rot, center, f, frame_list) for a, rot, center in sc.boxes_at(f)]
+        return [ActorPose(str(a), rot, center, f, frame_list, frame_id=f) for a, rot, center in sc.boxes_at(f)]
 
     rs = RefineSettings(refine_every=refine_every)
     cfg = SceneGraphConfig(use_sky_sphere=sky, ssim_lambda=ssim_lambda, fused_loss=fused_loss, full_gradient_arena=world > 1, refine=rs, async_binning=async_binning,
@@ -61,10 +64,17 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     if sky:
         from street_gaussians_ns_b200.sky import CubeMapSky
         env_map = CubeMapSky(1024)
+    boxes = None
+    if bbox_opt:
+        from street_gaussians_ns_b200.box_pose import BoxPoseOptimizer
+        boxes = BoxPoseOptimizer(num_frames, [str(k) for k in sc.actors], {f: f for f in range(num_frames)}, mode="simple")
     model = SceneGraphRasterModel(sc.background.to(dev), {k: v.to(dev) for k, v in sc.actors.items()}, cfg, poses_at=poses_at,
-                                  sky=env_map).to(dev)
+                                  sky=env_map, bbox_optimizer=boxes).to(dev)
     model.train()
-    extra = {"sky": (model.env_map.base, 0.005)} if sky else None
+    extra = {"sky": (model.env_map.base, 0.005)} if sky else {}
+    if bbox_opt:
+        extra["bbox_opt.delta_center"] = (boxes.delta_center, 1e-3)
+        extra["bbox_opt.delta_yaw"] = (boxes.delta_yaw, 1e-3)
     opt = FusedAdam(model.optimizer_params(), extra=extra, reserve_spare=True)  # no cudaMalloc of moment arenas inside the training loop
     step_fn = TrainStep(model, opt, refine_every=refine_every, pipeline_chunks=pipeline_chunks, overlap=overlap, metrics=metrics)
     g = torch.Generator().manual_seed(5)
@@ -173,6 +183,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                                f"{W}x{H}; rank r renders camera (step*g + r) mod 425; actors have a box within {actor_range} m of the ego vehicle",
                    "parallelism": f"camera-sharded dp{world}", "ssim_lambda": ssim_lambda,
                    **({"sky": "CubeMapSky(1024), Adam lr 0.005"} if sky else {}),
+                   **({"bbox_opt": "BoxPoseOptimizer(simple), Adam lr 1e-3"} if bbox_opt else {}),
                    "loss": "fused kernels" if fused_loss else "torch ops", "metrics": "get_metrics_dict every step" if metrics else "none",
                    "start_step": start_step, "refine_every": refine_every,
                    "refinement_kernels_loaded_before_timing": refine_warm,
@@ -203,6 +214,7 @@ def main():
     ap.add_argument("--torch-loss", action="store_true", help="loss terms as torch ops (SceneGraphConfig.fused_loss = False)")
     ap.add_argument("--sky", action="store_true", help="train the learnable sky cube map (the reference's use_sky_sphere = True)")
     ap.add_argument("--metrics", action="store_true", help="get_metrics_dict every step, between get_outputs and get_loss_dict")
+    ap.add_argument("--bbox-opt", action="store_true", help="train the box corrections (the reference's bbox_optimizer mode 'simple')")
     args = ap.parse_args()
 
     import torch
@@ -215,7 +227,7 @@ def main():
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     res = run(args.steps, args.warmup, args.scale, args.refine_every, args.start_step, args.actor_range, args.pipeline_chunks,
               args.overlap, not args.host_table, ssim_lambda=args.ssim_lambda, fused_loss=not args.torch_loss, sky=args.sky,
-              metrics=args.metrics)
+              metrics=args.metrics, bbox_opt=args.bbox_opt)
     if res is not None:
         print(json.dumps(res))
     if world > 1:
