@@ -179,6 +179,43 @@ int sgn_project_bwd_pose(const sgn_segment* segs_dev, const sgn_segment_grads* g
 int sgn_pose_grad_reduce(const sgn_segment* segs_dev, int nseg, int num_chunks, const float* pose_partials, float* v_pose,
                          void* stream);
 
+/* ---- the view on the device (camera pose optimisation) ------------------------------------------------------------------
+ * `view` is a DEVICE array of SGN_VIEW_FLOATS + 3 floats: viewmat[12] (world->camera 3x4, row-major), then cam_pos[3]; it
+ * replaces cam->viewmat / cam->cam_pos (every other field of `cam` is used as given).  A view computed on the device --
+ * sgn_camera_adjust_fwd -- thus reaches the projection without a host read-back.
+ * sgn_project_fwd_view: sgn_project_fwd (its direct form) with that view; with the camera's own view the outputs are the
+ * same bits.  sgn_project_bwd_view: sgn_project_bwd_range with that view that also stores, per 128-row chunk of
+ * [chunk_begin, chunk_end), the sums over its rows of the cotangent of viewmat[12] (v_W = sum v_pc p_w^T + 2 G W S_w,
+ * v_c = sum v_pc; p_c = W p_w + c and S_c = W S_w W^T the camera-space mean and covariance, v_pc and G their cotangents) to
+ * view_partials[num_chunks, SGN_VIEW_FLOATS]; cam_pos only orients the SH colour, whose view direction is treated as
+ * constant, so it gets no cotangent.  With pose_partials non-NULL it also yields the pose sums of sgn_project_bwd_pose.
+ * The parameter gradients are bit-identical to sgn_project_bwd_range's.  sgn_view_grad_reduce, after the last range,
+ * sums all chunks into v_view[SGN_VIEW_FLOATS] in a fixed order: no atomics, the same bits on every run. */
+#define SGN_VIEW_FLOATS 12
+int sgn_project_fwd_view(const sgn_segment* segs_dev, int nseg, int N, int num_chunks, const sgn_camera* cam, const float* view,
+                         float* records, int32_t* radii, int32_t* num_tiles_hit, uint16_t* tile_bbox, int32_t* tiles_touched,
+                         uint32_t* touch_mask, void* stream);
+int sgn_project_bwd_view(const sgn_segment* segs_dev, const sgn_segment_grads* grads_dev, int nseg, int N, int num_chunks,
+                         const sgn_camera* cam, const float* view, const float* records, const int32_t* radii,
+                         const float* v_records, int chunk_begin, int chunk_end, float* pose_partials /* or NULL */,
+                         float* view_partials, void* stream);
+int sgn_view_grad_reduce(int num_chunks, const float* view_partials, float* v_view, void* stream);
+
+/* nerfstudio's CameraOptimizer, mode "SO3xR3" (cameras/camera_optimizers.py, lie_groups.py), one launch each way.
+ * pose_adjustment: device, float32 [num_cameras, 6] (translation 0:3, axis-angle 3:6).
+ * Forward: reg[1] (device) = mean_rows |x[:, 0:3]| w_t + mean_rows |x[:, 3:6]| w_r (the regulariser), norms[2] (device) =
+ * {|x[:, 0:3]|, |x[:, 3:6]|} (Frobenius norms); sums in a fixed order.  With cam_idx >= 0 also the corrected view of that camera:
+ * x = pose_adjustment[cam_idx], theta = sqrt(max(|w|^2, 1e-4)), R_a = I + sin(theta)/theta K + (1 - cos(theta))/theta^2 K^2
+ * (K = skew(w)), t_a = x[0:3];  c2w' = c2w [R_a t_a; 0 1];  view = (viewmat of c2w' as Camera._viewmat builds it, then
+ * cam_pos = c2w'[:3, 3]), float32.  c2w: 12 HOST floats (3x4 row-major), ignored (may be NULL) when cam_idx == -1.
+ * Backward: writes EVERY row of v_pose_adjustment: the regulariser's gradient for the cotangent g_reg[0] (device scalar; a
+ * row with a zero norm gets zero from that norm, as torch gives) plus, in row cam_idx, the chain from v_view[SGN_VIEW_FLOATS]
+ * (cam_pos has no cotangent, see above).  g_reg / v_view NULL: that share is zero. */
+int sgn_camera_adjust_fwd(const float* pose_adjustment, int num_cameras, int cam_idx, const float* c2w, float w_t, float w_r,
+                          float* view, float* reg, float* norms, void* stream);
+int sgn_camera_adjust_bwd(const float* pose_adjustment, int num_cameras, int cam_idx, const float* c2w, float w_t, float w_r,
+                          const float* v_view, const float* g_reg, float* v_pose_adjustment, void* stream);
+
 /* ---- Level-1: gsplat 0.1.x function API on plain tensors (sgn_splatfacto.py:11-14) -------------------
  * gsplat.project_gaussians(means3d, scales, glob_scale, quats, viewmat, fx, fy, cx, cy, H, W, block_width,
  * clip_thresh) -> xys[N,2], depths[N], radii[N] i32, conics[N,3], compensation[N], num_tiles_hit[N] i32,
@@ -403,6 +440,14 @@ int sgn_sky_bwd_det(const sgn_camera* cam, const float* jitter_u, const float* j
                     void* scratch, size_t scratch_bytes, void* stream);
 int sgn_cube_texture_bwd_det(int P, const float* uv, int R, const float* v_out, float* v_tex, void* scratch, size_t scratch_bytes,
                              void* stream);
+/* The three camera-path sky entry points with c2w[:3,:3] recovered from a DEVICE view (viewmat[12], cam_pos[3]; see
+ * sgn_project_fwd_view) instead of cam->viewmat, by the same exact transpose and negation.  No cotangent for the view. */
+int sgn_sky_fwd_view(const sgn_camera* cam, const float* view, const float* jitter_u, const float* jitter_v, const float* tex, int R,
+                     float* sky, float* dirs, void* stream);
+int sgn_sky_bwd_view(const sgn_camera* cam, const float* view, const float* jitter_u, const float* jitter_v, int R, const float* v_sky,
+                     float* v_tex, void* stream);
+int sgn_sky_bwd_det_view(const sgn_camera* cam, const float* view, const float* jitter_u, const float* jitter_v, int R,
+                         const float* v_sky, float* v_tex, void* scratch, size_t scratch_bytes, void* stream);
 
 /* ---- densification statistics (SURVEY.md 8f rank 3) -------------------------------------------------------
  * What each sub-model's `after_train` accumulates after backward (sgn_splatfacto.py:513-541), for all visible

@@ -135,7 +135,10 @@ EXPORTS = [
     "sgn_bin_local_cap", "sgn_bin_local_scratch_bytes", "sgn_bin_local_count", "sgn_bin_local_sort",
     "sgn_project_bwd_range", "sgn_allreduce_sym", "sgn_blend_extra_fwd", "sgn_blend_extra_bwd", "sgn_blend_extra_bwd_det",
     "sgn_bin_sort_capped", "sgn_visible_flags", "sgn_visible_union", "sgn_project_bwd_pose", "sgn_pose_grad_reduce",
+    "sgn_project_fwd_view", "sgn_project_bwd_view", "sgn_view_grad_reduce", "sgn_sky_fwd_view", "sgn_sky_bwd_view",
+    "sgn_sky_bwd_det_view", "sgn_camera_adjust_fwd", "sgn_camera_adjust_bwd",
 ]
+VIEW_FLOATS = 12  # SGN_VIEW_FLOATS: the view's cotangent, viewmat[12] row-major; the device view itself is 12 + 3 (cam_pos) floats
 POSE_FLOATS = 16  # SGN_POSE_FLOATS: a segment's pose (and its cotangent) as R[9] row-major, t[3], q[4]
 AR_MAX_SLICES = 48  # SGN_AR_MAX_SLICES
 
@@ -165,6 +168,13 @@ def load():
     L.sgn_project_bwd_pose.argtypes = [vp, vp, i32, i32, i32, C.POINTER(CameraStruct), vp, vp, vp, i32, i32, vp, vp]
     L.sgn_pose_grad_reduce.argtypes = [vp, i32, i32, vp, vp, vp]
     L.sgn_project_bwd_pose.restype = L.sgn_pose_grad_reduce.restype = C.c_int
+    L.sgn_project_fwd_view.argtypes = [vp, i32, i32, i32, C.POINTER(CameraStruct), vp, vp, vp, vp, vp, vp, vp, vp]
+    L.sgn_project_bwd_view.argtypes = [vp, vp, i32, i32, i32, C.POINTER(CameraStruct), vp, vp, vp, vp, i32, i32, vp, vp, vp]
+    L.sgn_view_grad_reduce.argtypes = [i32, vp, vp, vp]
+    L.sgn_camera_adjust_fwd.argtypes = [vp, i32, i32, C.POINTER(C.c_float), C.c_float, C.c_float, vp, vp, vp, vp]
+    L.sgn_camera_adjust_bwd.argtypes = [vp, i32, i32, C.POINTER(C.c_float), C.c_float, C.c_float, vp, vp, vp, vp]
+    for f in ("sgn_project_fwd_view", "sgn_project_bwd_view", "sgn_view_grad_reduce", "sgn_camera_adjust_fwd", "sgn_camera_adjust_bwd"):
+        getattr(L, f).restype = C.c_int
     L.sgn_allreduce_sym.argtypes = [vp, vp, vp, i32, i32, i32, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int32),
                                     C.POINTER(C.c_int64), C.POINTER(C.c_int64), vp, C.c_float, i32, vp]
     L.sgn_visible_flags.argtypes = [vp, i64, vp, vp]
@@ -234,7 +244,11 @@ def load():
     L.sgn_sky_det_scratch_bytes.restype = sz
     L.sgn_sky_bwd_det.argtypes = [C.POINTER(CameraStruct), vp, vp, i32, vp, vp, vp, sz, vp]
     L.sgn_cube_texture_bwd_det.argtypes = [i32, vp, i32, vp, vp, vp, sz, vp]
-    for f in ("sgn_sky_fwd", "sgn_sky_bwd", "sgn_cube_texture_fwd", "sgn_cube_texture_bwd", "sgn_sky_bwd_det", "sgn_cube_texture_bwd_det"):
+    L.sgn_sky_fwd_view.argtypes = [C.POINTER(CameraStruct), vp, vp, vp, vp, i32, vp, vp, vp]
+    L.sgn_sky_bwd_view.argtypes = [C.POINTER(CameraStruct), vp, vp, vp, i32, vp, vp, vp]
+    L.sgn_sky_bwd_det_view.argtypes = [C.POINTER(CameraStruct), vp, vp, vp, i32, vp, vp, vp, sz, vp]
+    for f in ("sgn_sky_fwd", "sgn_sky_bwd", "sgn_cube_texture_fwd", "sgn_cube_texture_bwd", "sgn_sky_bwd_det", "sgn_cube_texture_bwd_det",
+              "sgn_sky_fwd_view", "sgn_sky_bwd_view", "sgn_sky_bwd_det_view"):
         getattr(L, f).restype = C.c_int
     L.sgn_sizeof_adam_tensor.restype = sz
     L.sgn_adam_chunk_elems.restype = C.c_int

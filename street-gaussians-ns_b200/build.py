@@ -30,6 +30,7 @@ SOURCES = {
     "adam.cu": ["--fmad=false"],  # keep torch.optim.Adam's rounding sequence (no contraction)
     "refine.cu": ["--fmad=false"],
     "collective.cu": [],  # the refinement rules mirror torch's separately rounded elementwise kernels
+    "camera.cu": [],  # IEEE sinf / cosf / sqrtf (no fast math)
 }
 
 

@@ -48,6 +48,16 @@ extern "C" int sgn_upload(const void* host, size_t bytes, void* dev, void* strea
 #define MAX_REST 45       // (4^2 - 1) * 3
 #define MAX_DC (3 * SGN_MAX_FOURIER)
 
+// the camera struct with its view (viewmat[12], then cam_pos[3]) replaced by the 15 floats at `view` (device memory)
+__device__ __forceinline__ sgn_camera sgn_camera_with_view(const sgn_camera& c, const float* __restrict__ view) {
+    sgn_camera o = c;
+#pragma unroll
+    for (int k = 0; k < 12; ++k) o.viewmat[k] = __ldg(view + k);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) o.cam_pos[k] = __ldg(view + 12 + k);
+    return o;
+}
+
 __device__ __forceinline__ int find_segment_by_chunk(const int* s_chunk0, int nseg, int c) {
     int lo = 0, hi = nseg - 1;
     while (lo < hi) {
@@ -85,10 +95,17 @@ __device__ __forceinline__ void coop_store(float* __restrict__ dst, const float*
 // Forward: one thread per row, direct loads (independent per-thread loads keep more requests in flight
 // than a stage-sync-compute split; measured).  Rows the camera does not see skip the colour work:
 // nothing downstream ever reads the colour of an invisible Gaussian.
+// VIEW: the world->camera view (viewmat[12], cam_pos[3]) is read from the device (`view`) instead of the camera struct --
+// a view computed on the device (camera pose optimisation) reaches the kernel without a host read-back.
+template <bool VIEW>
 __global__ void __launch_bounds__(CH)
-project_fwd_direct_kernel(const sgn_segment* __restrict__ segs, int nseg, const sgn_camera cam,
+project_fwd_direct_kernel(const sgn_segment* __restrict__ segs, int nseg, const sgn_camera cam_arg,
                    float4* __restrict__ records, int32_t* __restrict__ radii, int32_t* __restrict__ num_tiles_hit,
-                   ushort4* __restrict__ tile_bbox, int32_t* __restrict__ tiles_touched, uint32_t* __restrict__ touch_mask) {
+                   ushort4* __restrict__ tile_bbox, int32_t* __restrict__ tiles_touched, uint32_t* __restrict__ touch_mask,
+                   const float* __restrict__ view) {
+    sgn_camera cam_view;
+    if constexpr (VIEW) cam_view = sgn_camera_with_view(cam_arg, view);
+    const sgn_camera& cam = VIEW ? cam_view : cam_arg;
     extern __shared__ int s_chunk0[];
     for (int i = threadIdx.x; i < nseg; i += blockDim.x) s_chunk0[i] = segs[i].chunk0;
     __syncthreads();
@@ -339,20 +356,43 @@ project_fwd_staged_kernel(const sgn_segment* __restrict__ segs, int nseg, const 
     }
 }
 
-extern "C" int sgn_project_fwd(const sgn_segment* segs_dev, int nseg, int N, int num_chunks, const sgn_camera* cam,
-                               float* records, int32_t* radii, int32_t* num_tiles_hit, uint16_t* tile_bbox,
-                               int32_t* tiles_touched, uint32_t* touch_mask, void* stream) {
-    SGN_RANGE("sgn_project_fwd");
+static int project_fwd_check(const char* what, const sgn_segment* segs_dev, int nseg, int N, int num_chunks, const sgn_camera* cam,
+                             float* records, int32_t* radii, int32_t* num_tiles_hit, uint16_t* tile_bbox,
+                             int32_t* tiles_touched, uint32_t* touch_mask) {
     SGN_REQUIRE(segs_dev && cam && records && radii && num_tiles_hit && tile_bbox && tiles_touched && touch_mask,
-                "sgn_project_fwd: null pointer");
-    SGN_REQUIRE(nseg >= 1 && nseg <= SGN_MAX_SEGMENTS, "sgn_project_fwd: nseg=%d out of range [1,%d]", nseg, SGN_MAX_SEGMENTS);
-    SGN_REQUIRE(N >= 0 && num_chunks >= 0, "sgn_project_fwd: negative size");
+                "%s: null pointer", what);
+    SGN_REQUIRE(nseg >= 1 && nseg <= SGN_MAX_SEGMENTS, "%s: nseg=%d out of range [1,%d]", what, nseg, SGN_MAX_SEGMENTS);
+    SGN_REQUIRE(N >= 0 && num_chunks >= 0, "%s: negative size", what);
     SGN_REQUIRE(cam->block_width >= 2 && cam->block_width <= 16, "block_width must be between 2 and 16 (got %d)", cam->block_width);
     SGN_REQUIRE(cam->sh_degree >= 0 && cam->sh_degree <= 3 && cam->sh_degree_to_use >= 0 && cam->sh_degree_to_use <= cam->sh_degree,
                 "sh_degree must be in [0,3] and sh_degree_to_use <= sh_degree");
     SGN_REQUIRE((cam->width + cam->block_width - 1) / cam->block_width < 65536 && (cam->height + cam->block_width - 1) / cam->block_width < 65536,
                 "image too large for 16-bit tile coordinates");
     SGN_REQUIRE(sgn_aligned16(records), "records must be 16-byte aligned");
+    return SGN_OK;
+}
+
+extern "C" int sgn_project_fwd_view(const sgn_segment* segs_dev, int nseg, int N, int num_chunks, const sgn_camera* cam,
+                                    const float* view, float* records, int32_t* radii, int32_t* num_tiles_hit, uint16_t* tile_bbox,
+                                    int32_t* tiles_touched, uint32_t* touch_mask, void* stream) {
+    SGN_RANGE("sgn_project_fwd_view");
+    if (int rc = project_fwd_check("sgn_project_fwd_view", segs_dev, nseg, N, num_chunks, cam, records, radii, num_tiles_hit, tile_bbox,
+                                   tiles_touched, touch_mask)) return rc;
+    SGN_REQUIRE(view, "sgn_project_fwd_view: null view");
+    if (N == 0 || num_chunks == 0) return SGN_OK;
+    project_fwd_direct_kernel<true><<<num_chunks, CH, nseg * sizeof(int), (cudaStream_t)stream>>>(
+        segs_dev, nseg, *cam, reinterpret_cast<float4*>(records), radii, num_tiles_hit,
+        reinterpret_cast<ushort4*>(tile_bbox), tiles_touched, touch_mask, view);
+    SGN_CHECK_LAUNCH("project_fwd_kernel<view>");
+    return SGN_OK;
+}
+
+extern "C" int sgn_project_fwd(const sgn_segment* segs_dev, int nseg, int N, int num_chunks, const sgn_camera* cam,
+                               float* records, int32_t* radii, int32_t* num_tiles_hit, uint16_t* tile_bbox,
+                               int32_t* tiles_touched, uint32_t* touch_mask, void* stream) {
+    SGN_RANGE("sgn_project_fwd");
+    if (int rc = project_fwd_check("sgn_project_fwd", segs_dev, nseg, N, num_chunks, cam, records, radii, num_tiles_hit, tile_bbox,
+                                   tiles_touched, touch_mask)) return rc;
     if (N == 0 || num_chunks == 0) return SGN_OK;
     // SGN_PROJECT_STAGED=1: the two-phase form (compaction + shared-memory staging of the visible rows' colour parameters);
     // the direct form is the default.  Read on every call (one getenv per frame), so one process can run both forms.
@@ -362,17 +402,23 @@ extern "C" int sgn_project_fwd(const sgn_segment* segs_dev, int nseg, int N, int
             segs_dev, nseg, *cam, reinterpret_cast<float4*>(records), radii, num_tiles_hit,
             reinterpret_cast<ushort4*>(tile_bbox), tiles_touched, touch_mask);
     else
-        project_fwd_direct_kernel<<<num_chunks, CH, nseg * sizeof(int), (cudaStream_t)stream>>>(
+        project_fwd_direct_kernel<false><<<num_chunks, CH, nseg * sizeof(int), (cudaStream_t)stream>>>(
             segs_dev, nseg, *cam, reinterpret_cast<float4*>(records), radii, num_tiles_hit,
-            reinterpret_cast<ushort4*>(tile_bbox), tiles_touched, touch_mask);
+            reinterpret_cast<ushort4*>(tile_bbox), tiles_touched, touch_mask, nullptr);
     SGN_CHECK_LAUNCH("project_fwd_kernel");
     return SGN_OK;
 }
 
 // geometry backward shared by the fused and the Level-1 kernels: cotangents of (xy, depth, conic) ->
-// (world mean, scale as used [st.s], composed quaternion qr)
+// (world mean, scale as used [st.s], composed quaternion qr).
+// VIEW: also this row's cotangent of the view [W | c] (viewmat[12] row-major) into vview.  With the camera-space mean
+// p_c = W p_w + c and covariance S_c = W S_w W^T: v_W = v_pc p_w^T + 2 G W S_w, v_c = v_pc, where v_pc (vpv below) is the
+// complete cotangent of p_c (xy, depth and the Jacobian's dependence on p_c) and G = J^T g J that of S_c; 2 G W S_w = J^T vT
+// since T = J W and vT = 2 g T S_w.
+template <bool VIEW = false>
 __device__ __forceinline__ void sgn_project_vjp(const sgn_camera& cam, const SgnProj& st, const float v_xy[2], float v_depth,
-                                                const float v_conic[3], float vmw[3], float vs[3], float vqr[4]) {
+                                                const float v_conic[3], float vmw[3], float vs[3], float vqr[4],
+                                                float* vview = nullptr) {
     const float* W = cam.viewmat;
     const float fx = cam.fx, fy = cam.fy;
     float vpv[3];
@@ -425,6 +471,17 @@ __device__ __forceinline__ void sgn_project_vjp(const sgn_camera& cam, const Sgn
         if (st.clampx == 0) vpv[0] += vtx; else vpv[2] += (st.clampx > 0 ? cam.limx : -cam.limx) * vtx;
         if (st.clampy == 0) vpv[1] += vty; else vpv[2] += (st.clampy > 0 ? cam.limy : -cam.limy) * vty;
         vpv[2] += vtz;
+        if constexpr (VIEW) {
+            const float J00 = fx * rz, J11 = fy * rz, J02 = -fx * st.tx * rz2, J12 = -fy * st.ty * rz2;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                vview[c] = vpv[0] * st.mw[c] + J00 * vT[c];
+                vview[4 + c] = vpv[1] * st.mw[c] + J11 * vT[3 + c];
+                vview[8 + c] = vpv[2] * st.mw[c] + J02 * vT[c] + J12 * vT[3 + c];
+            }
+#pragma unroll
+            for (int r = 0; r < 3; ++r) vview[4 * r + 3] = vpv[r];
+        }
     }
 #pragma unroll
     for (int c = 0; c < 3; ++c) vmw[c] = W[c] * vpv[0] + W[4 + c] * vpv[1] + W[8 + c] * vpv[2];
@@ -465,11 +522,17 @@ __device__ __forceinline__ void sgn_project_vjp(const sgn_camera& cam, const Sgn
 // v_R[r][c] = sum vmw[r] m[c] (means_w = R m + t), v_t = sum vmw, v_a = sum vqr (x) conj(q) (q_w = a (x) q, q un-normalised) --
 // and stores the 16 sums to pose_partials[chunk]: warp shuffles, then the four warps in fixed order; no atomics, so the
 // sums do not depend on the run.  Colour contributes nothing (the SH view direction is taken from detached means).
-template <bool POSE>
+// VIEW: the view is read from the device (`view`, as in the forward) and every block also reduces the rows' cotangents of
+// it (sgn_project_vjp<true>) the same way, storing SGN_VIEW_FLOATS sums to view_partials[chunk].
+template <bool POSE, bool VIEW = false>
 __global__ void __launch_bounds__(CH)
 project_bwd_kernel(const sgn_segment* __restrict__ segs, const sgn_segment_grads* __restrict__ grads, int nseg,
-                   const sgn_camera cam, const float4* __restrict__ records, const int32_t* __restrict__ radii,
-                   const float4* __restrict__ v_records, const int chunk_begin, float* __restrict__ pose_partials) {
+                   const sgn_camera cam_arg, const float4* __restrict__ records, const int32_t* __restrict__ radii,
+                   const float4* __restrict__ v_records, const int chunk_begin, float* __restrict__ pose_partials,
+                   const float* __restrict__ view, float* __restrict__ view_partials) {
+    sgn_camera cam_view;
+    if constexpr (VIEW) cam_view = sgn_camera_with_view(cam_arg, view);
+    const sgn_camera& cam = VIEW ? cam_view : cam_arg;
     extern __shared__ int s_chunk0[];
     __shared__ __align__(16) float s_rest[CH * MAX_REST];   // out: features_rest gradient rows
     __shared__ __align__(16) float s_dc[CH * MAX_DC];       // out: features_dc gradient rows
@@ -491,6 +554,7 @@ project_bwd_kernel(const sgn_segment* __restrict__ segs, const sgn_segment_grads
     const int tid = threadIdx.x;
     float gm[3] = {0.f, 0.f, 0.f}, gs[3] = {0.f, 0.f, 0.f}, gq[4] = {0.f, 0.f, 0.f, 0.f};
     float vp[POSE ? SGN_POSE_FLOATS : 1] = {};  // this row's share of (v_R 9, v_t 3, v_a 4)
+    float vv[VIEW ? SGN_VIEW_FLOATS : 1] = {};  // this row's share of v_view
     const bool row_vis = (tid < rows) && radii[(size_t)sg.row0 + r0 + tid] > 0;
     if (tid < rows && !row_vis) {
         // the rasterizer never touched this Gaussian: every cotangent is zero, so is every gradient
@@ -561,7 +625,7 @@ project_bwd_kernel(const sgn_segment* __restrict__ segs, const sgn_segment_grads
         }
         if (vis && radii[g] > 0) {
             float vmw[3], vs[3], vqr[4];
-            sgn_project_vjp(cam, st, v_xy, v_depth, v_conic, vmw, vs, vqr);
+            sgn_project_vjp<VIEW>(cam, st, v_xy, v_depth, v_conic, vmw, vs, vqr, vv);
 #pragma unroll
             for (int c = 0; c < 3; ++c) gs[c] = vs[c] * st.s[c];  // through exp
             if (sg.has_pose) {
@@ -613,6 +677,23 @@ project_bwd_kernel(const sgn_segment* __restrict__ segs, const sgn_segment_grads
             }
         }
     }
+    if constexpr (VIEW) {
+        __shared__ float s_view[(CH / 32) * SGN_VIEW_FLOATS];
+#pragma unroll
+        for (int k = 0; k < SGN_VIEW_FLOATS; ++k) {
+            float x = vv[k];
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) x += __shfl_down_sync(0xffffffffu, x, o);
+            if ((tid & 31) == 0) s_view[(tid >> 5) * SGN_VIEW_FLOATS + k] = x;
+        }
+        __syncthreads();
+        if (tid < SGN_VIEW_FLOATS) {
+            float x = s_view[tid];
+#pragma unroll
+            for (int w = 1; w < CH / 32; ++w) x += s_view[w * SGN_VIEW_FLOATS + tid];
+            view_partials[(size_t)chunk * SGN_VIEW_FLOATS + tid] = x;
+        }
+    }
     __syncthreads();  // every thread has consumed its means / scales inputs
     if (tid < rows) {
 #pragma unroll
@@ -627,18 +708,21 @@ project_bwd_kernel(const sgn_segment* __restrict__ segs, const sgn_segment_grads
 
 static int project_bwd_launch(const char* what, const sgn_segment* segs_dev, const sgn_segment_grads* grads_dev, int nseg, int N, int num_chunks,
                               const sgn_camera* cam, const float* records, const int32_t* radii, const float* v_records,
-                              int chunk_begin, int chunk_end, float* pose_partials, bool pose, void* stream) {
+                              int chunk_begin, int chunk_end, float* pose_partials, bool pose, void* stream,
+                              const float* view = nullptr, float* view_partials = nullptr) {
     SGN_REQUIRE(segs_dev && grads_dev && cam && records && radii && v_records, "%s: null pointer", what);
     SGN_REQUIRE(!pose || pose_partials, "%s: null pose_partials", what);
+    SGN_REQUIRE((view == nullptr) == (view_partials == nullptr), "%s: give both view and view_partials, or neither", what);
     SGN_REQUIRE(nseg >= 1 && nseg <= SGN_MAX_SEGMENTS, "%s: nseg=%d out of range", what, nseg);
     SGN_REQUIRE(sgn_aligned16(records) && sgn_aligned16(v_records), "records / v_records must be 16-byte aligned");
     SGN_REQUIRE(chunk_begin >= 0 && chunk_begin <= chunk_end && chunk_end <= num_chunks, "%s: chunk range [%d, %d) outside [0, %d)",
                 what, chunk_begin, chunk_end, num_chunks);
     if (N == 0 || chunk_end == chunk_begin) return SGN_OK;
-    auto kernel = pose ? project_bwd_kernel<true> : project_bwd_kernel<false>;
+    auto kernel = view ? (pose ? project_bwd_kernel<true, true> : project_bwd_kernel<false, true>)
+                       : (pose ? project_bwd_kernel<true, false> : project_bwd_kernel<false, false>);
     kernel<<<chunk_end - chunk_begin, CH, nseg * sizeof(int), (cudaStream_t)stream>>>(
         segs_dev, grads_dev, nseg, *cam, reinterpret_cast<const float4*>(records), radii,
-        reinterpret_cast<const float4*>(v_records), chunk_begin, pose_partials);
+        reinterpret_cast<const float4*>(v_records), chunk_begin, pose_partials, view, view_partials);
     SGN_CHECK_LAUNCH("project_bwd_kernel");
     return SGN_OK;
 }
@@ -663,6 +747,45 @@ extern "C" int sgn_project_bwd_pose(const sgn_segment* segs_dev, const sgn_segme
     SGN_RANGE("sgn_project_bwd_pose");
     return project_bwd_launch("sgn_project_bwd_pose", segs_dev, grads_dev, nseg, N, num_chunks, cam, records, radii, v_records,
                               chunk_begin, chunk_end, pose_partials, true, stream);
+}
+
+extern "C" int sgn_project_bwd_view(const sgn_segment* segs_dev, const sgn_segment_grads* grads_dev, int nseg, int N, int num_chunks,
+                                    const sgn_camera* cam, const float* view, const float* records, const int32_t* radii,
+                                    const float* v_records, int chunk_begin, int chunk_end, float* pose_partials, float* view_partials,
+                                    void* stream) {
+    SGN_RANGE("sgn_project_bwd_view");
+    SGN_REQUIRE(view && view_partials, "sgn_project_bwd_view: null view or view_partials");
+    return project_bwd_launch("sgn_project_bwd_view", segs_dev, grads_dev, nseg, N, num_chunks, cam, records, radii, v_records,
+                              chunk_begin, chunk_end, pose_partials, pose_partials != nullptr, stream, view, view_partials);
+}
+
+// One block of VR_THREADS = 80 x SGN_VIEW_FLOATS threads: thread t sums the floats t, t + VR_THREADS, ... of view_partials
+// (all of one value k = t % 12, coalesced), in ascending order; then thread k < 12 sums the 80 partial sums of value k in
+// ascending order.  A fixed order throughout: v_view is the same bits on every run.
+#define VR_THREADS (80 * SGN_VIEW_FLOATS)
+__global__ void __launch_bounds__(VR_THREADS)
+view_reduce_kernel(int num_chunks, const float* __restrict__ view_partials, float* __restrict__ v_view) {
+    __shared__ float s_sum[VR_THREADS];
+    const int tid = threadIdx.x;
+    const long long n = (long long)num_chunks * SGN_VIEW_FLOATS;
+    float x = 0.f;
+    for (long long e = tid; e < n; e += VR_THREADS) x += __ldg(view_partials + e);
+    s_sum[tid] = x;
+    __syncthreads();
+    if (tid < SGN_VIEW_FLOATS) {
+        float y = 0.f;
+        for (int j = tid; j < VR_THREADS; j += SGN_VIEW_FLOATS) y += s_sum[j];
+        v_view[tid] = y;
+    }
+}
+
+extern "C" int sgn_view_grad_reduce(int num_chunks, const float* view_partials, float* v_view, void* stream) {
+    SGN_RANGE("sgn_view_grad_reduce");
+    SGN_REQUIRE(v_view, "sgn_view_grad_reduce: null v_view");
+    SGN_REQUIRE(num_chunks >= 0 && (num_chunks == 0 || view_partials), "sgn_view_grad_reduce: null view_partials for %d chunks", num_chunks);
+    view_reduce_kernel<<<1, VR_THREADS, 0, (cudaStream_t)stream>>>(num_chunks, view_partials, v_view);
+    SGN_CHECK_LAUNCH("view_reduce_kernel");
+    return SGN_OK;
 }
 
 // One warp per segment: the sums of pose_partials over the segment's chunks, in a fixed order (lane = value + 16 x chunk

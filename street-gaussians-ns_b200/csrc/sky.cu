@@ -266,10 +266,25 @@ static __device__ __forceinline__ float3 item_direction(const SkyCam& c, const f
     return make_float3(uv[3 * p], uv[3 * p + 1], uv[3 * p + 2]);
 }
 
-template <bool CAM>
-__global__ void __launch_bounds__(SKY_THREADS) cube_fwd_kernel(const SkyCam c, const float* __restrict__ ju, const float* __restrict__ jv,
+// c2w[:3,:3] from a device view (viewmat[12] row-major, then cam_pos[3]): the transpose and negation of sky_cam, exact
+static __device__ __forceinline__ SkyCam sky_cam_with_view(const SkyCam& c, const float* __restrict__ view) {
+    SkyCam o = c;
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) o.R[3 * i + j] = j == 0 ? __ldg(view + 4 * j + i) : -__ldg(view + 4 * j + i);
+    return o;
+}
+
+// VIEW: the camera's rotation is read from `view` (device memory) instead of c.R
+template <bool CAM, bool VIEW = false>
+__global__ void __launch_bounds__(SKY_THREADS) cube_fwd_kernel(const SkyCam c_arg, const float* __restrict__ ju, const float* __restrict__ jv,
                                                                const float* __restrict__ uv, int P, const float* __restrict__ tex, int R,
-                                                               float* __restrict__ out, float* __restrict__ dirs) {
+                                                               float* __restrict__ out, float* __restrict__ dirs,
+                                                               const float* __restrict__ view) {
+    SkyCam c_view;
+    if constexpr (VIEW) c_view = sky_cam_with_view(c_arg, view);
+    const SkyCam& c = VIEW ? c_view : c_arg;
     const int p = blockIdx.x * SKY_THREADS + threadIdx.x;
     if (p >= P) return;
     const float3 l = item_direction<CAM>(c, ju, jv, uv, p);
@@ -289,10 +304,13 @@ __global__ void __launch_bounds__(SKY_THREADS) cube_fwd_kernel(const SkyCam c, c
 
 // DET = false: float atomics into v_tex.  DET = true: v_tex is the fixed-point scratch, int64 [6,R,R,3] followed by the
 // grid scale (one float), and the box holds int64 (SKY_DET_BOX_TEXELS).  The float instantiations carry no fixed-point code.
-template <bool CAM, bool DET>
-__global__ void __launch_bounds__(SKY_THREADS) cube_bwd_kernel(const SkyCam c, const float* __restrict__ ju, const float* __restrict__ jv,
+template <bool CAM, bool DET, bool VIEW = false>
+__global__ void __launch_bounds__(SKY_THREADS) cube_bwd_kernel(const SkyCam c_arg, const float* __restrict__ ju, const float* __restrict__ jv,
                                                                const float* __restrict__ uv, int P, int R, const float* __restrict__ v_out,
-                                                               SkyAcc<DET>* __restrict__ v_tex) {
+                                                               SkyAcc<DET>* __restrict__ v_tex, const float* __restrict__ view) {
+    SkyCam c_view;
+    if constexpr (VIEW) c_view = sky_cam_with_view(c_arg, view);
+    const SkyCam& c = VIEW ? c_view : c_arg;
     constexpr int BOX_TEXELS = DET ? SKY_DET_BOX_TEXELS : SKY_BOX_TEXELS;
     __shared__ SkyAcc<DET> box[BOX_TEXELS * 3];
     __shared__ int s_dom, s_lo[2], s_hi[2];
@@ -429,33 +447,60 @@ static int check_jitter(const float* ju, const float* jv, const char* who) {
     return SGN_OK;
 }
 
+// the camera-path forward / backward, with the camera's rotation from `view` (device) when it is non-NULL
+static int sky_fwd(const char* who, const sgn_camera* cam, const float* view, const float* jitter_u, const float* jitter_v, const float* tex,
+                   int R, float* sky, float* dirs, void* stream) {
+    SkyCam c;
+    if (int rc = sky_cam(c, cam, who)) return rc;
+    if (int rc = check_res(R, who)) return rc;
+    if (int rc = check_jitter(jitter_u, jitter_v, who)) return rc;
+    SGN_REQUIRE(tex && sky, "%s: null texture or output", who);
+    const int P = c.W * c.H;
+    auto kernel = view ? cube_fwd_kernel<true, true> : cube_fwd_kernel<true, false>;
+    kernel<<<(P + SKY_THREADS - 1) / SKY_THREADS, SKY_THREADS, 0, (cudaStream_t)stream>>>(c, jitter_u, jitter_v, nullptr, P, tex, R, sky,
+                                                                                          dirs, view);
+    SGN_CHECK_LAUNCH("cube_fwd_kernel<camera>");
+    return SGN_OK;
+}
+
+static int sky_bwd(const char* who, const sgn_camera* cam, const float* view, const float* jitter_u, const float* jitter_v, int R,
+                   const float* v_sky, float* v_tex, void* stream) {
+    SkyCam c;
+    if (int rc = sky_cam(c, cam, who)) return rc;
+    if (int rc = check_res(R, who)) return rc;
+    if (int rc = check_jitter(jitter_u, jitter_v, who)) return rc;
+    SGN_REQUIRE(v_sky && v_tex, "%s: null v_sky or v_tex", who);
+    const dim3 grid((c.W + SKY_TILE - 1) / SKY_TILE, (c.H + SKY_TILE - 1) / SKY_TILE);
+    auto kernel = view ? cube_bwd_kernel<true, false, true> : cube_bwd_kernel<true, false, false>;
+    kernel<<<grid, SKY_THREADS, 0, (cudaStream_t)stream>>>(c, jitter_u, jitter_v, nullptr, c.W * c.H, R, v_sky, v_tex, view);
+    SGN_CHECK_LAUNCH("cube_bwd_kernel<camera>");
+    return SGN_OK;
+}
+
 extern "C" int sgn_sky_fwd(const sgn_camera* cam, const float* jitter_u, const float* jitter_v, const float* tex, int R, float* sky,
                            float* dirs, void* stream) {
     SGN_RANGE("sgn_sky_fwd");
-    SkyCam c;
-    if (int rc = sky_cam(c, cam, "sgn_sky_fwd")) return rc;
-    if (int rc = check_res(R, "sgn_sky_fwd")) return rc;
-    if (int rc = check_jitter(jitter_u, jitter_v, "sgn_sky_fwd")) return rc;
-    SGN_REQUIRE(tex && sky, "sgn_sky_fwd: null texture or output");
-    const int P = c.W * c.H;
-    cube_fwd_kernel<true><<<(P + SKY_THREADS - 1) / SKY_THREADS, SKY_THREADS, 0, (cudaStream_t)stream>>>(c, jitter_u, jitter_v, nullptr, P, tex,
-                                                                                                          R, sky, dirs);
-    SGN_CHECK_LAUNCH("cube_fwd_kernel<camera>");
-    return SGN_OK;
+    return sky_fwd("sgn_sky_fwd", cam, nullptr, jitter_u, jitter_v, tex, R, sky, dirs, stream);
+}
+
+extern "C" int sgn_sky_fwd_view(const sgn_camera* cam, const float* view, const float* jitter_u, const float* jitter_v, const float* tex,
+                                int R, float* sky, float* dirs, void* stream) {
+    SGN_RANGE("sgn_sky_fwd_view");
+    SGN_REQUIRE(view, "sgn_sky_fwd_view: null view");
+    return sky_fwd("sgn_sky_fwd_view", cam, view, jitter_u, jitter_v, tex, R, sky, dirs, stream);
 }
 
 extern "C" int sgn_sky_bwd(const sgn_camera* cam, const float* jitter_u, const float* jitter_v, int R, const float* v_sky, float* v_tex,
                            void* stream) {
     SGN_RANGE("sgn_sky_bwd");
-    SkyCam c;
-    if (int rc = sky_cam(c, cam, "sgn_sky_bwd")) return rc;
-    if (int rc = check_res(R, "sgn_sky_bwd")) return rc;
-    if (int rc = check_jitter(jitter_u, jitter_v, "sgn_sky_bwd")) return rc;
-    SGN_REQUIRE(v_sky && v_tex, "sgn_sky_bwd: null v_sky or v_tex");
-    const dim3 grid((c.W + SKY_TILE - 1) / SKY_TILE, (c.H + SKY_TILE - 1) / SKY_TILE);
-    cube_bwd_kernel<true, false><<<grid, SKY_THREADS, 0, (cudaStream_t)stream>>>(c, jitter_u, jitter_v, nullptr, c.W * c.H, R, v_sky, v_tex);
-    SGN_CHECK_LAUNCH("cube_bwd_kernel<camera>");
-    return SGN_OK;
+    return sky_bwd("sgn_sky_bwd", cam, nullptr, jitter_u, jitter_v, R, v_sky, v_tex, stream);
+}
+
+extern "C" int sgn_sky_bwd_view(const sgn_camera* cam, const float* view, const float* jitter_u, const float* jitter_v, int R,
+                                const float* v_sky, float* v_tex, void* stream) {
+    SGN_RANGE("sgn_sky_bwd_view");
+    SGN_REQUIRE(view, "sgn_sky_bwd_view: null view");
+    return sky_bwd("sgn_sky_bwd_view", cam, view, jitter_u, jitter_v, R, v_sky, v_tex, stream);
 }
 
 // ---- deterministic backward: zero the scratch, the grid from max|v_out|, the kernel into the int64 sums, then v_tex += sums
@@ -478,9 +523,9 @@ static int check_det_scratch(const void* scratch, size_t scratch_bytes, int R, c
     return SGN_OK;
 }
 
-template <bool CAM>
+template <bool CAM, bool VIEW = false>
 static int launch_bwd_det(const SkyCam& c, const float* ju, const float* jv, const float* uv, int P, int R, const float* v_out,
-                          float* v_tex, void* scratch, dim3 grid, cudaStream_t stream) {
+                          float* v_tex, void* scratch, dim3 grid, cudaStream_t stream, const float* view = nullptr) {
     const long long n = 18LL * R * R;
     unsigned long long* fx = reinterpret_cast<unsigned long long*>(scratch);
     float* scale = reinterpret_cast<float*>(fx + n);
@@ -489,24 +534,39 @@ static int launch_bwd_det(const SkyCam& c, const float* ju, const float* jv, con
     SGN_CHECK_LAUNCH("cot_max_kernel");
     fixed_scale_kernel<<<1, 1, 0, stream>>>(scale);
     SGN_CHECK_LAUNCH("fixed_scale_kernel");
-    cube_bwd_kernel<CAM, true><<<grid, SKY_THREADS, 0, stream>>>(c, ju, jv, uv, P, R, v_out, fx);
+    cube_bwd_kernel<CAM, true, VIEW><<<grid, SKY_THREADS, 0, stream>>>(c, ju, jv, uv, P, R, v_out, fx, view);
     SGN_CHECK_LAUNCH(CAM ? "cube_bwd_kernel<camera, det>" : "cube_bwd_kernel<uv, det>");
     sky_fixed_add_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const long long*>(fx), scale, v_tex, n);
     SGN_CHECK_LAUNCH("sky_fixed_add_kernel");
     return SGN_OK;
 }
 
+static int sky_bwd_det(const char* who, const sgn_camera* cam, const float* view, const float* jitter_u, const float* jitter_v, int R,
+                       const float* v_sky, float* v_tex, void* scratch, size_t scratch_bytes, void* stream) {
+    SkyCam c;
+    if (int rc = sky_cam(c, cam, who)) return rc;
+    if (int rc = check_res(R, who)) return rc;
+    if (int rc = check_jitter(jitter_u, jitter_v, who)) return rc;
+    SGN_REQUIRE(v_sky && v_tex, "%s: null v_sky or v_tex", who);
+    if (int rc = check_det_scratch(scratch, scratch_bytes, R, who)) return rc;
+    const dim3 grid((c.W + SKY_TILE - 1) / SKY_TILE, (c.H + SKY_TILE - 1) / SKY_TILE);
+    if (view)
+        return launch_bwd_det<true, true>(c, jitter_u, jitter_v, nullptr, c.W * c.H, R, v_sky, v_tex, scratch, grid, (cudaStream_t)stream,
+                                          view);
+    return launch_bwd_det<true>(c, jitter_u, jitter_v, nullptr, c.W * c.H, R, v_sky, v_tex, scratch, grid, (cudaStream_t)stream);
+}
+
 extern "C" int sgn_sky_bwd_det(const sgn_camera* cam, const float* jitter_u, const float* jitter_v, int R, const float* v_sky, float* v_tex,
                                void* scratch, size_t scratch_bytes, void* stream) {
     SGN_RANGE("sgn_sky_bwd_det");
-    SkyCam c;
-    if (int rc = sky_cam(c, cam, "sgn_sky_bwd_det")) return rc;
-    if (int rc = check_res(R, "sgn_sky_bwd_det")) return rc;
-    if (int rc = check_jitter(jitter_u, jitter_v, "sgn_sky_bwd_det")) return rc;
-    SGN_REQUIRE(v_sky && v_tex, "sgn_sky_bwd_det: null v_sky or v_tex");
-    if (int rc = check_det_scratch(scratch, scratch_bytes, R, "sgn_sky_bwd_det")) return rc;
-    const dim3 grid((c.W + SKY_TILE - 1) / SKY_TILE, (c.H + SKY_TILE - 1) / SKY_TILE);
-    return launch_bwd_det<true>(c, jitter_u, jitter_v, nullptr, c.W * c.H, R, v_sky, v_tex, scratch, grid, (cudaStream_t)stream);
+    return sky_bwd_det("sgn_sky_bwd_det", cam, nullptr, jitter_u, jitter_v, R, v_sky, v_tex, scratch, scratch_bytes, stream);
+}
+
+extern "C" int sgn_sky_bwd_det_view(const sgn_camera* cam, const float* view, const float* jitter_u, const float* jitter_v, int R,
+                                    const float* v_sky, float* v_tex, void* scratch, size_t scratch_bytes, void* stream) {
+    SGN_RANGE("sgn_sky_bwd_det_view");
+    SGN_REQUIRE(view, "sgn_sky_bwd_det_view: null view");
+    return sky_bwd_det("sgn_sky_bwd_det_view", cam, view, jitter_u, jitter_v, R, v_sky, v_tex, scratch, scratch_bytes, stream);
 }
 
 static int check_items(int P, const char* who) {
@@ -522,7 +582,7 @@ extern "C" int sgn_cube_texture_fwd(int P, const float* uv, const float* tex, in
     if (P == 0) return SGN_OK;
     const SkyCam c{};
     cube_fwd_kernel<false><<<(P + SKY_THREADS - 1) / SKY_THREADS, SKY_THREADS, 0, (cudaStream_t)stream>>>(c, nullptr, nullptr, uv, P, tex, R,
-                                                                                                           out, nullptr);
+                                                                                                           out, nullptr, nullptr);
     SGN_CHECK_LAUNCH("cube_fwd_kernel<uv>");
     return SGN_OK;
 }
@@ -535,7 +595,7 @@ extern "C" int sgn_cube_texture_bwd(int P, const float* uv, int R, const float* 
     if (P == 0) return SGN_OK;
     const SkyCam c{};
     const int tile = SKY_TILE * SKY_TILE;
-    cube_bwd_kernel<false, false><<<(P + tile - 1) / tile, SKY_THREADS, 0, (cudaStream_t)stream>>>(c, nullptr, nullptr, uv, P, R, v_out, v_tex);
+    cube_bwd_kernel<false, false><<<(P + tile - 1) / tile, SKY_THREADS, 0, (cudaStream_t)stream>>>(c, nullptr, nullptr, uv, P, R, v_out, v_tex, nullptr);
     SGN_CHECK_LAUNCH("cube_bwd_kernel<uv>");
     return SGN_OK;
 }

@@ -305,9 +305,18 @@ _MODEL_SERIAL = itertools.count()
 class SceneGraphRasterModel(torch.nn.Module):
     def __init__(self, background: GaussianSet, actors: Dict[str, GaussianSet], config: Optional[SceneGraphConfig] = None,
                  poses_at: Optional[Callable[[float], List[ActorPose]]] = None,
-                 sky: Optional[Callable[[Camera, bool], torch.Tensor]] = None, bbox_optimizer: Optional[torch.nn.Module] = None):
+                 sky: Optional[Callable[[Camera, bool], torch.Tensor]] = None, bbox_optimizer: Optional[torch.nn.Module] = None,
+                 camera_optimizer: Optional[torch.nn.Module] = None):
         super().__init__()
         self.config = config or SceneGraphConfig()
+        # trainable camera poses (camera_pose.CameraPoseOptimizer, nerfstudio's attribute name).  None, or one in mode "off":
+        # every camera is rendered as given, by the same calls as without it
+        if camera_optimizer is not None and camera_optimizer.mode != "off" and sky is not None:
+            from .sky import CubeMapSky
+            if not isinstance(sky, CubeMapSky):
+                raise TypeError("a camera optimizer needs the sky to be a sky.CubeMapSky: the corrected view lives on the device, "
+                                f"and {type(sky).__name__} cannot take it")
+        self.camera_optimizer = camera_optimizer
         # trainable corrections of the actor boxes (box_pose.BoxPoseOptimizer; the reference's attribute name, scene graph
         # :91).  None, or one in mode "off": the boxes are rendered as annotated, by the same calls as without it
         self.bbox_optimizer = bbox_optimizer
@@ -486,13 +495,29 @@ class SceneGraphRasterModel(torch.nn.Module):
                 slot["box_stage"] = staged
         return bo(staged)
 
+    def _camera_view(self, camera: Camera) -> Optional[torch.Tensor]:
+        """The corrected device view of ``camera`` from ``camera_optimizer`` -- in training, for a camera with an index
+        (nerfstudio applies the correction to the training cameras, which carry ``cam_idx``); None otherwise.  The same
+        launch yields the regulariser and the metrics' norms: kept for this step's get_loss_dict / get_metrics_dict."""
+        self._camera_terms = None
+        co = self.camera_optimizer
+        if co is None or co.mode == "off" or not self.training or camera.index is None:
+            return None
+        view, reg, norms = co.terms(camera)
+        self._camera_terms = (reg, norms)
+        return view
+
     def get_outputs(self, camera: Camera) -> Dict[str, torch.Tensor]:
         """``SplatfactoSceneGraphModel.get_outputs`` (scene graph :305-374)."""
         assert camera.time is not None
         frame = self._frame(camera)
         H, W = camera.height, camera.width
         self.last_size = (H, W)
-        sky = self.env_map(camera, self.training) if (self.config.use_sky_sphere and self.env_map is not None) else None
+        view = self._camera_view(camera)
+        if self.config.use_sky_sphere and self.env_map is not None:
+            sky = self.env_map(camera, self.training) if view is None else self.env_map(camera, self.training, view=view)
+        else:
+            sky = None
         sink = anchor = None
         if torch.is_grad_enabled():
             flat = [t for seg in frame.segments for t in seg.params.tensors()]
@@ -506,7 +531,8 @@ class SceneGraphRasterModel(torch.nn.Module):
                     self._anchor = torch.zeros(1, device=flat[0].device, requires_grad=True)
                 anchor = self._anchor
         pose = self._box_poses(frame)
-        out, holder = raster.render_frame(frame, self._settings(class_streams=True), sky=sky, grad_sink=sink, anchor=anchor, pose=pose)
+        out, holder = raster.render_frame(frame, self._settings(class_streams=True), sky=sky, grad_sink=sink, anchor=anchor, pose=pose,
+                                          view=view)
         self._holder = holder
         self._publish_side_effects(frame, holder)
         if isinstance(holder.M, raster.LazyCount):
@@ -808,6 +834,10 @@ class SceneGraphRasterModel(torch.nn.Module):
                 oa = torch.clamp(outputs["object_acc"], min=1e-5, max=1 - 1e-5)
                 losses["object_acc_entropy_loss"] = c.object_acc_entropy_loss_mult * -(
                     oa * torch.log(oa) + (1.0 - oa) * torch.log(1.0 - oa)).mean()
+        co = self.camera_optimizer
+        if self.training and co is not None and co.mode != "off":
+            terms = getattr(self, "_camera_terms", None)
+            losses["camera_opt_regularizer"] = terms[0] if terms is not None else co.regularizer()
         return losses
 
     def _fused_metrics_ok(self, rgb: torch.Tensor) -> bool:
@@ -845,6 +875,10 @@ class SceneGraphRasterModel(torch.nn.Module):
         d["log_scale_mean"] = log_scale_mean
         d["sigmoid_opacity"] = sig
         d["self.radii"] = radii_mean  # sic: the reference's key
+        co = self.camera_optimizer
+        if co is not None and co.mode != "off":
+            terms = getattr(self, "_camera_terms", None)
+            d.update(co.metrics_of(terms[1]) if terms is not None else co.metrics())
         return d
 
     def get_image_metrics_and_images(self, outputs, batch):

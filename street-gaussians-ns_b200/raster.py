@@ -263,15 +263,32 @@ class Projected:
         return iter((self.records, self.radii, self.tiles_hit, self.bbox))
 
 
-def project_fwd(table: SegmentTable, cs: _lib.CameraStruct, device) -> Projected:
+def check_view(view: torch.Tensor, device) -> torch.Tensor:
+    """A device view (viewmat 12 row-major, cam_pos 3): float32 [15] on ``device``; returns it detached and contiguous."""
+    if not (view.is_cuda and view.device == device and view.dtype == torch.float32 and tuple(view.shape) == (VIEW_LEN,)):
+        raise _lib.SgnError(f"view must be a float32 [{VIEW_LEN}] tensor on {device} (viewmat 3x4 row-major, then cam_pos); "
+                            f"got {view.dtype} {tuple(view.shape)} on {view.device}")
+    return view.detach().contiguous()
+
+
+VIEW_LEN = _lib.VIEW_FLOATS + 3
+
+
+def project_fwd(table: SegmentTable, cs: _lib.CameraStruct, device, view: Optional[torch.Tensor] = None) -> Projected:
+    """``view``: a device view (check_view) in place of the camera's (sgn_project_fwd_view)."""
     L = _lib.load()
     N = table.N
     records = torch.empty(N, _lib.RECORD_FLOATS, device=device, dtype=torch.float32)
     ints = torch.empty(4, max(N, 1), device=device, dtype=torch.int32)  # radii, num_tiles_hit, tiles_touched, touch_mask
     bbox = torch.empty(N, 4, device=device, dtype=torch.int16)
     with _timed("project_fwd"):
-        _lib.check(L.sgn_project_fwd(_ptr(table.dev), table.nseg, N, table.num_chunks, C.byref(cs), _ptr(records), _ptr(ints[0]),
-                                     _ptr(ints[1]), _ptr(bbox), _ptr(ints[2]), _ptr(ints[3]), _stream()), "sgn_project_fwd")
+        if view is not None:
+            _lib.check(L.sgn_project_fwd_view(_ptr(table.dev), table.nseg, N, table.num_chunks, C.byref(cs), _ptr(view), _ptr(records),
+                                              _ptr(ints[0]), _ptr(ints[1]), _ptr(bbox), _ptr(ints[2]), _ptr(ints[3]), _stream()),
+                       "sgn_project_fwd_view")
+        else:
+            _lib.check(L.sgn_project_fwd(_ptr(table.dev), table.nseg, N, table.num_chunks, C.byref(cs), _ptr(records), _ptr(ints[0]),
+                                         _ptr(ints[1]), _ptr(bbox), _ptr(ints[2]), _ptr(ints[3]), _stream()), "sgn_project_fwd")
     return Projected(records, ints[0][:N], ints[1][:N], bbox, ints[2][:N], ints[3][:N])
 
 
@@ -600,12 +617,16 @@ def arena_views(arena: torch.Tensor, static: dict) -> List[torch.Tensor]:
 
 def project_bwd(table: SegmentTable, params: List[List[torch.Tensor]], cs, records, radii, v_records, make_views: bool = True,
                 out: Optional[torch.Tensor] = None, out_offsets: Optional[np.ndarray] = None, chunk_ranges=None, after_range=None,
-                v_pose: Optional[torch.Tensor] = None):
+                v_pose: Optional[torch.Tensor] = None, view: Optional[torch.Tensor] = None, v_view: Optional[torch.Tensor] = None):
     """Dense parameter gradients, one flat arena (a single allocation, 16-byte aligned slices; ``out`` reuses one).
     ``out_offsets`` (floats, one per parameter tensor of the frame, multiples of 4) places the slices inside a larger
     ``out`` -- the data-parallel arena that has the layout of ALL sub-models (model._FullArenaSink).
     ``v_pose`` [nseg, 16] float32: also filled with the cotangents of the segments' poses (R 9, t 3, q 4; zero rows for
-    segments without one) -- sgn_project_bwd_pose for every range, then sgn_pose_grad_reduce.  The arena is the same bits."""
+    segments without one) -- sgn_project_bwd_pose for every range, then sgn_pose_grad_reduce.  The arena is the same bits.
+    ``view``: the device view the forward projected with (check_view); ``v_view`` [12] float32 is then filled with its
+    cotangent -- sgn_project_bwd_view for every range (with the pose sums too when ``v_pose`` is given), then
+    sgn_view_grad_reduce.  The arena is the same bits as sgn_project_bwd_range's with that view."""
+    assert (view is None) == (v_view is None), "view and v_view go together"
     L = _lib.load()
     device = records.device
     st = table.static
@@ -627,6 +648,12 @@ def project_bwd(table: SegmentTable, params: List[List[torch.Tensor]], cs, recor
         partials = torch.empty(max(table.num_chunks, 1), _lib.POSE_FLOATS, device=device, dtype=torch.float32)
         if chunk_ranges is None:
             chunk_ranges = [(0, table.num_chunks)]
+    view_partials = None
+    if v_view is not None:
+        assert v_view.shape == (_lib.VIEW_FLOATS,) and v_view.dtype == torch.float32 and v_view.is_contiguous() and v_view.device == device
+        view_partials = torch.empty(max(table.num_chunks, 1), _lib.VIEW_FLOATS, device=device, dtype=torch.float32)
+        if chunk_ranges is None:
+            chunk_ranges = [(0, table.num_chunks)]
     with _timed("project_bwd"):
         if chunk_ranges is None:
             _lib.check(L.sgn_project_bwd(_ptr(table.dev), _ptr(gt), table.nseg, table.N, table.num_chunks, C.byref(cs), _ptr(records),
@@ -635,7 +662,11 @@ def project_bwd(table: SegmentTable, params: List[List[torch.Tensor]], cs, recor
             # range by range (data parallel): ``after_range(k)`` is called once range k's launch is enqueued -- the exchange of
             # that range's slices starts there and overlaps the production of the next range (dp.SymmetricExchange)
             for k, (c0, c1) in enumerate(chunk_ranges):
-                if partials is not None:
+                if view_partials is not None:
+                    _lib.check(L.sgn_project_bwd_view(_ptr(table.dev), _ptr(gt), table.nseg, table.N, table.num_chunks, C.byref(cs),
+                                                      _ptr(view), _ptr(records), _ptr(radii), _ptr(v_records), int(c0), int(c1),
+                                                      _ptr(partials), _ptr(view_partials), _stream()), "sgn_project_bwd_view")
+                elif partials is not None:
                     _lib.check(L.sgn_project_bwd_pose(_ptr(table.dev), _ptr(gt), table.nseg, table.N, table.num_chunks, C.byref(cs),
                                                       _ptr(records), _ptr(radii), _ptr(v_records), int(c0), int(c1), _ptr(partials),
                                                       _stream()), "sgn_project_bwd_pose")
@@ -648,6 +679,8 @@ def project_bwd(table: SegmentTable, params: List[List[torch.Tensor]], cs, recor
         if partials is not None:
             _lib.check(L.sgn_pose_grad_reduce(_ptr(table.dev), table.nseg, table.num_chunks, _ptr(partials), _ptr(v_pose), _stream()),
                        "sgn_pose_grad_reduce")
+        if view_partials is not None:
+            _lib.check(L.sgn_view_grad_reduce(table.num_chunks, _ptr(view_partials), _ptr(v_view), _stream()), "sgn_view_grad_reduce")
     return flat, arena
 
 
@@ -665,6 +698,7 @@ class _Holder:
         self.param_grads = None
         self.v_sky = None
         self.v_pose = None  # [nseg, 16] after a backward through a render whose ``pose`` required grad
+        self.v_view = None  # [12] after a backward through a render whose ``view`` required grad
         self.M = 0
         self.tile_bins = self.tile_depth = None
         self.table = None  # the frame's SegmentTable: its device rows are what sgn_metrics reads the parameters through
@@ -677,7 +711,7 @@ class _Holder:
 class _SceneGraphRasterize(torch.autograd.Function):
     @staticmethod
     def forward(ctx, frame: Frame, settings: RenderSettings, holder: _Holder, sky: Optional[torch.Tensor],
-                extra: Optional[torch.Tensor], pose: Optional[torch.Tensor], *flat):
+                extra: Optional[torch.Tensor], pose: Optional[torch.Tensor], view: Optional[torch.Tensor], *flat):
         # unused outputs must reach backward as None, not as zero tensors: the kernels specialise on
         # which cotangents exist (depth / background_acc have none in training)
         ctx.set_materialize_grads(False)
@@ -702,7 +736,11 @@ class _SceneGraphRasterize(torch.autograd.Function):
         if pose is not None:
             table = with_poses(table, pose)
         ctx.pose_needs_grad = pose is not None and pose.requires_grad
-        proj = project_fwd(table, cs, device)
+        ctx.view_needs_grad = view is not None and view.requires_grad
+        if view is not None:
+            view = check_view(view, device)
+        ctx.view = view
+        proj = project_fwd(table, cs, device, view)
         records, radii, tiles_hit, bbox = proj
         M, sorted_ids, tile_bins = bin_and_sort(cs, records, radii, proj=proj, async_binning=settings.async_binning)
         obj_ids = obj_bins = None
@@ -750,6 +788,11 @@ class _SceneGraphRasterize(torch.autograd.Function):
         v_pose = g_pose = None
         if ctx.pose_needs_grad:
             v_pose = torch.empty(ctx.table.nseg, _lib.POSE_FLOATS, device=v_records.device, dtype=torch.float32)
+        # a render with a device view differentiates with that view and yields its cotangent (cam_pos, detached like the SH
+        # view direction, gets 0)
+        view = ctx.view
+        g_view = torch.zeros(VIEW_LEN, device=v_records.device, dtype=torch.float32) if view is not None else None
+        v_view = g_view[:_lib.VIEW_FLOATS] if g_view is not None else None
         if sink is not None:
             target = sink.target(ctx.table.static, v_records.device)
             offsets = sink.grad_offsets(ctx.table.static) if target is not None else None  # None: the frame's own layout
@@ -758,12 +801,14 @@ class _SceneGraphRasterize(torch.autograd.Function):
             if plan is not None and target is not None:
                 chunk_ranges, after_range = plan(ctx.table)
             _, arena = project_bwd(ctx.table, ctx.params, ctx.cs, ctx.records, ctx.radii, v_records, make_views=False,
-                                   out=target, out_offsets=offsets, chunk_ranges=chunk_ranges, after_range=after_range, v_pose=v_pose)
+                                   out=target, out_offsets=offsets, chunk_ranges=chunk_ranges, after_range=after_range, v_pose=v_pose,
+                                   view=view, v_view=v_view)
             sink.publish(arena, ctx.table.static)
             flat = (None,)
         else:
-            flat, arena = project_bwd(ctx.table, ctx.params, ctx.cs, ctx.records, ctx.radii, v_records, v_pose=v_pose)
-        h.v_records, h.grad_arena, h.v_pose = v_records, arena, v_pose
+            flat, arena = project_bwd(ctx.table, ctx.params, ctx.cs, ctx.records, ctx.radii, v_records, v_pose=v_pose, view=view,
+                                      v_view=v_view)
+        h.v_records, h.grad_arena, h.v_pose, h.v_view = v_records, arena, v_pose, v_view
         if v_pose is not None:
             g_pose = v_pose[posed_rows(ctx.table)[0]]
         # the reference reads ``self.xys.grad`` after backward (densification statistics,
@@ -771,7 +816,7 @@ class _SceneGraphRasterize(torch.autograd.Function):
         h.xys.grad = v_records[:, 0:2]
         if h.post_backward is not None:
             h.post_backward(h)
-        return (None, None, None, v_sky, v_extra, g_pose, *flat)
+        return (None, None, None, v_sky, v_extra, g_pose, g_view if ctx.view_needs_grad else None, *flat)
 
 
 def forward_backward(frame: Frame, settings: RenderSettings, cotangents: Dict[str, Optional[torch.Tensor]],
@@ -857,8 +902,16 @@ def blend_extra_bwd(cs, bo, records, sorted_ids, tile_bins, final_T, final_idx, 
 
 def render_frame(frame: Frame, settings: Optional[RenderSettings] = None, sky: Optional[torch.Tensor] = None,
                  grad_sink=None, anchor: Optional[torch.Tensor] = None, extra: Optional[torch.Tensor] = None,
-                 pose: Optional[torch.Tensor] = None):
+                 pose: Optional[torch.Tensor] = None, view: Optional[torch.Tensor] = None):
     """Render one camera.  Returns (outputs dict, holder).  Segment parameters must be CUDA tensors.
+
+    ``view`` [15] (float32, on the device): the world->camera view to project with -- viewmat 3x4 row-major, then cam_pos
+    (the SH view directions' origin) -- in place of the one ``frame.camera`` gives; intrinsics and image size still come
+    from the camera.  It is read on the device (sgn_project_fwd_view), so a view computed there (camera_pose) costs no
+    read-back.  Differentiable: when it requires grad, backward returns its cotangent -- viewmat's 12 floats from the
+    projection backward (sgn_project_bwd_view + sgn_view_grad_reduce, no atomics: the same bits on every run over the same
+    image cotangents), zeros for cam_pos, whose SH direction is treated as constant -- and composes with ``pose``: both come
+    out of the same launches.  Without ``view`` the call sequence is unchanged.
 
     ``pose`` [n_posed, 16] (float32, on the device; one row per posed segment in the frame's order: R 9 row-major, t 3,
     q 4 -- the unit quaternion of R with w >= 0, as ``object2world_gs`` hands it on): the object->world poses to render
@@ -878,7 +931,7 @@ def render_frame(frame: Frame, settings: Optional[RenderSettings] = None, sky: O
     holder = _Holder()
     holder.grad_sink = grad_sink
     flat = [anchor] if grad_sink is not None else [t for seg in frame.segments for t in seg.params.tensors()]
-    outs = _SceneGraphRasterize.apply(frame, settings, holder, sky, extra, pose, *flat)
+    outs = _SceneGraphRasterize.apply(frame, settings, holder, sky, extra, pose, view, *flat)
     extra_img = None
     if extra is not None:
         outs, extra_img = outs[:-1], outs[-1]

@@ -224,6 +224,8 @@ class Camera:
     width: int
     height: int
     time: float = 0.0
+    # the camera's row of a camera pose optimiser (nerfstudio: camera.metadata["cam_idx"]); None: rendered as given
+    index: Optional[int] = None
 
     def __post_init__(self):
         self.c2w = np.asarray(self.c2w, dtype=np.float32).reshape(3, 4)

@@ -43,13 +43,19 @@ def _check_tex(tex: torch.Tensor) -> int:
 
 
 def sky_forward(cs: _lib.CameraStruct, tex: torch.Tensor, ju: Optional[torch.Tensor], jv: Optional[torch.Tensor],
-                want_dirs: bool = False):
-    """(sky [H, W, 3], dirs [H, W, 3] or None) through sgn_sky_fwd."""
+                want_dirs: bool = False, view: Optional[torch.Tensor] = None):
+    """(sky [H, W, 3], dirs [H, W, 3] or None) through sgn_sky_fwd -- or sgn_sky_fwd_view, with the camera's rotation taken
+    from ``view`` (a device view, raster.check_view)."""
     R = _check_tex(tex)
     tex = tex.contiguous()
     sky = torch.empty(cs.height, cs.width, 3, device=tex.device)
     dirs = torch.empty_like(sky) if want_dirs else None
-    _lib.check(_lib.load().sgn_sky_fwd(C.byref(cs), _ptr(ju), _ptr(jv), _ptr(tex), R, _ptr(sky), _ptr(dirs), _stream()), "sgn_sky_fwd")
+    L = _lib.load()
+    if view is not None:
+        _lib.check(L.sgn_sky_fwd_view(C.byref(cs), _ptr(view), _ptr(ju), _ptr(jv), _ptr(tex), R, _ptr(sky), _ptr(dirs), _stream()),
+                   "sgn_sky_fwd_view")
+    else:
+        _lib.check(L.sgn_sky_fwd(C.byref(cs), _ptr(ju), _ptr(jv), _ptr(tex), R, _ptr(sky), _ptr(dirs), _stream()), "sgn_sky_fwd")
     return sky, dirs
 
 
@@ -62,15 +68,24 @@ def _det_scratch(R: int, device) -> torch.Tensor:
     return torch.empty(_lib.load().sgn_sky_det_scratch_bytes(R), dtype=torch.uint8, device=device)
 
 
-def sky_backward(cs: _lib.CameraStruct, R: int, ju, jv, v_sky: torch.Tensor, device, deterministic: Optional[bool] = None) -> torch.Tensor:
-    """v_tex [6, R, R, 3] through sgn_sky_bwd, or sgn_sky_bwd_det when ``deterministic`` (None: raster.DETERMINISTIC)."""
+def sky_backward(cs: _lib.CameraStruct, R: int, ju, jv, v_sky: torch.Tensor, device, deterministic: Optional[bool] = None,
+                 view: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """v_tex [6, R, R, 3] through sgn_sky_bwd, or sgn_sky_bwd_det when ``deterministic`` (None: raster.DETERMINISTIC); the
+    ``_view`` entry points when ``view`` is given (as in sky_forward)."""
     L = _lib.load()
     v_tex = torch.zeros(6, R, R, 3, device=device)
     v_sky = v_sky.contiguous()
     if _deterministic(deterministic):
         scratch = _det_scratch(R, device)
-        _lib.check(L.sgn_sky_bwd_det(C.byref(cs), _ptr(ju), _ptr(jv), R, _ptr(v_sky), _ptr(v_tex), _ptr(scratch), scratch.numel(),
-                                     _stream()), "sgn_sky_bwd_det")
+        if view is not None:
+            _lib.check(L.sgn_sky_bwd_det_view(C.byref(cs), _ptr(view), _ptr(ju), _ptr(jv), R, _ptr(v_sky), _ptr(v_tex), _ptr(scratch),
+                                              scratch.numel(), _stream()), "sgn_sky_bwd_det_view")
+        else:
+            _lib.check(L.sgn_sky_bwd_det(C.byref(cs), _ptr(ju), _ptr(jv), R, _ptr(v_sky), _ptr(v_tex), _ptr(scratch), scratch.numel(),
+                                         _stream()), "sgn_sky_bwd_det")
+    elif view is not None:
+        _lib.check(L.sgn_sky_bwd_view(C.byref(cs), _ptr(view), _ptr(ju), _ptr(jv), R, _ptr(v_sky), _ptr(v_tex), _stream()),
+                   "sgn_sky_bwd_view")
     else:
         _lib.check(L.sgn_sky_bwd(C.byref(cs), _ptr(ju), _ptr(jv), R, _ptr(v_sky), _ptr(v_tex), _stream()), "sgn_sky_bwd")
     return v_tex
@@ -78,9 +93,11 @@ def sky_backward(cs: _lib.CameraStruct, R: int, ju, jv, v_sky: torch.Tensor, dev
 
 class _CubeMapSky(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, base: torch.Tensor, cs: _lib.CameraStruct, ju, jv, deterministic: Optional[bool]):
-        sky, _ = sky_forward(cs, base.detach(), ju, jv)
-        ctx.cs, ctx.R, ctx.device, ctx.deterministic = cs, int(base.shape[1]), base.device, deterministic
+    def forward(ctx, base: torch.Tensor, cs: _lib.CameraStruct, ju, jv, deterministic: Optional[bool], view: Optional[torch.Tensor]):
+        if view is not None:
+            view = raster.check_view(view, base.device)
+        sky, _ = sky_forward(cs, base.detach(), ju, jv, view=view)
+        ctx.cs, ctx.R, ctx.device, ctx.deterministic, ctx.view = cs, int(base.shape[1]), base.device, deterministic, view
         ctx.save_for_backward(*(t for t in (ju, jv) if t is not None))
         return sky
 
@@ -88,8 +105,8 @@ class _CubeMapSky(torch.autograd.Function):
     def backward(ctx, v_sky):
         saved = ctx.saved_tensors
         ju, jv = (saved[0], saved[1]) if saved else (None, None)
-        v_tex = sky_backward(ctx.cs, ctx.R, ju, jv, v_sky, ctx.device, ctx.deterministic) if ctx.needs_input_grad[0] else None
-        return v_tex, None, None, None, None
+        v_tex = sky_backward(ctx.cs, ctx.R, ju, jv, v_sky, ctx.device, ctx.deterministic, ctx.view) if ctx.needs_input_grad[0] else None
+        return v_tex, None, None, None, None, None  # no gradient for the view: the sky is a function of the view direction only
 
 
 class CubeMapSky(torch.nn.Module):
@@ -108,9 +125,12 @@ class CubeMapSky(torch.nn.Module):
         jv = torch.rand(camera.height, camera.width, device=self.base.device)
         return ju, jv
 
-    def forward(self, camera: Camera, train: bool = False) -> torch.Tensor:
+    def forward(self, camera: Camera, train: bool = False, view: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``view``: a device view (raster.render_frame's ``view``) whose rotation orients the sky in place of the camera's, so
+        that a corrected camera sees geometry and sky alike; the sky gives the view no gradient."""
         ju, jv = self.jitter(camera) if train else (None, None)
-        return _CubeMapSky.apply(self.base, camera_struct(camera, RenderSettings()), ju, jv, self.deterministic)
+        return _CubeMapSky.apply(self.base, camera_struct(camera, RenderSettings()), ju, jv, self.deterministic,
+                                 None if view is None else view.detach())
 
 
 def cube_texture(tex: torch.Tensor, uv: torch.Tensor, deterministic: Optional[bool] = None) -> torch.Tensor:

@@ -30,12 +30,22 @@ from .scene import Camera
 class TrainStep:
     def __init__(self, model: SceneGraphRasterModel, optimizer: FusedAdam, refine_every: Optional[int] = None,
                  group: Optional[dist.ProcessGroup] = None, pipeline_chunks: int = 0, refine_seed: int = 0,
-                 check_replicas: bool = True, overlap: bool = False, exchange: str = "auto", metrics: bool = False):
+                 check_replicas: bool = True, overlap: bool = False, exchange: str = "auto", metrics: bool = False,
+                 gradient_accumulation_steps: Optional[Dict[str, int]] = None):
         """``pipeline_chunks`` > 0 (data parallel only): all-reduce and Adam are pipelined over that many ranges of the
         arena (dp.allreduce_and_step) instead of running one after the other.  ``metrics``: every step calls
         ``model.get_metrics_dict`` between ``get_outputs`` and ``get_loss_dict`` (nerfstudio's order,
-        ``VanillaPipeline.get_train_loss_dict``) and keeps its result on ``self.metrics`` (device tensors, no read-back)."""
+        ``VanillaPipeline.get_train_loss_dict``) and keeps its result on ``self.metrics`` (device tensors, no read-back).
+        ``gradient_accumulation_steps``: name of one of the optimizer's extra tensors -> n, nerfstudio's trainer rule (the
+        reference sets ``{"camera_opt": 100}``, sgn_config.py:30): the tensor's gradient is zeroed at the steps where
+        ``step % n == 0``, summed over the steps in between, and the tensor is stepped where ``step % n == n - 1``.  None (or a
+        tensor not named): every step."""
         self.model, self.optimizer, self.group = model, optimizer, group
+        self.accumulate = dict(gradient_accumulation_steps or {})
+        unknown = sorted(set(self.accumulate) - set(optimizer.extra_tensors()))
+        if unknown or any(int(n) < 1 for n in self.accumulate.values()):
+            raise ValueError(f"gradient_accumulation_steps names tensors the optimizer does not step ({unknown}) or a count < 1: "
+                             f"{self.accumulate}")
         self.want_metrics, self.metrics = metrics, None
         self.pipeline_chunks = pipeline_chunks if pipeline_chunks > 0 or not overlap else 4
         self.refine_seed, self.check_replicas, self._gen = refine_seed, check_replicas, None
@@ -79,10 +89,14 @@ class TrainStep:
         if world > 1:
             self._ensure_exchange()
         m.step = step                                     # step_cb (sgn_splatfacto.py:754-755)
+        # accumulated tensors keep their gradient except where their cycle starts; they step where it ends
+        keep = {id(extras[k]) for k, n in self.accumulate.items() if step % n != 0}
         for p in m.parameters():                          # Optimizers.zero_grad_all()
-            p.grad = None
+            if id(p) not in keep:
+                p.grad = None
         for t in extras.values():
-            t.grad = None
+            if id(t) not in keep:
+                t.grad = None
         out = m.get_outputs(camera)
         if world > 1 and self._exchange is not None:  # which background rows this replica sees (rows nobody sees are not exchanged)
             h = m._holder
@@ -100,17 +114,25 @@ class TrainStep:
         rendered = isinstance(total, torch.Tensor) and total.requires_grad
         if rendered:
             total.backward()
+            # with nothing in view a loss term of another tensor (the camera regulariser) can still carry a gradient
+            rendered = m._holder is not None and m._holder.grad_arena is not None
+        if rendered:
             arena = m._holder.grad_arena
         else:
             # nothing in view on this replica (the reference's early-out, sgn_splatfacto.py:878-886): no gradient here.
             # A single replica skips backward / optimizer / after_train only: the refinement callbacks still run
             # (nerfstudio fires them on the step count, whatever was rendered)
             if world == 1:
+                # a loss term of a further tensor (the camera regulariser) may still have left a gradient: that tensor steps
+                # on its own step count, as nerfstudio steps a group whatever was rendered
+                due = self._due_extra_grads(step, extras)
+                if due:
+                    opt.step(next(iter(due.values())), present=[], full_layout=True, extra_grads=due)
                 self._maybe_refine(step)
                 return losses
             arena = m.zero_gradient_arena()
         # the further tensors of the optimizer (the sky cube map, sky.CubeMapSky.base) step with the gradient autograd left
-        extra_grads = {name: t.grad for name, t in extras.items() if t.grad is not None}
+        extra_grads = self._due_extra_grads(step, extras)
         if world > 1:
             present = sorted(set(i for cam in all_cameras for i in self.submodels_in_view(cam)))
         else:
@@ -128,6 +150,12 @@ class TrainStep:
             m.after_train(step)                           # AFTER_TRAIN_ITERATION callbacks, in the reference's order
         self._maybe_refine(step)
         return losses
+
+    def _due_extra_grads(self, step: int, extras: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        """The gradients of the extra tensors that step at ``step``: every one that has a gradient, an accumulated one only at
+        the end of its cycle (``step % n == n - 1``)."""
+        return {name: t.grad for name, t in extras.items()
+                if t.grad is not None and (name not in self.accumulate or step % self.accumulate[name] == self.accumulate[name] - 1)}
 
     def _ensure_exchange(self) -> None:
         """(Re)allocates the symmetric gradient arena when the model's layout changed (first step, after a refinement).

@@ -26,13 +26,15 @@ sys.path.insert(0, ROOT)
 def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int = 100, start_step: int = 600,
         actor_range: float = 45.0, pipeline_chunks: int = 0, overlap: bool = False, resident_table: bool = True,
         async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True, sky: bool = False, metrics: bool = False,
-        bbox_opt: bool = False) -> dict:
+        bbox_opt: bool = False, camera_opt: bool = False) -> dict:
     """One measurement.  torch.distributed must already be initialised when WORLD_SIZE > 1.  Returns the result dict on
     rank 0 (None elsewhere).  ``sky``: the reference's default learnable sky (use_sky_sphere, a 1024^2 cube map stepped by
     the same Adam launch at the ``sky_sphere`` group's lr 0.005, sgn_config.py:72-75).  ``metrics``: every step also computes
     ``get_metrics_dict`` (psnr, gaussian_count, scale / opacity / radii means), as nerfstudio's training pipeline does.
     ``bbox_opt``: the reference's default box corrections (``bbox_optimizer`` mode "simple": delta_center / delta_yaw per
-    (frame, box), stepped by the same Adam launch at the ``bbox_opt`` group's lr 1e-3, sgn_config.py:80-83)."""
+    (frame, box), stepped by the same Adam launch at the ``bbox_opt`` group's lr 1e-3, sgn_config.py:80-83).
+    ``camera_opt``: trainable camera poses (``camera_optimizer`` mode "SO3xR3" over the indexed rig cameras, the ``camera_opt``
+    group's lr 1e-3 and its 100-step gradient accumulation, sgn_config.py:30,76-79)."""
     import torch
     import torch.distributed as dist
 
@@ -68,15 +70,26 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     if bbox_opt:
         from street_gaussians_ns_b200.box_pose import BoxPoseOptimizer
         boxes = BoxPoseOptimizer(num_frames, [str(k) for k in sc.actors], {f: f for f in range(num_frames)}, mode="simple")
+    cam_opt = None
+    if camera_opt:
+        from street_gaussians_ns_b200.camera_pose import CameraPoseOptimizer
+        cam_opt = CameraPoseOptimizer(len(cams))
+        for i, c in enumerate(cams):
+            c.index = i
     model = SceneGraphRasterModel(sc.background.to(dev), {k: v.to(dev) for k, v in sc.actors.items()}, cfg, poses_at=poses_at,
-                                  sky=env_map, bbox_optimizer=boxes).to(dev)
+                                  sky=env_map, bbox_optimizer=boxes, camera_optimizer=cam_opt).to(dev)
     model.train()
     extra = {"sky": (model.env_map.base, 0.005)} if sky else {}
     if bbox_opt:
         extra["bbox_opt.delta_center"] = (boxes.delta_center, 1e-3)
         extra["bbox_opt.delta_yaw"] = (boxes.delta_yaw, 1e-3)
+    accumulate = None
+    if camera_opt:
+        extra["camera_opt.pose_adjustment"] = (cam_opt.pose_adjustment, 1e-3)
+        accumulate = {"camera_opt.pose_adjustment": 100}
     opt = FusedAdam(model.optimizer_params(), extra=extra, reserve_spare=True)  # no cudaMalloc of moment arenas inside the training loop
-    step_fn = TrainStep(model, opt, refine_every=refine_every, pipeline_chunks=pipeline_chunks, overlap=overlap, metrics=metrics)
+    step_fn = TrainStep(model, opt, refine_every=refine_every, pipeline_chunks=pipeline_chunks, overlap=overlap, metrics=metrics,
+                        gradient_accumulation_steps=accumulate)
     g = torch.Generator().manual_seed(5)
     gt = (torch.rand(H, W, 3, generator=g) * 255).to(torch.uint8).to(dev)  # get_loss_dict consumes uint8 directly
     counts0 = [sub.num_points for sub in model.all_models.values()]
@@ -184,6 +197,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                    "parallelism": f"camera-sharded dp{world}", "ssim_lambda": ssim_lambda,
                    **({"sky": "CubeMapSky(1024), Adam lr 0.005"} if sky else {}),
                    **({"bbox_opt": "BoxPoseOptimizer(simple), Adam lr 1e-3"} if bbox_opt else {}),
+                   **({"camera_opt": "CameraPoseOptimizer(SO3xR3), Adam lr 1e-3, gradient accumulation 100"} if camera_opt else {}),
                    "loss": "fused kernels" if fused_loss else "torch ops", "metrics": "get_metrics_dict every step" if metrics else "none",
                    "start_step": start_step, "refine_every": refine_every,
                    "refinement_kernels_loaded_before_timing": refine_warm,
@@ -215,6 +229,7 @@ def main():
     ap.add_argument("--sky", action="store_true", help="train the learnable sky cube map (the reference's use_sky_sphere = True)")
     ap.add_argument("--metrics", action="store_true", help="get_metrics_dict every step, between get_outputs and get_loss_dict")
     ap.add_argument("--bbox-opt", action="store_true", help="train the box corrections (the reference's bbox_optimizer mode 'simple')")
+    ap.add_argument("--camera-opt", action="store_true", help="train the camera poses (camera_optimizer mode 'SO3xR3', accumulation 100)")
     args = ap.parse_args()
 
     import torch
@@ -227,7 +242,7 @@ def main():
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     res = run(args.steps, args.warmup, args.scale, args.refine_every, args.start_step, args.actor_range, args.pipeline_chunks,
               args.overlap, not args.host_table, ssim_lambda=args.ssim_lambda, fused_loss=not args.torch_loss, sky=args.sky,
-              metrics=args.metrics, bbox_opt=args.bbox_opt)
+              metrics=args.metrics, bbox_opt=args.bbox_opt, camera_opt=args.camera_opt)
     if res is not None:
         print(json.dumps(res))
     if world > 1:
