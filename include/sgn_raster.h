@@ -416,7 +416,7 @@ int sgn_metrics(int H, int W, const sgn_loss_in* image, const sgn_segment* table
 
 /* ---- sky cube map (EnvLight, sgn_splatfacto.py:109-150; use_sky_sphere = True) ------------------------------
  * nvdiffrast dr.texture(tex[None], l, filter_mode='linear', boundary_mode='cube') on a learnable [6,R,R,3] map, and its
- * gradient for the map (no gradient for the directions).  The camera path generates the reference's per-pixel world
+ * gradient for the map (the gradient for the directions: the _uv / _rot entry points below).  The camera path generates the reference's per-pixel world
  * directions itself: d = normalize(((x - cx + ju) / fx, (y - cy + jv) / fy, 1)), rotated by c2w[:3,:3] (recovered from
  * cam->viewmat), then l = (d.x, d.z, -d.y); ju = jv = 0.5 in eval (jitter pointers NULL), two [H,W] uniform draws in
  * training.  The backward recomputes the directions from the same jitter.  v_tex is ACCUMULATED into (zero it first); it
@@ -441,13 +441,41 @@ int sgn_sky_bwd_det(const sgn_camera* cam, const float* jitter_u, const float* j
 int sgn_cube_texture_bwd_det(int P, const float* uv, int R, const float* v_out, float* v_tex, void* scratch, size_t scratch_bytes,
                              void* stream);
 /* The three camera-path sky entry points with c2w[:3,:3] recovered from a DEVICE view (viewmat[12], cam_pos[3]; see
- * sgn_project_fwd_view) instead of cam->viewmat, by the same exact transpose and negation.  No cotangent for the view. */
+ * sgn_project_fwd_view) instead of cam->viewmat, by the same exact transpose and negation.  No cotangent for the view (the
+ * _rot forms below give one). */
 int sgn_sky_fwd_view(const sgn_camera* cam, const float* view, const float* jitter_u, const float* jitter_v, const float* tex, int R,
                      float* sky, float* dirs, void* stream);
 int sgn_sky_bwd_view(const sgn_camera* cam, const float* view, const float* jitter_u, const float* jitter_v, int R, const float* v_sky,
                      float* v_tex, void* stream);
 int sgn_sky_bwd_det_view(const sgn_camera* cam, const float* view, const float* jitter_u, const float* jitter_v, int R,
                          const float* v_sky, float* v_tex, void* scratch, size_t scratch_bytes, void* stream);
+/* Gradient for the lookup direction (nvdiffrast's TextureGradKernelCubeLinear with indexCubeMapGrad, texture.cu:123-148 and
+ * :1005-1046, filter_mode='linear', boundary_mode='cube'): per lookup g_s = sum_ch v ((a10 - a00) + fv (a11 + a00 - a10 -
+ * a01)) R, g_t likewise with fu and a01, the four taps as the forward reads them (wrapped taps; at a cube corner the
+ * missing tap is the mean of the other three), mapped to the 3-vector through s = <l,U> / (2|<l,N>|) + 1/2 on the RAW
+ * direction (the [0,1] clamp of s, t is straight-through, as in nvdiffrast).  A zero cotangent, an invalid direction or a
+ * non-finite result gives 0.  Each lookup reads tex; nothing is reordered, so the direction gradient is bit-reproducible.
+ * The texture gradient beside it is that of the entry points above, bit for bit in the _det forms (the same kernel body);
+ * v_tex may be NULL to skip it (then scratch is not read).
+ * sgn_cube_texture_bwd_uv[_det]: nvdiffrast's gradTex + gradUV on given directions; v_uv[P,3] is WRITTEN.
+ * sgn_sky_bwd_view_rot / sgn_sky_bwd_det_view_rot: the _view backward that also reduces the direction gradient to the
+ * view's rotation (EnvLight.forward, sgn_splatfacto.py:140-147: l = to_opengl(c2w[:3,:3] u), u the normalised jittered
+ * camera-space direction, independent of the rotation): v_d = (v_l.x, -v_l.z, v_l.y), v_R[i][j] = sum_pixels v_d[i] u[j],
+ * v_view[4j+i] = s_j v_R[i][j] with s = (1, -1, -1) (the inverse of the view -> c2w mapping), v_view[3], [7], [11] = 0.
+ * Per 32 x 32 tile the nine sums go to rot_partials (device, 4-byte aligned, sgn_sky_rot_scratch_bytes(W, H) bytes); one
+ * more launch adds them in a fixed order and WRITES v_view[SGN_VIEW_FLOATS] (device).  No atomics: v_view is the same bits
+ * on every run, in both forms. */
+int sgn_cube_texture_bwd_uv(int P, const float* uv, const float* tex, int R, const float* v_out, float* v_tex /* or NULL */, float* v_uv,
+                            void* stream);
+int sgn_cube_texture_bwd_uv_det(int P, const float* uv, const float* tex, int R, const float* v_out, float* v_tex /* or NULL */,
+                                float* v_uv, void* scratch, size_t scratch_bytes, void* stream);
+size_t sgn_sky_rot_scratch_bytes(int width, int height); /* 0 for an empty image */
+int sgn_sky_bwd_view_rot(const sgn_camera* cam, const float* view, const float* jitter_u, const float* jitter_v, const float* tex, int R,
+                         const float* v_sky, float* v_tex /* or NULL */, float* rot_partials, size_t partials_bytes, float* v_view,
+                         void* stream);
+int sgn_sky_bwd_det_view_rot(const sgn_camera* cam, const float* view, const float* jitter_u, const float* jitter_v, const float* tex,
+                             int R, const float* v_sky, float* v_tex /* or NULL */, void* scratch, size_t scratch_bytes,
+                             float* rot_partials, size_t partials_bytes, float* v_view, void* stream);
 
 /* ---- densification statistics (SURVEY.md 8f rank 3) -------------------------------------------------------
  * What each sub-model's `after_train` accumulates after backward (sgn_splatfacto.py:513-541), for all visible

@@ -136,7 +136,8 @@ EXPORTS = [
     "sgn_project_bwd_range", "sgn_allreduce_sym", "sgn_blend_extra_fwd", "sgn_blend_extra_bwd", "sgn_blend_extra_bwd_det",
     "sgn_bin_sort_capped", "sgn_visible_flags", "sgn_visible_union", "sgn_project_bwd_pose", "sgn_pose_grad_reduce",
     "sgn_project_fwd_view", "sgn_project_bwd_view", "sgn_view_grad_reduce", "sgn_sky_fwd_view", "sgn_sky_bwd_view",
-    "sgn_sky_bwd_det_view", "sgn_camera_adjust_fwd", "sgn_camera_adjust_bwd",
+    "sgn_sky_bwd_det_view", "sgn_camera_adjust_fwd", "sgn_camera_adjust_bwd", "sgn_cube_texture_bwd_uv", "sgn_cube_texture_bwd_uv_det",
+    "sgn_sky_rot_scratch_bytes", "sgn_sky_bwd_view_rot", "sgn_sky_bwd_det_view_rot",
 ]
 VIEW_FLOATS = 12  # SGN_VIEW_FLOATS: the view's cotangent, viewmat[12] row-major; the device view itself is 12 + 3 (cam_pos) floats
 POSE_FLOATS = 16  # SGN_POSE_FLOATS: a segment's pose (and its cotangent) as R[9] row-major, t[3], q[4]
@@ -247,8 +248,15 @@ def load():
     L.sgn_sky_fwd_view.argtypes = [C.POINTER(CameraStruct), vp, vp, vp, vp, i32, vp, vp, vp]
     L.sgn_sky_bwd_view.argtypes = [C.POINTER(CameraStruct), vp, vp, vp, i32, vp, vp, vp]
     L.sgn_sky_bwd_det_view.argtypes = [C.POINTER(CameraStruct), vp, vp, vp, i32, vp, vp, vp, sz, vp]
+    L.sgn_cube_texture_bwd_uv.argtypes = [i32, vp, vp, i32, vp, vp, vp, vp]
+    L.sgn_cube_texture_bwd_uv_det.argtypes = [i32, vp, vp, i32, vp, vp, vp, vp, sz, vp]
+    L.sgn_sky_rot_scratch_bytes.argtypes = [i32, i32]
+    L.sgn_sky_rot_scratch_bytes.restype = sz
+    L.sgn_sky_bwd_view_rot.argtypes = [C.POINTER(CameraStruct), vp, vp, vp, vp, i32, vp, vp, vp, sz, vp, vp]
+    L.sgn_sky_bwd_det_view_rot.argtypes = [C.POINTER(CameraStruct), vp, vp, vp, vp, i32, vp, vp, vp, sz, vp, sz, vp, vp]
     for f in ("sgn_sky_fwd", "sgn_sky_bwd", "sgn_cube_texture_fwd", "sgn_cube_texture_bwd", "sgn_sky_bwd_det", "sgn_cube_texture_bwd_det",
-              "sgn_sky_fwd_view", "sgn_sky_bwd_view", "sgn_sky_bwd_det_view"):
+              "sgn_sky_fwd_view", "sgn_sky_bwd_view", "sgn_sky_bwd_det_view", "sgn_cube_texture_bwd_uv", "sgn_cube_texture_bwd_uv_det",
+              "sgn_sky_bwd_view_rot", "sgn_sky_bwd_det_view_rot"):
         getattr(L, f).restype = C.c_int
     L.sgn_sizeof_adam_tensor.restype = sz
     L.sgn_adam_chunk_elems.restype = C.c_int

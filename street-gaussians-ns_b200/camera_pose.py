@@ -27,9 +27,14 @@ that raster.render_frame(view=...) and sky.CubeMapSky take, the regulariser and 
 (sgn_camera_adjust_bwd: the view's and the regulariser's cotangents -> every row of the gradient).  Everything stays on the
 device: no read-back per step.
 
-Not provided: the ``SE3`` mode (NotImplementedError), ``non_trainable_camera_indices``, intrinsics, the sky's share of the
-rotation gradient (the sky is sampled with the corrected rotation but, like the SH colour, gives the camera no gradient),
-and a data-parallel exchange of the camera gradient (a data-parallel TrainStep refuses it).
+The sky is sampled with the corrected rotation.  By default it gives the camera no gradient; with
+``CubeMapSky(view_grad=True)`` it adds its share of the rotation cotangent (the reference's ``EnvLight`` looks up
+``c2w[:3,:3] @ d`` with a ``c2w`` that is not detached), which autograd sums with the projection's before
+sgn_camera_adjust_bwd runs.
+
+Not provided: the ``SE3`` mode (NotImplementedError), ``non_trainable_camera_indices``, intrinsics, the SH colour's view
+direction gradient (the reference detaches the camera there), and a data-parallel exchange of the camera gradient (a
+data-parallel TrainStep refuses it).
 """
 from __future__ import annotations
 

@@ -36,6 +36,11 @@
 // indexable size has fewer than 2^30 pixels (1920 x 1280: 2^21.2) and a uv array fewer than 2^29.5 lookups (3 P <= INT_MAX).
 // So, unlike the blend's conic components, no texel needs a coarser grid.  Halving the box capacity keeps the int64 box at
 // the float box's 24 KB of static shared memory.
+//
+// Direction gradient (cube_bwd_kernel<..., DIRG = true>, nvdiffrast's gradUV): the same launch also reads each lookup's four
+// taps (they stay in L2) and forms d<lookup, v>/dl (cube_dir_grad).  The uv form writes it per lookup; the camera form
+// chains it to the view's rotation and stores nine sums per tile, which sky_rot_reduce_kernel adds in a fixed order.  The
+// texture-gradient code is unchanged, so the _det texture gradient is bit-identical to the texture-only entry points'.
 #include <limits.h>
 
 #include <type_traits>
@@ -158,25 +163,72 @@ static __device__ __forceinline__ void cube_quad(float3 l, int R, Quad& q) {
 
 static __device__ __forceinline__ float lerpf(float a, float b, float c) { return fmaf(c, b - a, a); }
 
+// channel ch of the four taps as the lookup reads them: at a cube corner the missing tap is kThird times the sum of the
+// other three (an invalid lookup, all taps missing, reads four zeros)
+static __device__ __forceinline__ void quad_fetch(const Quad& q, const float* __restrict__ tex, int ch, float a[4]) {
+    if (quad_corner(q)) {
+        float avg = 0.f;
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+            if (q.idx[k] >= 0) avg += (a[k] = __ldg(tex + 3 * q.idx[k] + ch));
+        avg *= kThird;
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+            if (q.idx[k] < 0) a[k] = avg;
+    } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) a[k] = __ldg(tex + 3 * q.idx[k] + ch);
+    }
+}
+
 static __device__ __forceinline__ void cube_sample(const Quad& q, const float* __restrict__ tex, float* o) {
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) {
         float a[4];
-        if (quad_corner(q)) {
-            float avg = 0.f;
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-                if (q.idx[k] >= 0) avg += (a[k] = __ldg(tex + 3 * q.idx[k] + ch));
-            avg *= kThird;
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-                if (q.idx[k] < 0) a[k] = avg;
-        } else {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) a[k] = __ldg(tex + 3 * q.idx[k] + ch);
-        }
+        quad_fetch(q, tex, ch, a);
         o[ch] = lerpf(lerpf(a[0], a[1], q.fu), lerpf(a[2], a[3], q.fu), q.fv);
     }
+}
+
+// Gradient of <lookup(l), vy> for the direction l (nvdiffrast's TextureGradKernelCubeLinear, texture.cu:1005-1046, with
+// indexCubeMapGrad, :123-148).  In face coordinates: g_s = sum_ch vy ((a10 - a00) + fv (a11 + a00 - a10 - a01)) R and
+// g_t likewise with fu and a01, the taps as the forward reads them.  Through s = <l,U> / (2|c|) + 1/2 (c = <l,N> sigma,
+// sigma the sign of the major component, m = 1 / |c| rounded toward zero): dL/dl = (m/2) (g_s U + g_t V
+// - sigma m (g_s <l,U> + g_t <l,V>) N), evaluated on the raw direction -- the [0,1] clamp of s and t passes the gradient
+// straight through, as nvdiffrast's does.  Each product, sum and sign flip is rounded as that kernel rounds it; an invalid
+// lookup or a non-finite result gives 0.
+static __device__ __forceinline__ float3 cube_dir_grad(const Quad& q, float3 l, int R, const float* __restrict__ tex, const float vy[3]) {
+    if (q.idx[0] < 0 && q.idx[1] < 0 && q.idx[2] < 0 && q.idx[3] < 0) return make_float3(0.f, 0.f, 0.f);
+    float gu = 0.f, gv = 0.f;
+    const float sc = (float)R;
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+        float a[4];
+        quad_fetch(q, tex, ch, a);
+        const float ad = a[3] + a[0] - a[1] - a[2];
+        gu += vy[ch] * ((a[1] - a[0]) + q.fv * ad) * sc;
+        gv += vy[ch] * ((a[2] - a[0]) + q.fu * ad) * sc;
+    }
+    const float mx = fabsf(l.x), my = fabsf(l.y), mz = fabsf(l.z);
+    const int axis = mz > fmaxf(mx, my) ? 2 : my > mx ? 1 : 0;
+    const float major = axis == 2 ? l.z : axis == 1 ? l.y : l.x;
+    const int face = 2 * axis + (major < 0.f);
+    const float m = __frcp_rz(fabsf(major));
+    const int iu = axis == 0 ? 2 : 0, iv = axis == 1 ? 2 : 1;
+    const int su = kCubeBasis[face][1][iu], sv = kCubeBasis[face][2][iv];  // U = su e_iu, V = sv e_iv
+    const bool neg = major < 0.f;
+    // c0 = -sigma g_s <l,U>, c1 = -sigma g_t <l,V>: a product with the raw component, then an exact sign
+    float c0 = __fmul_rn(gu, iu == 2 ? l.z : l.x), c1 = __fmul_rn(gv, iv == 2 ? l.z : l.y);
+    if ((su > 0) != neg) c0 = -c0;
+    if ((sv > 0) != neg) c1 = -c1;
+    const float gl = __fmul_rn(__fadd_rn(c0, c1), m);
+    const float h = m * 0.5f;
+    const float gU = su > 0 ? gu : -gu, gV = sv > 0 ? gv : -gv;
+    // the major axis takes gl; U lies along x (y or z major) or z (x major), V along y (x or z major) or z (y major)
+    const float gx = axis == 0 ? gl : gU, gy = axis == 1 ? gl : gV, gz = axis == 2 ? gl : axis == 0 ? gU : gV;
+    const float3 r = make_float3(__fmul_rn(gx, h), __fmul_rn(gy, h), __fmul_rn(gz, h));
+    if (!isfinite(r.x) || !isfinite(r.y) || !isfinite(r.z)) return make_float3(0.f, 0.f, 0.f);
+    return r;
 }
 
 // bilinear weights of taps (i,j), (i+1,j), (i,j+1), (i+1,j+1): the corner product fu fv once, the two edge weights as a
@@ -244,15 +296,24 @@ static __device__ __forceinline__ void quad_red_global(const Quad& q, const floa
     }
 }
 
-static __device__ __forceinline__ float3 sky_direction(const SkyCam& c, int x, int y, float ju, float jv) {
+// the normalised camera-space direction u of pixel (x, y)
+static __device__ __forceinline__ float3 sky_ray(const SkyCam& c, int x, int y, float ju, float jv) {
     const float dx = __fdiv_rn(__fadd_rn(__fsub_rn((float)x, c.cx), ju), c.fx);
     const float dy = __fdiv_rn(__fadd_rn(__fsub_rn((float)y, c.cy), jv), c.fy);
     const float n = fmaxf(__fsqrt_rn(__fadd_rn(__fmaf_rn(dy, dy, __fmul_rn(dx, dx)), 1.f)), 1e-12f);
-    const float ux = __fdiv_rn(dx, n), uy = __fdiv_rn(dy, n), uz = __fdiv_rn(1.f, n);
-    const float w0 = __fmaf_rn(c.R[2], uz, __fmaf_rn(c.R[1], uy, __fmul_rn(c.R[0], ux)));
-    const float w1 = __fmaf_rn(c.R[5], uz, __fmaf_rn(c.R[4], uy, __fmul_rn(c.R[3], ux)));
-    const float w2 = __fmaf_rn(c.R[8], uz, __fmaf_rn(c.R[7], uy, __fmul_rn(c.R[6], ux)));
+    return make_float3(__fdiv_rn(dx, n), __fdiv_rn(dy, n), __fdiv_rn(1.f, n));
+}
+
+// l = to_opengl(c2w[:3,:3] u)
+static __device__ __forceinline__ float3 sky_rotate(const SkyCam& c, float3 u) {
+    const float w0 = __fmaf_rn(c.R[2], u.z, __fmaf_rn(c.R[1], u.y, __fmul_rn(c.R[0], u.x)));
+    const float w1 = __fmaf_rn(c.R[5], u.z, __fmaf_rn(c.R[4], u.y, __fmul_rn(c.R[3], u.x)));
+    const float w2 = __fmaf_rn(c.R[8], u.z, __fmaf_rn(c.R[7], u.y, __fmul_rn(c.R[6], u.x)));
     return make_float3(w0, w2, -w1);  // to_opengl
+}
+
+static __device__ __forceinline__ float3 sky_direction(const SkyCam& c, int x, int y, float ju, float jv) {
+    return sky_rotate(c, sky_ray(c, x, y, ju, jv));
 }
 
 // the lookup direction of item p (pixel p = y * W + x of the camera, or row p of the uv array)
@@ -304,10 +365,16 @@ __global__ void __launch_bounds__(SKY_THREADS) cube_fwd_kernel(const SkyCam c_ar
 
 // DET = false: float atomics into v_tex.  DET = true: v_tex is the fixed-point scratch, int64 [6,R,R,3] followed by the
 // grid scale (one float), and the box holds int64 (SKY_DET_BOX_TEXELS).  The float instantiations carry no fixed-point code.
-template <bool CAM, bool DET, bool VIEW = false>
+// DIRG: also the direction gradient (cube_dir_grad), which reads the taps from `tex`.  The uv form writes it to
+// v_dir[P, 3] (0 for a zero cotangent or an invalid lookup); the camera form chains it to the rotation -- d = c2w[:3,:3] u,
+// l = (d.x, d.z, -d.y), so v_d = (v_l.x, -v_l.z, v_l.y) and v_R[i][j] = sum v_d[i] u[j] -- and stores the tile's nine sums
+// to v_dir[block, 9] (each thread's items in order, then a fixed tree over the block: no atomics).  With DIRG a NULL v_tex
+// skips the texture gradient.  Without DIRG the kernel is the one the texture-only entry points have always launched.
+template <bool CAM, bool DET, bool VIEW = false, bool DIRG = false>
 __global__ void __launch_bounds__(SKY_THREADS) cube_bwd_kernel(const SkyCam c_arg, const float* __restrict__ ju, const float* __restrict__ jv,
                                                                const float* __restrict__ uv, int P, int R, const float* __restrict__ v_out,
-                                                               SkyAcc<DET>* __restrict__ v_tex, const float* __restrict__ view) {
+                                                               SkyAcc<DET>* __restrict__ v_tex, const float* __restrict__ view,
+                                                               const float* __restrict__ tex = nullptr, float* __restrict__ v_dir = nullptr) {
     SkyCam c_view;
     if constexpr (VIEW) c_view = sky_cam_with_view(c_arg, view);
     const SkyCam& c = VIEW ? c_view : c_arg;
@@ -366,17 +433,43 @@ __global__ void __launch_bounds__(SKY_THREADS) cube_bwd_kernel(const SkyCam c_ar
     const int bi0 = s_lo[0], bj0 = s_lo[1];
     const bool some = dom >= 0 && s_hi[0] >= bi0;  // block-uniform: some lookup lies on the privatised face
     const int bw = some ? s_hi[0] - bi0 + 2 : 0, bh = some ? s_hi[1] - bj0 + 2 : 0;  // a quad spans two texels per axis
-    const bool priv = some && bw * bh <= BOX_TEXELS;
+    const bool want_tex = !DIRG || v_tex != nullptr;
+    const bool priv = want_tex && some && bw * bh <= BOX_TEXELS;
     if (priv) {
         for (int e = tid; e < bw * bh * 3; e += SKY_THREADS) box[e] = 0;
         __syncthreads();
     }
+    float rot[DIRG && CAM ? 9 : 1] = {};  // this thread's share of v_R (camera form)
 #pragma unroll
     for (int k = 0; k < SKY_ITEMS; ++k) {
         const int p = item[k];
         if (p < 0) continue;
         const float vy[3] = {v_out[3 * p], v_out[3 * p + 1], v_out[3 * p + 2]};
-        if (vy[0] == 0.f && vy[1] == 0.f && vy[2] == 0.f) continue;
+        if (vy[0] == 0.f && vy[1] == 0.f && vy[2] == 0.f) {
+            if constexpr (DIRG && !CAM) v_dir[3 * p] = v_dir[3 * p + 1] = v_dir[3 * p + 2] = 0.f;
+            continue;
+        }
+        if constexpr (DIRG) {
+            if constexpr (CAM) {
+                const int x = blockIdx.x * SKY_TILE + (tid & (SKY_TILE - 1));
+                const int y = blockIdx.y * SKY_TILE + (tid / SKY_TILE) + k * (SKY_THREADS / SKY_TILE);
+                const float3 u = sky_ray(c, x, y, ju ? ju[p] : 0.5f, jv ? jv[p] : 0.5f);
+                const float3 gl = cube_dir_grad(q[k], sky_rotate(c, u), R, tex, vy);
+                const float vd[3] = {gl.x, -gl.z, gl.y};
+#pragma unroll
+                for (int i = 0; i < 3; ++i) {
+                    rot[3 * i] = fmaf(vd[i], u.x, rot[3 * i]);
+                    rot[3 * i + 1] = fmaf(vd[i], u.y, rot[3 * i + 1]);
+                    rot[3 * i + 2] = fmaf(vd[i], u.z, rot[3 * i + 2]);
+                }
+            } else {
+                const float3 gl = cube_dir_grad(q[k], make_float3(uv[3 * p], uv[3 * p + 1], uv[3 * p + 2]), R, tex, vy);
+                v_dir[3 * p] = gl.x;
+                v_dir[3 * p + 1] = gl.y;
+                v_dir[3 * p + 2] = gl.z;
+            }
+        }
+        if (!want_tex) continue;
         if (priv && q[k].own_face == dom) {
             if constexpr (DET) {
                 float w[4];
@@ -416,6 +509,39 @@ __global__ void __launch_bounds__(SKY_THREADS) cube_bwd_kernel(const SkyCam c_ar
                 atomicAdd(v_tex + 3 * ((dom * R + bj0 + jj) * R + bi0 + ii) + ch, g);
             }
         }
+    }
+    if constexpr (DIRG && CAM) {
+        __shared__ float s_rot[SKY_THREADS / 32][9];
+#pragma unroll
+        for (int e = 0; e < 9; ++e) {
+            float r = rot[e];
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) r += __shfl_xor_sync(0xffffffffu, r, o);
+            if ((tid & 31) == 0) s_rot[tid >> 5][e] = r;
+        }
+        __syncthreads();
+        if (tid < 9) {
+            float r = s_rot[0][tid];
+#pragma unroll
+            for (int w = 1; w < SKY_THREADS / 32; ++w) r += s_rot[w][tid];
+            v_dir[9 * (blockIdx.y * gridDim.x + blockIdx.x) + tid] = r;
+        }
+    }
+}
+
+// v_view[SGN_VIEW_FLOATS] from the tiles' v_R sums (cube_bwd_kernel<camera, *, view, DIRG>): warp e sums entry e of every
+// tile in a fixed order (lane-strided, then a fixed shuffle tree), and v_view[4 j + i] = s_j v_R[i][j] with s = (1, -1, -1),
+// the transpose of sky_cam_with_view; the translation entries viewmat[:, 3] are 0.  Written, not accumulated.
+__global__ void __launch_bounds__(288) sky_rot_reduce_kernel(const float* __restrict__ partials, int n, float* __restrict__ v_view) {
+    const int e = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    float r = 0.f;
+    for (int b = lane; b < n; b += 32) r += partials[9 * b + e];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) r += __shfl_xor_sync(0xffffffffu, r, o);
+    if (lane == 0) {
+        const int i = e / 3, j = e - 3 * i;
+        v_view[4 * j + i] = j == 0 ? r : -r;
+        if (e < 3) v_view[4 * e + 3] = 0.f;
     }
 }
 
@@ -472,7 +598,7 @@ static int sky_bwd(const char* who, const sgn_camera* cam, const float* view, co
     SGN_REQUIRE(v_sky && v_tex, "%s: null v_sky or v_tex", who);
     const dim3 grid((c.W + SKY_TILE - 1) / SKY_TILE, (c.H + SKY_TILE - 1) / SKY_TILE);
     auto kernel = view ? cube_bwd_kernel<true, false, true> : cube_bwd_kernel<true, false, false>;
-    kernel<<<grid, SKY_THREADS, 0, (cudaStream_t)stream>>>(c, jitter_u, jitter_v, nullptr, c.W * c.H, R, v_sky, v_tex, view);
+    kernel<<<grid, SKY_THREADS, 0, (cudaStream_t)stream>>>(c, jitter_u, jitter_v, nullptr, c.W * c.H, R, v_sky, v_tex, view, nullptr, nullptr);
     SGN_CHECK_LAUNCH("cube_bwd_kernel<camera>");
     return SGN_OK;
 }
@@ -523,9 +649,10 @@ static int check_det_scratch(const void* scratch, size_t scratch_bytes, int R, c
     return SGN_OK;
 }
 
-template <bool CAM, bool VIEW = false>
+template <bool CAM, bool VIEW = false, bool DIRG = false>
 static int launch_bwd_det(const SkyCam& c, const float* ju, const float* jv, const float* uv, int P, int R, const float* v_out,
-                          float* v_tex, void* scratch, dim3 grid, cudaStream_t stream, const float* view = nullptr) {
+                          float* v_tex, void* scratch, dim3 grid, cudaStream_t stream, const float* view = nullptr,
+                          const float* tex = nullptr, float* v_dir = nullptr) {
     const long long n = 18LL * R * R;
     unsigned long long* fx = reinterpret_cast<unsigned long long*>(scratch);
     float* scale = reinterpret_cast<float*>(fx + n);
@@ -534,7 +661,7 @@ static int launch_bwd_det(const SkyCam& c, const float* ju, const float* jv, con
     SGN_CHECK_LAUNCH("cot_max_kernel");
     fixed_scale_kernel<<<1, 1, 0, stream>>>(scale);
     SGN_CHECK_LAUNCH("fixed_scale_kernel");
-    cube_bwd_kernel<CAM, true, VIEW><<<grid, SKY_THREADS, 0, stream>>>(c, ju, jv, uv, P, R, v_out, fx, view);
+    cube_bwd_kernel<CAM, true, VIEW, DIRG><<<grid, SKY_THREADS, 0, stream>>>(c, ju, jv, uv, P, R, v_out, fx, view, tex, v_dir);
     SGN_CHECK_LAUNCH(CAM ? "cube_bwd_kernel<camera, det>" : "cube_bwd_kernel<uv, det>");
     sky_fixed_add_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const long long*>(fx), scale, v_tex, n);
     SGN_CHECK_LAUNCH("sky_fixed_add_kernel");
@@ -567,6 +694,59 @@ extern "C" int sgn_sky_bwd_det_view(const sgn_camera* cam, const float* view, co
     SGN_RANGE("sgn_sky_bwd_det_view");
     SGN_REQUIRE(view, "sgn_sky_bwd_det_view: null view");
     return sky_bwd_det("sgn_sky_bwd_det_view", cam, view, jitter_u, jitter_v, R, v_sky, v_tex, scratch, scratch_bytes, stream);
+}
+
+// ---- direction gradient, camera form: the texture gradient of the _view entry points plus the view's rotation cotangent
+extern "C" size_t sgn_sky_rot_scratch_bytes(int width, int height) {
+    if (width < 1 || height < 1) return 0;
+    const size_t tiles = (size_t)((width + SKY_TILE - 1) / SKY_TILE) * ((height + SKY_TILE - 1) / SKY_TILE);
+    return tiles * 9 * sizeof(float);
+}
+
+static int sky_bwd_view_rot(const char* who, bool det, const sgn_camera* cam, const float* view, const float* jitter_u,
+                            const float* jitter_v, const float* tex, int R, const float* v_sky, float* v_tex, void* scratch,
+                            size_t scratch_bytes, float* rot_partials, size_t partials_bytes, float* v_view, void* stream) {
+    SkyCam c;
+    if (int rc = sky_cam(c, cam, who)) return rc;
+    if (int rc = check_res(R, who)) return rc;
+    if (int rc = check_jitter(jitter_u, jitter_v, who)) return rc;
+    SGN_REQUIRE(view && tex && v_sky && v_view, "%s: null view, texture, v_sky or v_view", who);
+    SGN_REQUIRE(rot_partials && (reinterpret_cast<uintptr_t>(rot_partials) & 3) == 0, "%s: null or misaligned rotation partials", who);
+    const size_t need = sgn_sky_rot_scratch_bytes(c.W, c.H);
+    SGN_REQUIRE(partials_bytes >= need, "%s: rotation partials of %zu bytes, sgn_sky_rot_scratch_bytes(%d, %d) = %zu", who,
+                partials_bytes, c.W, c.H, need);
+    if (det && v_tex)
+        if (int rc = check_det_scratch(scratch, scratch_bytes, R, who)) return rc;
+    const dim3 grid((c.W + SKY_TILE - 1) / SKY_TILE, (c.H + SKY_TILE - 1) / SKY_TILE);
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (det && v_tex) {
+        if (int rc = launch_bwd_det<true, true, true>(c, jitter_u, jitter_v, nullptr, c.W * c.H, R, v_sky, v_tex, scratch, grid, st, view,
+                                                      tex, rot_partials))
+            return rc;
+    } else {
+        cube_bwd_kernel<true, false, true, true><<<grid, SKY_THREADS, 0, st>>>(c, jitter_u, jitter_v, nullptr, c.W * c.H, R, v_sky, v_tex,
+                                                                               view, tex, rot_partials);
+        SGN_CHECK_LAUNCH("cube_bwd_kernel<camera, rot>");
+    }
+    sky_rot_reduce_kernel<<<1, 288, 0, st>>>(rot_partials, (int)(grid.x * grid.y), v_view);
+    SGN_CHECK_LAUNCH("sky_rot_reduce_kernel");
+    return SGN_OK;
+}
+
+extern "C" int sgn_sky_bwd_view_rot(const sgn_camera* cam, const float* view, const float* jitter_u, const float* jitter_v,
+                                    const float* tex, int R, const float* v_sky, float* v_tex, float* rot_partials,
+                                    size_t partials_bytes, float* v_view, void* stream) {
+    SGN_RANGE("sgn_sky_bwd_view_rot");
+    return sky_bwd_view_rot("sgn_sky_bwd_view_rot", false, cam, view, jitter_u, jitter_v, tex, R, v_sky, v_tex, nullptr, 0,
+                            rot_partials, partials_bytes, v_view, stream);
+}
+
+extern "C" int sgn_sky_bwd_det_view_rot(const sgn_camera* cam, const float* view, const float* jitter_u, const float* jitter_v,
+                                        const float* tex, int R, const float* v_sky, float* v_tex, void* scratch, size_t scratch_bytes,
+                                        float* rot_partials, size_t partials_bytes, float* v_view, void* stream) {
+    SGN_RANGE("sgn_sky_bwd_det_view_rot");
+    return sky_bwd_view_rot("sgn_sky_bwd_det_view_rot", true, cam, view, jitter_u, jitter_v, tex, R, v_sky, v_tex, scratch,
+                            scratch_bytes, rot_partials, partials_bytes, v_view, stream);
 }
 
 static int check_items(int P, const char* who) {
@@ -611,4 +791,37 @@ extern "C" int sgn_cube_texture_bwd_det(int P, const float* uv, int R, const flo
     const SkyCam c{};
     const int tile = SKY_TILE * SKY_TILE;
     return launch_bwd_det<false>(c, nullptr, nullptr, uv, P, R, v_out, v_tex, scratch, dim3((P + tile - 1) / tile), (cudaStream_t)stream);
+}
+
+// ---- direction gradient, uv form: nvdiffrast's gradUV (v_uv [P, 3], written) beside its gradTex (v_tex, optional)
+static int cube_texture_bwd_uv(const char* who, bool det, int P, const float* uv, const float* tex, int R, const float* v_out,
+                               float* v_tex, float* v_uv, void* scratch, size_t scratch_bytes, void* stream) {
+    if (int rc = check_items(P, who)) return rc;
+    if (int rc = check_res(R, who)) return rc;
+    SGN_REQUIRE(uv && tex && v_out && v_uv, "%s: null uv, texture, v_out or v_uv", who);
+    if (det && v_tex)
+        if (int rc = check_det_scratch(scratch, scratch_bytes, R, who)) return rc;
+    if (P == 0) return SGN_OK;
+    const SkyCam c{};
+    const int tile = SKY_TILE * SKY_TILE;
+    const dim3 grid((P + tile - 1) / tile);
+    if (det && v_tex)
+        return launch_bwd_det<false, false, true>(c, nullptr, nullptr, uv, P, R, v_out, v_tex, scratch, grid, (cudaStream_t)stream, nullptr,
+                                                  tex, v_uv);
+    cube_bwd_kernel<false, false, false, true><<<grid, SKY_THREADS, 0, (cudaStream_t)stream>>>(c, nullptr, nullptr, uv, P, R, v_out, v_tex,
+                                                                                             nullptr, tex, v_uv);
+    SGN_CHECK_LAUNCH("cube_bwd_kernel<uv, dir>");
+    return SGN_OK;
+}
+
+extern "C" int sgn_cube_texture_bwd_uv(int P, const float* uv, const float* tex, int R, const float* v_out, float* v_tex, float* v_uv,
+                                       void* stream) {
+    SGN_RANGE("sgn_cube_texture_bwd_uv");
+    return cube_texture_bwd_uv("sgn_cube_texture_bwd_uv", false, P, uv, tex, R, v_out, v_tex, v_uv, nullptr, 0, stream);
+}
+
+extern "C" int sgn_cube_texture_bwd_uv_det(int P, const float* uv, const float* tex, int R, const float* v_out, float* v_tex, float* v_uv,
+                                           void* scratch, size_t scratch_bytes, void* stream) {
+    SGN_RANGE("sgn_cube_texture_bwd_uv_det");
+    return cube_texture_bwd_uv("sgn_cube_texture_bwd_uv_det", true, P, uv, tex, R, v_out, v_tex, v_uv, scratch, scratch_bytes, stream);
 }

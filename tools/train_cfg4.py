@@ -26,7 +26,7 @@ sys.path.insert(0, ROOT)
 def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int = 100, start_step: int = 600,
         actor_range: float = 45.0, pipeline_chunks: int = 0, overlap: bool = False, resident_table: bool = True,
         async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True, sky: bool = False, metrics: bool = False,
-        bbox_opt: bool = False, camera_opt: bool = False) -> dict:
+        bbox_opt: bool = False, camera_opt: bool = False, sky_view_grad: bool = False) -> dict:
     """One measurement.  torch.distributed must already be initialised when WORLD_SIZE > 1.  Returns the result dict on
     rank 0 (None elsewhere).  ``sky``: the reference's default learnable sky (use_sky_sphere, a 1024^2 cube map stepped by
     the same Adam launch at the ``sky_sphere`` group's lr 0.005, sgn_config.py:72-75).  ``metrics``: every step also computes
@@ -34,10 +34,13 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     ``bbox_opt``: the reference's default box corrections (``bbox_optimizer`` mode "simple": delta_center / delta_yaw per
     (frame, box), stepped by the same Adam launch at the ``bbox_opt`` group's lr 1e-3, sgn_config.py:80-83).
     ``camera_opt``: trainable camera poses (``camera_optimizer`` mode "SO3xR3" over the indexed rig cameras, the ``camera_opt``
-    group's lr 1e-3 and its 100-step gradient accumulation, sgn_config.py:30,76-79)."""
+    group's lr 1e-3 and its 100-step gradient accumulation, sgn_config.py:30,76-79).  ``sky_view_grad`` (with ``sky`` and
+    ``camera_opt``): the sky also gives the camera rotation its gradient (CubeMapSky(view_grad=True))."""
     import torch
     import torch.distributed as dist
 
+    if sky_view_grad and not (sky and camera_opt):
+        raise ValueError("sky_view_grad needs sky and camera_opt")
     import street_gaussians_ns_b200.synthetic as syn
     from street_gaussians_ns_b200 import dp
     from street_gaussians_ns_b200.model import ActorPose, SceneGraphConfig, SceneGraphRasterModel
@@ -65,7 +68,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     env_map = None
     if sky:
         from street_gaussians_ns_b200.sky import CubeMapSky
-        env_map = CubeMapSky(1024)
+        env_map = CubeMapSky(1024, view_grad=sky_view_grad)
     boxes = None
     if bbox_opt:
         from street_gaussians_ns_b200.box_pose import BoxPoseOptimizer
@@ -198,6 +201,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                    **({"sky": "CubeMapSky(1024), Adam lr 0.005"} if sky else {}),
                    **({"bbox_opt": "BoxPoseOptimizer(simple), Adam lr 1e-3"} if bbox_opt else {}),
                    **({"camera_opt": "CameraPoseOptimizer(SO3xR3), Adam lr 1e-3, gradient accumulation 100"} if camera_opt else {}),
+                   **({"sky_view_grad": "the sky's rotation cotangent reaches the camera"} if sky_view_grad else {}),
                    "loss": "fused kernels" if fused_loss else "torch ops", "metrics": "get_metrics_dict every step" if metrics else "none",
                    "start_step": start_step, "refine_every": refine_every,
                    "refinement_kernels_loaded_before_timing": refine_warm,
@@ -230,7 +234,10 @@ def main():
     ap.add_argument("--metrics", action="store_true", help="get_metrics_dict every step, between get_outputs and get_loss_dict")
     ap.add_argument("--bbox-opt", action="store_true", help="train the box corrections (the reference's bbox_optimizer mode 'simple')")
     ap.add_argument("--camera-opt", action="store_true", help="train the camera poses (camera_optimizer mode 'SO3xR3', accumulation 100)")
+    ap.add_argument("--sky-view-grad", action="store_true", help="with --sky --camera-opt: the sky also trains the camera rotation")
     args = ap.parse_args()
+    if args.sky_view_grad and not (args.sky and args.camera_opt):
+        ap.error("--sky-view-grad needs --sky and --camera-opt")
 
     import torch
     import torch.distributed as dist
@@ -242,7 +249,8 @@ def main():
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     res = run(args.steps, args.warmup, args.scale, args.refine_every, args.start_step, args.actor_range, args.pipeline_chunks,
               args.overlap, not args.host_table, ssim_lambda=args.ssim_lambda, fused_loss=not args.torch_loss, sky=args.sky,
-              metrics=args.metrics, bbox_opt=args.bbox_opt, camera_opt=args.camera_opt)
+              metrics=args.metrics, bbox_opt=args.bbox_opt, camera_opt=args.camera_opt,
+              sky_view_grad=args.sky_view_grad)
     if res is not None:
         print(json.dumps(res))
     if world > 1:
