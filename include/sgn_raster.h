@@ -585,6 +585,20 @@ int sgn_refine_decide(int n, const sgn_refine_config* cfg, const float* scales /
 int sgn_refine_apply(int n, const sgn_refine_config* cfg, const sgn_refine_tensors* tensors, const uint8_t* flags,
                      const int32_t* scan, const int32_t* totals, const float* samples, void* stream);
 
+/* ---- exact k-nearest-neighbour search (model initialisation, lidar chamfer distance) -------------------------
+ * The initial scales of SplatfactoModel.populate_modules (sgn_splatfacto.py:260-264: log of the mean distance to the 3 nearest
+ * other seed points, from sklearn's NearestNeighbors on the CPU, :439-457) and the nearest distances of calc_chamfer_distance
+ * (data/utils/geometric_metric.py:59-69).  points [n,3] fp32; query [m,3] fp32 or NULL.  For every query row: its k nearest
+ * points (1 <= k <= 16), ascending by fp32 distance, a tie going to the smaller row.  With query == NULL the queries are the
+ * points themselves (m is ignored, n >= k + 1) and row i is never its own neighbour, while an exact duplicate of it is one at
+ * distance 0; with a query set n >= k.  Exact: no cap on how far a search looks.  Deterministic: the same bytes every run.
+ * Outputs, any of which may be NULL (not all three): dist [m,k] fp32 Euclidean distances, idx [m,k] int32 rows of `points`,
+ * log_scales [m,3] = logf(mean of the k distances) broadcast (the scales tensor of populate_modules; -inf when they are all 0).
+ * Inputs must be finite.  n, m < 2^31 - 1. */
+size_t sgn_knn_scratch_bytes(int64_t n, int64_t m /* 0 without a query set */);
+int sgn_knn(const float* points, int64_t n, const float* query, int64_t m, int k, float* dist, int32_t* idx, float* log_scales,
+            void* scratch, size_t scratch_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

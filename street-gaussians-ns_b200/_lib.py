@@ -137,7 +137,7 @@ EXPORTS = [
     "sgn_bin_sort_capped", "sgn_visible_flags", "sgn_visible_union", "sgn_project_bwd_pose", "sgn_pose_grad_reduce",
     "sgn_project_fwd_view", "sgn_project_bwd_view", "sgn_view_grad_reduce", "sgn_sky_fwd_view", "sgn_sky_bwd_view",
     "sgn_sky_bwd_det_view", "sgn_camera_adjust_fwd", "sgn_camera_adjust_bwd", "sgn_cube_texture_bwd_uv", "sgn_cube_texture_bwd_uv_det",
-    "sgn_sky_rot_scratch_bytes", "sgn_sky_bwd_view_rot", "sgn_sky_bwd_det_view_rot",
+    "sgn_sky_rot_scratch_bytes", "sgn_sky_bwd_view_rot", "sgn_sky_bwd_det_view_rot", "sgn_knn_scratch_bytes", "sgn_knn",
 ]
 VIEW_FLOATS = 12  # SGN_VIEW_FLOATS: the view's cotangent, viewmat[12] row-major; the device view itself is 12 + 3 (cam_pos) floats
 POSE_FLOATS = 16  # SGN_POSE_FLOATS: a segment's pose (and its cotangent) as R[9] row-major, t[3], q[4]
@@ -258,6 +258,10 @@ def load():
               "sgn_sky_fwd_view", "sgn_sky_bwd_view", "sgn_sky_bwd_det_view", "sgn_cube_texture_bwd_uv", "sgn_cube_texture_bwd_uv_det",
               "sgn_sky_bwd_view_rot", "sgn_sky_bwd_det_view_rot"):
         getattr(L, f).restype = C.c_int
+    L.sgn_knn_scratch_bytes.argtypes = [i64, i64]
+    L.sgn_knn_scratch_bytes.restype = sz
+    L.sgn_knn.argtypes = [vp, i64, vp, i64, i32, vp, vp, vp, vp, sz, vp]
+    L.sgn_knn.restype = C.c_int
     L.sgn_sizeof_adam_tensor.restype = sz
     L.sgn_adam_chunk_elems.restype = C.c_int
     L.sgn_adam_step.argtypes = [vp, i32, i32, vp, vp, vp, vp]

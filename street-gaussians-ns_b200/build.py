@@ -31,6 +31,7 @@ SOURCES = {
     "refine.cu": ["--fmad=false"],
     "collective.cu": [],  # the refinement rules mirror torch's separately rounded elementwise kernels
     "camera.cu": [],  # IEEE sinf / cosf / sqrtf (no fast math)
+    "knn.cu": [],  # distances through explicit _rn intrinsics: the box bound must not exceed a point's distance
 }
 
 

@@ -341,6 +341,39 @@ class SceneGraphRasterModel(torch.nn.Module):
         # weights are not part of this library; an integration that has them sets a callable (gt, rgb) -> score here
         self.lpips = None
 
+    @classmethod
+    def from_points(cls, background=None, actors: Optional[Dict[str, tuple]] = None, config: Optional[SceneGraphConfig] = None,
+                    generator: Optional[torch.Generator] = None, replay_scene_graph_init: bool = True, device=None,
+                    **model_kwargs) -> "SceneGraphRasterModel":
+        """A model initialised from seed points, as ``SplatfactoSceneGraphModel.populate_modules`` builds its sub-models
+        (sgn_splatfacto_scene_graph.py:49-96, each one by ``SplatfactoModel.populate_modules``, see populate.py).
+
+        ``background``: ``(xyz, rgb)`` -- COLMAP / lidar ``points3D``, rgb uint8 or float 0..255 -- with ``fourier_dim`` 1, or
+        None for the reference's random initialisation of 50 000 points in a cube of side 10.  ``actors``: ``{track_id:
+        (xyz, rgb)}``, one aggregated lidar cloud per tracked actor, with ``config.fourier_features_dim``, in the given order.
+        Every sub-model uses ``config.sh_degree``.  The initial scales come from the GPU nearest-neighbour search (knn.py).
+
+        Draws come from ``generator`` (default: torch's default CPU generator) in the reference's order.  With
+        ``replay_scene_graph_init`` (the default) the draws of the scene graph's own random initialisation, which the reference
+        makes and discards before the background (:50-52), are consumed first, so that after ``torch.manual_seed(s)`` the
+        sub-models equal those of the reference's populate_modules seeded with ``s``.  Draws the reference makes outside
+        populate_modules' initialisation (e.g. by modules its trainer builds in between) are not replayed.  ``device``: where
+        the parameters live (default: the current CUDA device).  ``model_kwargs`` go to the constructor (poses_at, sky, ...).
+        """
+        from . import populate
+        config = config or SceneGraphConfig()
+        if replay_scene_graph_init:
+            populate.replay_scene_graph_init(generator)
+        if background is None:
+            bg = populate.random_gaussians(50000, 10.0, config.sh_degree, 1, generator=generator, device=device)
+        else:
+            bg = populate.gaussians_from_points(*background, sh_degree=config.sh_degree, fourier_dim=1, generator=generator,
+                                                device=device)
+        acts = {tid: populate.gaussians_from_points(xyz, rgb, sh_degree=config.sh_degree, fourier_dim=config.fourier_features_dim,
+                                                    generator=generator, device=device)
+                for tid, (xyz, rgb) in (actors or {}).items()}
+        return cls(bg, acts, config=config, **model_kwargs)
+
     @staticmethod
     def get_object_model_name(object_id) -> str:
         return f"object_{object_id}"

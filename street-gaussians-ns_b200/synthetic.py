@@ -77,6 +77,34 @@ def actor_pose(index: int, seed: int = 1000) -> Tuple[np.ndarray, np.ndarray]:
     return rot, center
 
 
+def street_points(n: int, seed: int = 0, box=((-40.0, 40.0), (-6.0, 14.0), (-90.0, -1.5)), n_outliers: int = 8) -> torch.Tensor:
+    """A street-like seed cloud [n, 3] float32 over config 3's box: 70 % a thin ground slab, 30 % sparse volume, and
+    ``n_outliers`` points 1-5 km away (lidar returns off buildings and the sky) -- the non-uniform density initialisation sees."""
+    g = torch.Generator().manual_seed(seed)
+    lo = torch.tensor([b[0] for b in box])
+    hi = torch.tensor([b[1] for b in box])
+    n_ground = int(0.7 * n)
+    n_vol = n - n_ground - n_outliers
+    ground = lo + torch.rand(n_ground, 3, generator=g) * (hi - lo)
+    ground[:, 1] = -1.6 + 0.05 * torch.randn(n_ground, generator=g)
+    vol = lo + torch.rand(n_vol, 3, generator=g) * (hi - lo)
+    far = torch.randn(n_outliers, 3, generator=g)
+    far = far / far.norm(dim=1, keepdim=True) * (1000.0 + 4000.0 * torch.rand(n_outliers, 1, generator=g))
+    pts = torch.cat([ground, vol, far])
+    return pts[torch.randperm(n, generator=g)].contiguous()
+
+
+def actor_points(n: int, seed: int = 0) -> torch.Tensor:
+    """An aggregated lidar cloud [n, 3] of one actor: points on the faces of the ACTOR_EXTENT box."""
+    g = torch.Generator().manual_seed(seed)
+    ext = torch.tensor(ACTOR_EXTENT)
+    p = (torch.rand(n, 3, generator=g) - 0.5) * ext
+    axis = torch.randint(0, 3, (n,), generator=g)
+    side = torch.where(torch.rand(n, generator=g) < 0.5, -0.5, 0.5)
+    p[torch.arange(n), axis] = side * ext[axis]
+    return p.contiguous()
+
+
 def make_camera(width: int = 1920, height: int = 1280, c2w: Optional[np.ndarray] = None, time: float = 0.0) -> Camera:
     if c2w is None:
         c2w = np.concatenate([np.eye(3), np.zeros((3, 1))], axis=1)
