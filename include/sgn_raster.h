@@ -599,6 +599,34 @@ size_t sgn_knn_scratch_bytes(int64_t n, int64_t m /* 0 without a query set */);
 int sgn_knn(const float* points, int64_t n, const float* query, int64_t m, int k, float* dist, int32_t* idx, float* log_scales,
             void* scratch, size_t scratch_bytes, void* stream);
 
+/* ---- lidar depth supervision (Street Gaussians' depth term; the reference's batch["depth_image"], sgn_datamanager.py:360-361,
+ * and the depth_result its eval calls, sgn_splatfacto.py:1160-1168) ------------------------------------------------------------
+ * sgn_lidar_depth_map: points [M,3] fp32 (device) into depth_map [H,W] fp32 (device; H, W = cam->height, cam->width) for the
+ * camera the render uses.  to_world: NULL (the points are in the world frame) or a HOST 3x4 row-major sweep-to-world matrix,
+ * composed with cam->viewmat in fp64 and rounded once to fp32.  A point's camera-space position pv, its depth z = pv.z and its
+ * pixel centre u = (pv.x * rw) * fx + cx, v = (pv.y * rw) * fy + cy with rw = 1 / (z + 1e-6) are the projection's own
+ * individually rounded arithmetic.  A point with z <= clip_thresh, or with u or v outside [0, W) x [0, H), is dropped; any
+ * other goes to pixel (floor(u), floor(v)), where the nearest return wins.  Pixels without a return are 0.  The map is the same
+ * bits every run; M = 0 is valid (an all-zero map).  cam->clip_thresh must be >= 0.  No host synchronisation.
+ *
+ * Loss over the valid pixels (target > 0 and, with a mask [H,W], mask != 0): *loss = weight * sum |depth - target| / n_valid,
+ * exactly 0 when n_valid = 0; *n_valid (device int32) is what the backward divides by.  The backward writes all of v_depth:
+ * grad_loss * weight * sign(depth - target) / n_valid on the valid pixels, 0 elsewhere (grad_loss: device scalar, NULL = 1).
+ *
+ * Metrics over the same valid pixels, with d = max(depth, 1e-3f), t = target: out[8] (device fp32) = {abs_rel = mean |d-t|/t,
+ * sq_rel = mean (d-t)^2/t, rmse = sqrt(mean (d-t)^2), rmse_log = sqrt(mean (log d - log t)^2), a1, a2, a3 = fraction with
+ * max(d/t, t/d) < 1.25^k, n_valid}; NaN means when n_valid = 0.
+ * Loss and metrics sum in fp64 in a fixed order (bit-identical run to run).  Null inputs, an empty image, a null output
+ * (SGN_ERR_INVALID) or a short scratch (SGN_ERR_WORKSPACE) launch nothing. */
+int sgn_lidar_depth_map(const float* points, int64_t M, const sgn_camera* cam, const float* to_world, float* depth_map, void* stream);
+size_t sgn_depth_scratch_bytes(void);
+int sgn_depth_loss_fwd(int H, int W, const float* depth, const float* target, const float* mask, float weight, float* loss,
+                       int32_t* n_valid, void* scratch, size_t scratch_bytes, void* stream);
+int sgn_depth_loss_bwd(int H, int W, const float* depth, const float* target, const float* mask, float weight, const int32_t* n_valid,
+                       const float* grad_loss, float* v_depth, void* stream);
+int sgn_depth_metrics(int H, int W, const float* depth, const float* target, const float* mask, float* out, void* scratch,
+                      size_t scratch_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

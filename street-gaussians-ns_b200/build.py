@@ -32,6 +32,7 @@ SOURCES = {
     "collective.cu": [],  # the refinement rules mirror torch's separately rounded elementwise kernels
     "camera.cu": [],  # IEEE sinf / cosf / sqrtf (no fast math)
     "knn.cu": [],  # distances through explicit _rn intrinsics: the box bound must not exceed a point's distance
+    "depth.cu": [],  # the lidar projection is the projection's xf arithmetic; IEEE log / division in the metrics
 }
 
 

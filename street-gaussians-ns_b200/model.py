@@ -11,7 +11,8 @@ parts of ``SplatfactoModel`` it inherits (street_gaussians_ns/sgn_splatfacto.py:
   * side-effect attributes ``xys`` (with ``.grad`` = pixel-space mean gradient after backward),
     ``depths, radii, conics, num_tiles_hit, last_size`` on the model and split per sub-model
     (``SplatfactoModel.after_train`` reads ``self.xys.grad`` and ``self.radii``, :513-541);
-  * ``get_loss_dict`` (L1 + SSIM + sky accumulation + object-accumulation entropy);
+  * ``get_loss_dict`` (L1 + SSIM + sky accumulation + object-accumulation entropy, + the lidar depth term when
+    ``depth_loss_mult > 0``);
   * ``get_metrics_dict`` (per-step psnr, Gaussian count, scale / opacity / radii means: one reduction kernel),
     ``get_image_metrics_and_images`` and ``get_outputs_for_camera`` (eval).
 
@@ -63,6 +64,8 @@ class SceneGraphConfig:
     alpha_clamp_bwd: float = 0.99
     render_background_acc: bool = True
     fused_loss: bool = True  # L1 / sky / entropy and SSIM terms through the loss kernels (loss.py) instead of torch ops
+    # weight of the lidar depth term (depth.py): w * mean |depth - target| over the pixels with a return; 0 = off
+    depth_loss_mult: float = 0.0
     # refinement (sgn_splatfacto.py:550-646): the sub-model configs of sgn_config.py:46-66 (background / object template)
     refine: RefineSettings = field(default_factory=lambda: RefineSettings(cull_alpha_thresh=0.02))
     object_refine: RefineSettings = field(default_factory=lambda: RefineSettings(cull_alpha_thresh=0.005))
@@ -333,6 +336,7 @@ class SceneGraphRasterModel(torch.nn.Module):
         self.xys = self.depths = self.radii = self.conics = self.num_tiles_hit = None
         self.last_size = None
         self._holder = None
+        self._last_camera = None
         self._frame_cache: dict = {}
         self.__dict__["_serial"] = next(_MODEL_SERIAL)  # names this model in raster's static segment-table cache (ids are recycled)
         self._grad_sink = _FullArenaSink() if self.config.full_gradient_arena else _GradSink()
@@ -546,6 +550,7 @@ class SceneGraphRasterModel(torch.nn.Module):
         frame = self._frame(camera)
         H, W = camera.height, camera.width
         self.last_size = (H, W)
+        self._last_camera = camera  # the nominal camera: a batch's lidar sweep is projected with it (_depth_target)
         view = self._camera_view(camera)
         if self.config.use_sky_sphere and self.env_map is not None:
             sky = self.env_map(camera, self.training) if view is None else self.env_map(camera, self.training, view=view)
@@ -814,7 +819,13 @@ class SceneGraphRasterModel(torch.nn.Module):
     # ------------------------------------------------------------------------------------------
     def get_loss_dict(self, outputs, batch, metrics_dict=None) -> Dict[str, torch.Tensor]:
         """sgn_splatfacto.py:1042-1094 + scene graph :376-391.  ``batch["image"]`` may be the float image or the
-        uint8 one the data loader holds (converted as the reference does: ``.float() / 255``)."""
+        uint8 one the data loader holds (converted as the reference does: ``.float() / 255``).
+
+        With ``depth_loss_mult > 0`` and a lidar target in the batch (see ``_depth_target``), ``depth_loss`` =
+        depth_loss_mult * mean |depth - target| over the pixels with a return (and mask != 0): Street Gaussians' lidar depth
+        term, which the reference's nerfstudio port dropped.  Its gradient reaches the geometry through the rendered depth,
+        ``where(alpha > 1e-3, d / alpha, 10)``: a return on a pixel with alpha <= 1e-3 adds to the loss value but pulls on
+        nothing."""
         c = self.config
         want_sky = "semantic" in batch and c.sky_acc_loss_mult > 0
         want_ent = c.object_acc_entropy_loss_mult > 0.0 and self.step > c.refine.stop_split_at  # background_model.stop_split_at (:386)
@@ -867,11 +878,29 @@ class SceneGraphRasterModel(torch.nn.Module):
                 oa = torch.clamp(outputs["object_acc"], min=1e-5, max=1 - 1e-5)
                 losses["object_acc_entropy_loss"] = c.object_acc_entropy_loss_mult * -(
                     oa * torch.log(oa) + (1.0 - oa) * torch.log(1.0 - oa)).mean()
+        if c.depth_loss_mult > 0:
+            target = self._depth_target(batch)
+            if target is not None:
+                from .depth import depth_loss_torch, fused_depth_loss
+                term = fused_depth_loss if fused else depth_loss_torch
+                losses["depth_loss"] = term(outputs["depth"], target, batch.get("mask"), c.depth_loss_mult)
         co = self.camera_optimizer
         if self.training and co is not None and co.mode != "off":
             terms = getattr(self, "_camera_terms", None)
             losses["camera_opt_regularizer"] = terms[0] if terms is not None else co.regularizer()
         return losses
+
+    def _depth_target(self, batch) -> Optional[torch.Tensor]:
+        """The lidar depth target [H,W,1] of ``batch``, or None: ``batch["depth_image"]`` as it is (0 = no measurement), else
+        ``batch["lidar_points"]`` [M,3] (with the optional 3x4 ``batch["lidar_to_world"]``) projected by ``depth.lidar_depth_map``
+        with the nominal camera of the last ``get_outputs``: the sweep is registered with the dataset's vehicle pose and
+        calibration, not with the camera optimizer's correction (which still feels the term through the rendered depth)."""
+        if "depth_image" in batch:
+            return batch["depth_image"]
+        if "lidar_points" not in batch:
+            return None
+        from .depth import lidar_depth_map
+        return lidar_depth_map(batch["lidar_points"], self._last_camera, batch.get("lidar_to_world"), self._settings(class_streams=True))
 
     def _fused_metrics_ok(self, rgb: torch.Tensor) -> bool:
         return self.config.fused_loss and rgb.is_cuda
@@ -921,7 +950,10 @@ class SceneGraphRasterModel(torch.nn.Module):
         ``lpips`` when ``self.lpips`` is a callable (it receives the masked [1,3,H,W] gt and rgb, in that order).  Fused path:
         psnr from ``sgn_metrics``, ssim = 1 - the SSIM loss kernel at weight 1.  Images: ``img`` = cat([gt, rgb], dim=1), built
         before masking as the reference does; ``accumulation`` and ``depth`` as the model's [H,W,1] maps, not colour-mapped.
-        Unlike the reference, ``outputs["rgb"]`` and ``batch["image"]`` are not multiplied by the mask in place."""
+        Unlike the reference, ``outputs["rgb"]`` and ``batch["image"]`` are not multiplied by the mask in place.  When the batch
+        carries a lidar target (``depth_image`` or ``lidar_points``, see ``_depth_target``), the depth metrics of
+        ``depth.depth_metrics`` over the pixels with a return (and mask != 0) are added as ``depth_abs_rel``, ``depth_sq_rel``,
+        ``depth_rmse``, ``depth_rmse_log``, ``depth_a1``, ``depth_a2`` and ``depth_a3`` (NaN when no pixel has a return)."""
         rgb, gt = outputs["rgb"], batch["image"]
         gt_f = gt.float() / 255.0 if gt.dtype == torch.uint8 else gt
         mask = batch.get("mask")
@@ -943,6 +975,12 @@ class SceneGraphRasterModel(torch.nn.Module):
                 if masked is None:
                     masked = (gt_f * mask, rgb * mask) if mask is not None else (gt_f, rgb)
                 metrics["lpips"] = float(self.lpips(torch.moveaxis(masked[0], -1, 0)[None], torch.moveaxis(masked[1], -1, 0)[None]))
+            target = self._depth_target(batch)
+            if target is not None:
+                # the depth_result the reference's eval calls but never defines (sgn_splatfacto.py:1160-1168)
+                from .depth import METRIC_NAMES, depth_metrics
+                vals = depth_metrics(outputs["depth"], target, mask).tolist()
+                metrics.update({f"depth_{k}": v for k, v in zip(METRIC_NAMES[:7], vals[:7])})
         images = {"img": img, "accumulation": outputs["accumulation"], "depth": outputs["depth"]}
         return metrics, images
 

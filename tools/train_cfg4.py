@@ -26,7 +26,7 @@ sys.path.insert(0, ROOT)
 def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int = 100, start_step: int = 600,
         actor_range: float = 45.0, pipeline_chunks: int = 0, overlap: bool = False, resident_table: bool = True,
         async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True, sky: bool = False, metrics: bool = False,
-        bbox_opt: bool = False, camera_opt: bool = False, sky_view_grad: bool = False) -> dict:
+        bbox_opt: bool = False, camera_opt: bool = False, sky_view_grad: bool = False, lidar_depth: float = 0.0) -> dict:
     """One measurement.  torch.distributed must already be initialised when WORLD_SIZE > 1.  Returns the result dict on
     rank 0 (None elsewhere).  ``sky``: the reference's default learnable sky (use_sky_sphere, a 1024^2 cube map stepped by
     the same Adam launch at the ``sky_sphere`` group's lr 0.005, sgn_config.py:72-75).  ``metrics``: every step also computes
@@ -35,7 +35,10 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     (frame, box), stepped by the same Adam launch at the ``bbox_opt`` group's lr 1e-3, sgn_config.py:80-83).
     ``camera_opt``: trainable camera poses (``camera_optimizer`` mode "SO3xR3" over the indexed rig cameras, the ``camera_opt``
     group's lr 1e-3 and its 100-step gradient accumulation, sgn_config.py:30,76-79).  ``sky_view_grad`` (with ``sky`` and
-    ``camera_opt``): the sky also gives the camera rotation its gradient (CubeMapSky(view_grad=True))."""
+    ``camera_opt``): the sky also gives the camera rotation its gradient (CubeMapSky(view_grad=True)).  ``lidar_depth`` > 0: the
+    lidar depth term at that weight (SceneGraphConfig.depth_loss_mult), against a synthetic sweep per step
+    (``synthetic.street_points(170_000, seed=step)``, about one top-lidar sweep, all drawn onto the device before the first step)
+    projected with the step's camera."""
     import torch
     import torch.distributed as dist
 
@@ -64,7 +67,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     rs = RefineSettings(refine_every=refine_every)
     cfg = SceneGraphConfig(use_sky_sphere=sky, ssim_lambda=ssim_lambda, fused_loss=fused_loss, full_gradient_arena=world > 1, refine=rs, async_binning=async_binning,
                            object_refine=RefineSettings(refine_every=refine_every, cull_alpha_thresh=0.005),
-                           num_train_data=len(cams), refine_record=True)
+                           num_train_data=len(cams), refine_record=True, depth_loss_mult=lidar_depth)
     env_map = None
     if sky:
         from street_gaussians_ns_b200.sky import CubeMapSky
@@ -130,12 +133,18 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         model.config.async_binning = True
         torch.cuda.synchronize()
 
+    # one sweep per step, drawn before the timed steps as a data loader would have prefetched them
+    sweeps = [syn.street_points(170_000, seed=start_step + i).to(dev) for i in range(warmup + steps)] if lidar_depth > 0 else []
+
     def one(i):
         step = start_step + i
         mine = [cams[dp.camera_for_rank(step, r, world, len(cams))] for r in range(world)]
         # after a refinement replaced parameter tensors the model drops the resident table; a timestamp's rows are then
         # re-staged (and kept on the device) the first time it is rendered again
-        return step_fn(step, mine[rank], {"image": gt}, all_cameras=mine if world > 1 else None)
+        batch = {"image": gt}
+        if lidar_depth > 0:
+            batch["lidar_points"] = sweeps[i % len(sweeps)]
+        return step_fn(step, mine[rank], batch, all_cameras=mine if world > 1 else None)
 
     def sync():
         if world > 1:
@@ -202,6 +211,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                    **({"bbox_opt": "BoxPoseOptimizer(simple), Adam lr 1e-3"} if bbox_opt else {}),
                    **({"camera_opt": "CameraPoseOptimizer(SO3xR3), Adam lr 1e-3, gradient accumulation 100"} if camera_opt else {}),
                    **({"sky_view_grad": "the sky's rotation cotangent reaches the camera"} if sky_view_grad else {}),
+                   **({"lidar_depth": f"depth_loss_mult {lidar_depth}, street_points(170_000, seed=step) per step"} if lidar_depth > 0 else {}),
                    "loss": "fused kernels" if fused_loss else "torch ops", "metrics": "get_metrics_dict every step" if metrics else "none",
                    "start_step": start_step, "refine_every": refine_every,
                    "refinement_kernels_loaded_before_timing": refine_warm,
@@ -235,6 +245,8 @@ def main():
     ap.add_argument("--bbox-opt", action="store_true", help="train the box corrections (the reference's bbox_optimizer mode 'simple')")
     ap.add_argument("--camera-opt", action="store_true", help="train the camera poses (camera_optimizer mode 'SO3xR3', accumulation 100)")
     ap.add_argument("--sky-view-grad", action="store_true", help="with --sky --camera-opt: the sky also trains the camera rotation")
+    ap.add_argument("--lidar-depth", type=float, default=0.0, metavar="W",
+                    help="> 0: the lidar depth term at weight W against a synthetic 170 k-point sweep per step")
     args = ap.parse_args()
     if args.sky_view_grad and not (args.sky and args.camera_opt):
         ap.error("--sky-view-grad needs --sky and --camera-opt")
@@ -250,7 +262,7 @@ def main():
     res = run(args.steps, args.warmup, args.scale, args.refine_every, args.start_step, args.actor_range, args.pipeline_chunks,
               args.overlap, not args.host_table, ssim_lambda=args.ssim_lambda, fused_loss=not args.torch_loss, sky=args.sky,
               metrics=args.metrics, bbox_opt=args.bbox_opt, camera_opt=args.camera_opt,
-              sky_view_grad=args.sky_view_grad)
+              sky_view_grad=args.sky_view_grad, lidar_depth=args.lidar_depth)
     if res is not None:
         print(json.dumps(res))
     if world > 1:
