@@ -627,6 +627,34 @@ int sgn_depth_loss_bwd(int H, int W, const float* depth, const float* target, co
 int sgn_depth_metrics(int H, int W, const float* depth, const float* target, const float* mask, float* out, void* scratch,
                       size_t scratch_bytes, void* stream);
 
+/* ---- per-Gaussian semantic logits (Street Gaussians' semantic term; the reference's batch["semantic"], data/sgn_dataset.py:125)
+ * logits [H,W,C] fp32 (the semantic map sgn_blend_extra_fwd composites from extra[N,C]), labels [H,W] int64, mask [H,W] fp32 or
+ * NULL; 1 <= C <= 64.  A pixel is valid when 0 <= label < C and (mask is NULL or mask != 0): any other label (e.g. 255) is ignored.
+ *
+ * Loss: *loss = weight * sum_valid CE(p) / n_valid with CE(p) = logsumexp(S[p,:]) - S[p,label], logsumexp in fp32 with the max
+ * subtracted; exactly 0 when n_valid = 0.  *n_valid (device int32) is what the backward divides by.  The backward writes all of
+ * v_logits: grad_loss * weight / n_valid * (softmax(S[p]) - onehot(label)) on the valid pixels, 0 elsewhere (grad_loss: device
+ * scalar, NULL = 1).  Sums in fp64 per-block partials added in a fixed order (bit-identical run to run).
+ *
+ * Metrics: confusion [C,C] (device int64, overwritten) = counts of (label, argmax S) over the valid pixels, a tie going to the
+ * lowest class index; integer atomics, so the counts are the same every run.
+ *
+ * Refinement carry: one further per-row tensor src [n,width] (1 <= width <= 64) and, optionally, its Adam moments rebuilt with
+ * the row map of sgn_refine_apply for the same flags / scan / totals: [survivors | split samples, sample-major, each a copy of
+ * its parent | duplicates]; survivors keep their moments, new rows get zero moments.  This is exactly what sgn_refine_apply
+ * does to features_dc.  dst [totals[0] + n_split_samples * totals[1] + totals[2], width].
+ * Null inputs, C or width out of range (SGN_ERR_INVALID) or a short scratch (SGN_ERR_WORKSPACE) launch nothing. */
+size_t sgn_semantic_scratch_bytes(void);
+int sgn_semantic_loss_fwd(int H, int W, int C, const float* logits, const int64_t* labels, const float* mask, float weight, float* loss,
+                          int32_t* n_valid, void* scratch, size_t scratch_bytes, void* stream);
+int sgn_semantic_loss_bwd(int H, int W, int C, const float* logits, const int64_t* labels, const float* mask, float weight,
+                          const int32_t* n_valid, const float* grad_loss, float* v_logits, void* stream);
+int sgn_semantic_metrics(int H, int W, int C, const float* logits, const int64_t* labels, const float* mask, int64_t* confusion,
+                         void* stream);
+int sgn_refine_carry(int n, const sgn_refine_config* cfg, const uint8_t* flags, const int32_t* scan, const int32_t* totals,
+                     const float* src, float* dst, int width, const float* src_m, const float* src_v, float* dst_m, float* dst_v,
+                     void* stream);
+
 #ifdef __cplusplus
 }
 #endif

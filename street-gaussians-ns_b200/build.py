@@ -33,6 +33,7 @@ SOURCES = {
     "camera.cu": [],  # IEEE sinf / cosf / sqrtf (no fast math)
     "knn.cu": [],  # distances through explicit _rn intrinsics: the box bound must not exceed a point's distance
     "depth.cu": [],  # the lidar projection is the projection's xf arithmetic; IEEE log / division in the metrics
+    "semantic.cu": [],  # IEEE expf / logf / division in the cross-entropy; the carry only copies
 }
 
 

@@ -66,6 +66,11 @@ class SceneGraphConfig:
     fused_loss: bool = True  # L1 / sky / entropy and SSIM terms through the loss kernels (loss.py) instead of torch ops
     # weight of the lidar depth term (depth.py): w * mean |depth - target| over the pixels with a return; 0 = off
     depth_loss_mult: float = 0.0
+    # per-Gaussian semantic logits (semantic.py): classes per Gaussian, 0 = none (3 for the reference's SemanticType: DEFAULT,
+    # GROUND, SKY); with classes the render publishes outputs["semantic"] [H,W,C]
+    semantic_classes: int = 0
+    # weight of the semantic cross-entropy term against batch["semantic"]; 0 = off
+    semantic_loss_mult: float = 0.0
     # refinement (sgn_splatfacto.py:550-646): the sub-model configs of sgn_config.py:46-66 (background / object template)
     refine: RefineSettings = field(default_factory=lambda: RefineSettings(cull_alpha_thresh=0.02))
     object_refine: RefineSettings = field(default_factory=lambda: RefineSettings(cull_alpha_thresh=0.005))
@@ -137,11 +142,19 @@ class GaussianSubModel(torch.nn.Module):
     conics = _FrameSlice("conics")
     num_tiles_hit = _FrameSlice("num_tiles_hit")
 
-    def __init__(self, params: GaussianSet):
+    def __init__(self, params: GaussianSet, semantic_classes: int = 0):
         super().__init__()
         self.gauss_params = torch.nn.ParameterDict(
             {k: torch.nn.Parameter(getattr(params, k).detach().clone()) for k in
              ("means", "scales", "quats", "features_dc", "features_rest", "opacities")})
+        # per-Gaussian class logits [n, C], zeros at the start.  Kept outside gauss_params: the six-tensor paths (gradient arena,
+        # FusedAdam's six tensors per sub-model, sgn_refine_apply, the data-parallel layout) never see it.  Its gradient comes
+        # through autograd (render_frame's ``extra``); the optimizer steps it as the row group "semantic"
+        if semantic_classes > 0:
+            self.semantic_logits = torch.nn.Parameter(torch.zeros(params.means.shape[0], int(semantic_classes),
+                                                                  device=params.means.device, dtype=torch.float32))
+        else:
+            self.semantic_logits = None
         self.xys = self.depths = self.radii = self.conics = self.num_tiles_hit = None
         self.last_size = None
         # densification statistics (sgn_splatfacto.py:513-541), created by the first after_train
@@ -172,6 +185,10 @@ class GaussianSubModel(torch.nn.Module):
                 shape = (rows,) + (tuple(want.shape[1:]) if want is not None else tuple(old.shape[1:]))
                 if tuple(old.shape) != shape:
                     self.gauss_params[k] = torch.nn.Parameter(torch.zeros(shape, device=old.device, dtype=old.dtype))
+            sem = self.semantic_logits
+            want = state_dict.get("semantic_logits")
+            if sem is not None and want is not None and tuple(sem.shape) != tuple(want.shape):
+                self.semantic_logits = torch.nn.Parameter(torch.zeros(tuple(want.shape), device=sem.device, dtype=sem.dtype))
             d = self.__dict__
             d["xys_grad_norm"] = d["vis_counts"] = d["max_2Dsize"] = None  # statistics of the old rows are meaningless
         return super().load_state_dict(state_dict, **kwargs)
@@ -324,9 +341,10 @@ class SceneGraphRasterModel(torch.nn.Module):
         # :91).  None, or one in mode "off": the boxes are rendered as annotated, by the same calls as without it
         self.bbox_optimizer = bbox_optimizer
         self.all_models = torch.nn.ModuleDict()
-        self.all_models["background"] = GaussianSubModel(background)
+        C = int(self.config.semantic_classes)
+        self.all_models["background"] = GaussianSubModel(background, C)
         for obj_id, ps in actors.items():
-            self.all_models[self.get_object_model_name(obj_id)] = GaussianSubModel(ps)
+            self.all_models[self.get_object_model_name(obj_id)] = GaussianSubModel(ps, C)
         self.poses_at = poses_at or (lambda t: [])
         # the learnable sky (EnvLight, sgn_splatfacto.py:109-150): sky.CubeMapSky on this library's kernels, or any callable
         # (camera, train) -> [H, W, 3] such as the reference's EnvLight on nvdiffrast
@@ -569,8 +587,14 @@ class SceneGraphRasterModel(torch.nn.Module):
                     self._anchor = torch.zeros(1, device=flat[0].device, requires_grad=True)
                 anchor = self._anchor
         pose = self._box_poses(frame)
-        out, holder = raster.render_frame(frame, self._settings(class_streams=True), sky=sky, grad_sink=sink, anchor=anchor, pose=pose,
-                                          view=view)
+        extra = self._semantic_rows(frame)
+        if extra is None:
+            out, holder = raster.render_frame(frame, self._settings(class_streams=True), sky=sky, grad_sink=sink, anchor=anchor,
+                                              pose=pose, view=view)
+        else:
+            out, holder = raster.render_frame(frame, self._settings(class_streams=True), sky=sky, grad_sink=sink, anchor=anchor,
+                                              extra=extra, pose=pose, view=view)
+            out["semantic"] = out.pop("extra")
         self._holder = holder
         self._publish_side_effects(frame, holder)
         if isinstance(holder.M, raster.LazyCount):
@@ -587,6 +611,8 @@ class SceneGraphRasterModel(torch.nn.Module):
                 res["sky"] = sky
             res["object_acc"] = torch.zeros(H, W, 1, device=dev)
             res["background_acc"] = torch.zeros(H, W, 1, device=dev)
+            if extra is not None:
+                res["semantic"] = torch.zeros(H, W, extra.shape[1], device=dev)
             return res
         if not self.training:
             # eval-only extra renders (scene graph :367-372): per-class rgb
@@ -598,6 +624,15 @@ class SceneGraphRasterModel(torch.nn.Module):
                     # (scene graph :264-267), which get_outputs publishes as object_rgb AND object_depth (:371-372)
                     out["object_depth"] = torch.zeros(H, W, 1, device=self.device)
         return out
+
+    def _semantic_rows(self, frame: Frame) -> Optional[torch.Tensor]:
+        """The frame's semantic logits [N, C] in its row order (the visible sub-models' ``semantic_logits``, concatenated in
+        segment order), or None without semantic classes.  The logits are static per Gaussian: actors carry no time
+        dependence for them."""
+        if self.config.semantic_classes <= 0:
+            return None
+        mods = self.all_models._modules
+        return torch.cat([mods[seg.name].semantic_logits for seg in frame.segments])
 
     def _class_rgb(self, frame: Frame, cls: int, sky, pose=None):
         segs = [s for s in frame.segments if s.cls == cls]
@@ -730,17 +765,29 @@ class SceneGraphRasterModel(torch.nn.Module):
         old = [[sub.gauss_params[k].data for k in PARAM_NAMES] for sub in subs]
         new = [o if p is None else [torch.empty((p.out_rows,) + tuple(t.shape[1:]), device=t.device, dtype=t.dtype) for t in o]
                for o, p in zip(old, plans)]
+        # the semantic logits ride along: the same row map as features_dc (sgn_refine_carry), with their moments
+        sem = self.config.semantic_classes > 0
+        old_sem = [sub.semantic_logits.data for sub in subs] if sem else None
+        new_sem = [o if p is None else torch.empty((p.out_rows,) + tuple(o.shape[1:]), device=o.device, dtype=o.dtype)
+                   for o, p in zip(old_sem, plans)] if sem else None
         if any(p is not None for p in plans):
-            src_m, dst_m = adapter.relayout(new, [p is not None for p in plans])
+            from .semantic import refine_carry
+            changed = [p is not None for p in plans]
+            src_m, dst_m = adapter.relayout(new, changed, {"semantic": new_sem} if sem else None)
             for i, p in enumerate(plans):
                 if p is not None:
                     refine.apply_plan(p, old[i], new[i], src_m[i], dst_m[i])
                     for k, t in zip(PARAM_NAMES, new[i]):
                         subs[i].gauss_params[k] = torch.nn.Parameter(t)
-            adapter.commit([[sub.gauss_params[k] for k in PARAM_NAMES] for sub in subs], [p is not None for p in plans])
+                    if sem:
+                        ms, md = adapter.row_moments("semantic", i)
+                        refine_carry(p, old_sem[i], new_sem[i], ms, md)
+                        subs[i].semantic_logits = torch.nn.Parameter(new_sem[i])
+            adapter.commit([[sub.gauss_params[k] for k in PARAM_NAMES] for sub in subs], changed,
+                           {"semantic": [sub.semantic_logits for sub in subs]} if sem else None)
             self.invalidate_frames()
         for i, st in enumerate(resets):
-            if st is not None:  # opacity reset on the survivors (:629-642)
+            if st is not None:  # opacity reset on the survivors (:629-642); the semantic logits are left alone
                 subs[i].gauss_params["opacities"].data.clamp_(max=refine.opacity_reset_logit(st))
                 adapter.zero_moments(i, 5)
         if records:  # the logged counters of all sub-models: one read-back, after everything else has been enqueued
@@ -796,6 +843,12 @@ class SceneGraphRasterModel(torch.nn.Module):
         ``FusedAdam`` is built over.  ``present_submodels()`` names the ones in the last frame's gradient arena."""
         return [[sub.gauss_params[k] for k in PARAM_NAMES] for sub in self.all_models._modules.values()]
 
+    def semantic_params(self) -> List[torch.Tensor]:
+        """Per sub-model (all_models order) its ``semantic_logits``: the row group ``FusedAdam(..., rows={"semantic":
+        (model.semantic_params(), lr)})`` steps (and ``refinement_after`` carries)."""
+        assert self.config.semantic_classes > 0, "the model has no semantic logits (SceneGraphConfig.semantic_classes = 0)"
+        return [sub.semantic_logits for sub in self.all_models._modules.values()]
+
     def present_submodels(self) -> List[int]:
         index = {n: i for i, n in enumerate(self.all_models._modules)}
         return [index[n] for n in self.visible_model_names]
@@ -825,7 +878,14 @@ class SceneGraphRasterModel(torch.nn.Module):
         depth_loss_mult * mean |depth - target| over the pixels with a return (and mask != 0): Street Gaussians' lidar depth
         term, which the reference's nerfstudio port dropped.  Its gradient reaches the geometry through the rendered depth,
         ``where(alpha > 1e-3, d / alpha, 10)``: a return on a pixel with alpha <= 1e-3 adds to the loss value but pulls on
-        nothing."""
+        nothing.
+
+        With ``semantic_loss_mult > 0``, semantic classes and ``batch["semantic"]``, ``semantic_loss`` = semantic_loss_mult *
+        mean cross-entropy of ``outputs["semantic"]`` against the labels over the pixels with a label in [0, C) (and mask != 0).
+        Sky-labelled pixels are supervised like any other class: the semantic map there is the blend of whatever Gaussians the
+        pixel sees, and ``sky_accumulation`` separately pushes their accumulation towards 0, which also shrinks the blended logits
+        (weights sum to the accumulation).  The two terms therefore pull against each other on sky pixels; nothing special-cases
+        that, as a segmentation with a sky class gives both signals."""
         c = self.config
         want_sky = "semantic" in batch and c.sky_acc_loss_mult > 0
         want_ent = c.object_acc_entropy_loss_mult > 0.0 and self.step > c.refine.stop_split_at  # background_model.stop_split_at (:386)
@@ -884,6 +944,10 @@ class SceneGraphRasterModel(torch.nn.Module):
                 from .depth import depth_loss_torch, fused_depth_loss
                 term = fused_depth_loss if fused else depth_loss_torch
                 losses["depth_loss"] = term(outputs["depth"], target, batch.get("mask"), c.depth_loss_mult)
+        if c.semantic_loss_mult > 0 and "semantic" in batch and "semantic" in outputs:
+            from .semantic import fused_semantic_loss, semantic_loss_torch
+            term = fused_semantic_loss if fused else semantic_loss_torch
+            losses["semantic_loss"] = term(outputs["semantic"], batch["semantic"], batch.get("mask"), c.semantic_loss_mult)
         co = self.camera_optimizer
         if self.training and co is not None and co.mode != "off":
             terms = getattr(self, "_camera_terms", None)
@@ -953,7 +1017,9 @@ class SceneGraphRasterModel(torch.nn.Module):
         Unlike the reference, ``outputs["rgb"]`` and ``batch["image"]`` are not multiplied by the mask in place.  When the batch
         carries a lidar target (``depth_image`` or ``lidar_points``, see ``_depth_target``), the depth metrics of
         ``depth.depth_metrics`` over the pixels with a return (and mask != 0) are added as ``depth_abs_rel``, ``depth_sq_rel``,
-        ``depth_rmse``, ``depth_rmse_log``, ``depth_a1``, ``depth_a2`` and ``depth_a3`` (NaN when no pixel has a return)."""
+        ``depth_rmse``, ``depth_rmse_log``, ``depth_a1``, ``depth_a2`` and ``depth_a3`` (NaN when no pixel has a return).  With
+        semantic classes and ``batch["semantic"]``: ``semantic_acc`` (pixel accuracy of the argmax) and ``semantic_miou`` (mean IoU
+        over the classes whose union is > 0) over the pixels with a label in [0, C) (and mask != 0)."""
         rgb, gt = outputs["rgb"], batch["image"]
         gt_f = gt.float() / 255.0 if gt.dtype == torch.uint8 else gt
         mask = batch.get("mask")
@@ -981,6 +1047,9 @@ class SceneGraphRasterModel(torch.nn.Module):
                 from .depth import METRIC_NAMES, depth_metrics
                 vals = depth_metrics(outputs["depth"], target, mask).tolist()
                 metrics.update({f"depth_{k}": v for k, v in zip(METRIC_NAMES[:7], vals[:7])})
+            if "semantic" in batch and "semantic" in outputs:
+                from .semantic import semantic_metrics
+                metrics.update(semantic_metrics(outputs["semantic"], batch["semantic"], mask))
         images = {"img": img, "accumulation": outputs["accumulation"], "depth": outputs["depth"]}
         return metrics, images
 
@@ -1002,10 +1071,14 @@ def _psnr(preds: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
 class _NoOptimizer:
     """refinement_after(None, ...): parameters only."""
 
-    def relayout(self, new, changed):
+    def relayout(self, new, changed, rows=None):
         return [None] * len(new), [None] * len(new)
 
-    def commit(self, params, changed):
+    def row_moments(self, name: str, sub: int):
+        """(old (exp_avg, exp_avg_sq), new pair) of a changed sub-model's tensor of row group ``name``, or (None, None)."""
+        return None, None
+
+    def commit(self, params, changed, rows=None):
         pass
 
     def zero_moments(self, sub: int, k: int):
@@ -1018,11 +1091,27 @@ class _FusedAdamAdapter(_NoOptimizer):
 
     def __init__(self, opt):
         self.opt = opt
+        self._rows = {}
 
-    def relayout(self, new, changed):
+    def relayout(self, new, changed, rows=None):
+        """``rows``: the row groups' tensors after the refinement (name -> one per sub-model: new ones for the changed
+        sub-models), for the groups the model carries; a group the optimizer does not hold is left out."""
         opt = self.opt
         old_params = opt._params
-        old_m, old_v, old_off = opt.rebuild(new)
+        rows = {k: v for k, v in (rows or {}).items() if k in opt.row_index}
+        old_index = dict(opt.row_index)
+        old_m, old_v, old_off = opt.rebuild(new, rows)
+        self._rows = {}
+        for name, ts in rows.items():  # changed sub-models: old moments (old layout) -> new moment views (zeroed) for the carry
+            pairs = []
+            for i, ch in enumerate(changed):
+                if not ch:
+                    pairs.append(None)
+                    continue
+                t, o = old_params[old_index[name] + i], int(old_off[old_index[name] + i])
+                pairs.append(((old_m[o:o + t.numel()].view(t.shape), old_v[o:o + t.numel()].view(t.shape)),
+                              opt.row_moment_views(name, i)))
+            self._rows[name] = pairs
         src, dst = [], []
         for i, ch in enumerate(changed):
             if ch:
@@ -1041,8 +1130,13 @@ class _FusedAdamAdapter(_NoOptimizer):
                 dst.append(None)
         return src, dst
 
-    def commit(self, params, changed):
-        self.opt.rebuild_pointers(params)
+    def row_moments(self, name: str, sub: int):
+        pairs = self._rows.get(name)
+        return (None, None) if pairs is None or pairs[sub] is None else pairs[sub]
+
+    def commit(self, params, changed, rows=None):
+        self.opt.rebuild_pointers(params, {k: v for k, v in (rows or {}).items() if k in self.opt.row_index})
+        self._rows = {}
 
     def zero_moments(self, sub: int, k: int):
         m, v = self.opt.moment_views(6 * sub + k)
@@ -1057,12 +1151,13 @@ class _TorchAdamGroupsAdapter(_NoOptimizer):
     def __init__(self, groups):
         self.groups = groups
         self._new_state = {}
+        self._row_state = {}
 
     def _state(self, k: int, i: int):
         opt = self.groups[PARAM_NAMES[k]]
         return opt, opt.state.get(opt.param_groups[0]["params"][i], {})
 
-    def relayout(self, new, changed):
+    def relayout(self, new, changed, rows=None):
         src, dst = [], []
         for i, ch in enumerate(changed):
             states = [self._state(k, i)[1] for k in range(6)] if ch else []
@@ -1073,9 +1168,39 @@ class _TorchAdamGroupsAdapter(_NoOptimizer):
             src.append([(st["exp_avg"], st["exp_avg_sq"]) for st in states])
             dst.append([(torch.empty_like(t), torch.empty_like(t)) for t in new[i]])
             self._new_state[i] = dst[-1]
+        self._row_state = {}
+        for name, ts in (rows or {}).items():  # a row group with its own Adam in the dict ("semantic"): carried likewise
+            if name not in self.groups:
+                continue
+            opt = self.groups[name]
+            for i, ch in enumerate(changed):
+                st = opt.state.get(opt.param_groups[0]["params"][i], {}) if ch else {}
+                if "exp_avg" in st:
+                    self._row_state[(name, i)] = ((st["exp_avg"], st["exp_avg_sq"]),
+                                                  (torch.empty_like(ts[i]), torch.empty_like(ts[i])))
         return src, dst
 
-    def commit(self, params, changed):
+    def row_moments(self, name: str, sub: int):
+        return self._row_state.get((name, sub), (None, None))
+
+    def commit(self, params, changed, rows=None):
+        for name, ts in (rows or {}).items():
+            if name not in self.groups:
+                continue
+            opt = self.groups[name]
+            plist = opt.param_groups[0]["params"]
+            for i, ch in enumerate(changed):
+                if not ch:
+                    continue
+                st = opt.state.pop(plist[i], {})
+                moved = self._row_state.get((name, i))
+                if moved is not None:
+                    st = dict(st)
+                    st["exp_avg"], st["exp_avg_sq"] = moved[1]
+                plist[i] = ts[i]
+                if st:
+                    opt.state[ts[i]] = st
+        self._row_state = {}
         for i, ch in enumerate(changed):
             if not ch:
                 continue

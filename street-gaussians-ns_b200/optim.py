@@ -17,7 +17,7 @@ Two torch.optim.Adam behaviours the scene graph depends on are kept:
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, Optional, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -60,16 +60,23 @@ class FusedAdam:
 
     def __init__(self, params: Sequence[Sequence[torch.Tensor]], lrs: Dict[str, float] = None, betas=(0.9, 0.999),
                  eps: float = 1e-15, chunk_elems: Optional[int] = None, extra: Optional[Dict[str, Tuple[torch.Tensor, float]]] = None,
-                 reserve_spare: bool = False):
+                 reserve_spare: bool = False, rows: Optional[Dict[str, Tuple[Sequence[torch.Tensor], float]]] = None):
         """``extra``: further tensors stepped by the same launch, name -> (tensor, lr): the reference's other Adam groups on
         the step -- the sky cube map ``env_map.base`` [6, res, res, 3] (sgn_splatfacto.py:114-116; group ``sky`` of
         sgn_config.py:71-108).  Their gradients are not part of the rasterizer's arena (the sky gradient comes out of
         nvdiffrast's backward): pass them to ``step(..., extra_grads={name: grad})``; a tensor without a gradient in a step is
-        skipped like any parameter whose ``.grad`` is None."""
+        skipped like any parameter whose ``.grad`` is None.
+
+        ``rows``: groups of per-row tensors, name -> (one tensor per sub-model, lr), stepped by the same launch: the per-Gaussian
+        semantic logits (group ``semantic``; the reference config names no optimizer for it, so the rate is the caller's).
+        Unlike ``extra`` they change shape at a refinement (``rebuild(params, rows=...)``).  Their moments sit behind the extra
+        tensors'; their gradients, like the extra tensors', are addressed relative to the gradient arena: pass them to
+        ``step(..., row_grads={name: [grad or None per sub-model]})``.  None: the tables and arenas are those without them."""
         self._chunk = chunk_elems if chunk_elems is not None else _lib.load().sgn_adam_chunk_elems()
         self.lrs = dict(REFERENCE_LRS if lrs is None else lrs)
         self.betas, self.eps = betas, eps
         self._extra = dict(extra or {})
+        self._rows = {name: (list(ts), lr) for name, (ts, lr) in (rows or {}).items()}
         self.step_count = 0  # calls of step(); the bias correction uses the per-tensor counts below
         self._install(params)
         if self.device.type == "cuda" and chunk_elems is not None and chunk_elems != _lib.load().sgn_adam_chunk_elems():
@@ -90,8 +97,10 @@ class FusedAdam:
         return torch.zeros(arena_capacity(self.moment_elems), device=self.device)[:self.moment_elems]
 
     # ---- layout ---------------------------------------------------------------------------------------------
-    def _install(self, params: Sequence[Sequence[torch.Tensor]]) -> None:
+    def _install(self, params: Sequence[Sequence[torch.Tensor]], rows: Optional[Dict[str, Sequence[torch.Tensor]]] = None) -> None:
         assert all(len(ps) == 6 for ps in params), "six parameter tensors per sub-model, in PARAM_NAMES order"
+        for name, ts in (rows or {}).items():
+            self._rows[name] = (list(ts), self._rows[name][1])
         flat = [t for ps in params for t in ps]
         self.kinds = [PARAM_NAMES[i % 6] for i in range(len(flat))]
         self.extra_index = {}
@@ -101,6 +110,15 @@ class FusedAdam:
             flat.append(t)
             self.kinds.append("extra:" + name)
             self.lrs["extra:" + name] = lr
+        self.row_index = {}
+        for name, (ts, lr) in self._rows.items():  # behind the extra tensors: one tensor per sub-model
+            assert len(ts) == len(params), f"row group {name}: {len(ts)} tensors for {len(params)} sub-models"
+            self.row_index[name] = len(flat)
+            for t in ts:
+                assert t.is_contiguous() and t.dtype == torch.float32 and t.data_ptr() % 16 == 0, name
+                flat.append(t)
+                self.kinds.append("row:" + name)
+            self.lrs["row:" + name] = lr
         self.device = flat[0].device
         self.sizes = np.array([padded(t.numel()) for t in flat], np.int64)
         self.offsets = np.concatenate([[0], np.cumsum(self.sizes)[:-1]]).astype(np.int64)
@@ -120,11 +138,20 @@ class FusedAdam:
         self.moment_elems = int(self.sizes.sum())                   # + the extra tensors' moments behind it
         self._params = flat  # keep the tensors (and their storage) alive
         self._extra_ptrs = {t.data_ptr() for t, _ in self._extra.values()}
+        self._extra_ptrs |= {t.data_ptr() for ts, _ in self._rows.values() for t in ts}  # addressed relative to the arena too
         self._lr_vec = np.array([self.lrs[k] for k in self.kinds], np.float64)
 
     def extra_tensors(self) -> Dict[str, torch.Tensor]:
         """The further tensors this optimizer steps (``extra``), by name."""
         return {name: t for name, (t, _) in self._extra.items()}
+
+    def row_tensors(self) -> Dict[str, List[torch.Tensor]]:
+        """The per-row groups this optimizer steps (``rows``), by name: one tensor per sub-model."""
+        return {name: list(ts) for name, (ts, _) in self._rows.items()}
+
+    def row_moment_views(self, name: str, sub: int) -> Tuple[torch.Tensor, torch.Tensor]:
+        """exp_avg / exp_avg_sq of sub-model ``sub``'s tensor of row group ``name``."""
+        return self.moment_views(self.row_index[name] + sub)
 
     def set_lr(self, kind: str, lr: float) -> None:
         """Schedulers (e.g. the exponential decay of the means lr, sgn_config.py:85-90) update rates here."""
@@ -139,7 +166,8 @@ class FusedAdam:
 
     # ---- the step -------------------------------------------------------------------------------------------
     def step_table(self, present: Optional[Sequence[int]] = None, full_layout: bool = False, grad_arena: Optional[torch.Tensor] = None,
-                   extra_grads: Optional[Dict[str, torch.Tensor]] = None) -> np.ndarray:
+                   extra_grads: Optional[Dict[str, torch.Tensor]] = None,
+                   row_grads: Optional[Dict[str, Sequence[Optional[torch.Tensor]]]] = None) -> np.ndarray:
         """Advance the step counts of the tensors that have a gradient and return their sgn_adam_tensor rows.
         ``present``: indices of the sub-models that have a gradient this step (None = all).  The gradient arena
         either holds exactly those, back to back in that order (a frame's arena, the default), or has the optimizer's
@@ -155,7 +183,19 @@ class FusedAdam:
                 delta = g.data_ptr() - grad_arena.data_ptr()
                 assert delta % 4 == 0
                 extras.append((i, delta // 4))  # the kernel addresses gradients as grad_arena + offset: any float address works
-        if present is None and not self.extra_index:
+        if self.row_index:  # rows of the per-row groups' tensors that have a gradient this step
+            assert not row_grads or grad_arena is not None, "row_grads need grad_arena (their offsets are relative to it)"
+            for name, gs in (row_grads or {}).items():
+                assert len(gs) == self.num_segments, (name, len(gs))
+                for s, g in enumerate(gs):
+                    if g is None:
+                        continue
+                    i = self.row_index[name] + s
+                    assert g.is_contiguous() and g.dtype == torch.float32 and g.numel() == self._params[i].numel(), (name, s)
+                    delta = g.data_ptr() - grad_arena.data_ptr()
+                    assert delta % 4 == 0
+                    extras.append((i, delta // 4))
+        if present is None and not self.extra_index and not self.row_index:
             idx = slice(None)
             tab = self.table  # grad_offset == arena_offset, chunk0 as installed
         else:
@@ -179,18 +219,22 @@ class FusedAdam:
         return tab
 
     def step(self, grad_arena: torch.Tensor, present: Optional[Sequence[int]] = None, full_layout: bool = False,
-             extra_grads: Optional[Dict[str, torch.Tensor]] = None) -> None:
+             extra_grads: Optional[Dict[str, torch.Tensor]] = None,
+             row_grads: Optional[Dict[str, Sequence[Optional[torch.Tensor]]]] = None) -> None:
         self.step_count += 1
-        self._keep = extra_grads  # the launch is asynchronous: keep the gradient tensors alive until the next step
-        self.launch(self.step_table(present, full_layout, grad_arena, extra_grads), grad_arena)
+        # the launch is asynchronous: keep the gradient tensors alive until the next step
+        self._keep = extra_grads if row_grads is None else (extra_grads, row_grads)
+        self.launch(self.step_table(present, full_layout, grad_arena, extra_grads, row_grads), grad_arena)
 
     def launch(self, tab: np.ndarray, grad_arena: torch.Tensor) -> None:
         """One ``sgn_adam_step`` over the rows of ``tab`` (from step_table, possibly cut by rows_in_range)."""
         assert grad_arena.is_cuda, "FusedAdam runs on the CUDA library only"
         if len(tab) == 0:
             return
-        # rows of the extra tensors (always last) address their gradient relative to the arena, wherever it lives
-        inside = tab[: len(tab) - sum(1 for k in tab["param"] if int(k) in self._extra_ptrs)] if self.extra_index else tab
+        # rows of the extra tensors and the row groups (always last) address their gradient relative to the arena, wherever it
+        # lives
+        outside = self.extra_index or self.row_index
+        inside = tab[: len(tab) - sum(1 for k in tab["param"] if int(k) in self._extra_ptrs)] if outside else tab
         if len(inside):
             need = int((inside["grad_offset"] + inside["numel"]).max())
             assert grad_arena.numel() >= need, (grad_arena.numel(), need)
@@ -233,26 +277,39 @@ class FusedAdam:
         return out
 
     # ---- refinement (sgn_splatfacto.py:459-511) ---------------------------------------------------------------
-    def rebuild(self, params: Sequence[Sequence[torch.Tensor]]) -> Tuple[torch.Tensor, torch.Tensor, np.ndarray]:
+    def rebuild(self, params: Sequence[Sequence[torch.Tensor]], rows: Optional[Dict[str, Sequence[torch.Tensor]]] = None
+                ) -> Tuple[torch.Tensor, torch.Tensor, np.ndarray]:
         """Move the optimizer onto new parameter tensors (same sub-models, new row counts).  Allocates new, ZEROED
         moment arenas for the new layout and returns the OLD ``(exp_avg, exp_avg_sq, offsets)`` so that the caller
         (refine.py) can carry the surviving rows' moments over; step counts are kept (the reference moves
-        ``param_state`` -- including ``step`` -- to the new parameter)."""
+        ``param_state`` -- including ``step`` -- to the new parameter).  ``rows``: the row groups' new tensors, name -> one per
+        sub-model (None: unchanged).  A row-group tensor that is still the same storage keeps its moments; a new one starts at
+        zero here and the caller carries its rows (semantic.refine_carry)."""
         assert len(params) == self.num_segments
         old = (self.exp_avg, self.exp_avg_sq, self.offsets.copy())
-        self._install(params)
+        before = {i: (t.data_ptr(), t.numel()) for name, i0 in self.row_index.items() for i, t in
+                  enumerate(self._params[i0:i0 + self.num_segments], i0)}
+        self._install(params, rows)
         self.exp_avg, self.exp_avg_sq = self._new_moments(), self._new_moments()
-        for i in self.extra_index.values():  # the extra tensors do not change in a refinement: their moments move along
+        same = [i for i in self.extra_index.values()]  # the extra tensors do not change in a refinement: their moments move along
+        same += [i for i, key in before.items() if key == (self._params[i].data_ptr(), self._params[i].numel())]
+        for i in same:
             a, b, n = int(old[2][i]), int(self.offsets[i]), int(self.sizes[i])
             self.exp_avg[b:b + n].copy_(old[0][a:a + n])
             self.exp_avg_sq[b:b + n].copy_(old[1][a:a + n])
         return old
 
-    def rebuild_pointers(self, params: Sequence[Sequence[torch.Tensor]]) -> None:
+    def rebuild_pointers(self, params: Sequence[Sequence[torch.Tensor]], rows: Optional[Dict[str, Sequence[torch.Tensor]]] = None) -> None:
         """The layout is unchanged but the tensors were re-wrapped (``nn.Parameter(t)`` shares storage): refresh the
-        pointer column and the keep-alive list."""
+        pointer column and the keep-alive list (and the row groups' tensors, when given)."""
         flat = [t for ps in params for t in ps]
         n = len(flat)
         assert [t.numel() for t in flat] == [int(x) for x in self.table["numel"][:n]]
         self.table["param"][:n] = [t.data_ptr() for t in flat]
         self._params = flat + self._params[n:]
+        for name, ts in (rows or {}).items():
+            i0 = self.row_index[name]
+            assert [t.numel() for t in ts] == [int(x) for x in self.table["numel"][i0:i0 + len(ts)]]
+            self.table["param"][i0:i0 + len(ts)] = [t.data_ptr() for t in ts]
+            self._params[i0:i0 + len(ts)] = list(ts)
+            self._rows[name] = (list(ts), self._rows[name][1])

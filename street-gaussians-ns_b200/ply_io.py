@@ -8,10 +8,13 @@ with ``f_dc`` = features_dc[:, 0, :] (the first Fourier coefficient only: ``shs_
 ``f_rest`` = features_rest transposed to channel-major ("to match the sh order in Inria version", exporter.py:78-81),
 opacity as logit, scales as log, rotation un-normalised wxyz; rows with any non-finite attribute are dropped
 (exporter.py:103-116).  plyfile is not needed: the binary little-endian PLY it would write is produced directly.
+
+A sub-model with semantic logits [n, C] (``SceneGraphConfig.semantic_classes``) appends ``semantic_0..C-1`` after ``rot_3``;
+``read_semantic`` reads them back.  Files without semantics are byte for byte what they were before.
 """
 from __future__ import annotations
 
-from typing import Dict, List, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -19,13 +22,14 @@ import torch
 from .scene import GaussianSet
 
 
-def property_names(n_rest: int) -> List[str]:
+def property_names(n_rest: int, n_semantic: int = 0) -> List[str]:
     return (["x", "y", "z", "nx", "ny", "nz"] + [f"f_dc_{i}" for i in range(3)] + [f"f_rest_{i}" for i in range(n_rest)]
-            + ["opacity"] + [f"scale_{i}" for i in range(3)] + [f"rot_{i}" for i in range(4)])
+            + ["opacity"] + [f"scale_{i}" for i in range(3)] + [f"rot_{i}" for i in range(4)]
+            + [f"semantic_{i}" for i in range(n_semantic)])
 
 
-def to_columns(params: GaussianSet) -> Tuple[List[str], np.ndarray]:
-    """[n, n_props] float32 table in the exporter's column order, finite rows only."""
+def to_columns(params: GaussianSet, semantic: Optional[torch.Tensor] = None) -> Tuple[List[str], np.ndarray]:
+    """[n, n_props] float32 table in the exporter's column order (+ the semantic logits [n, C], when given), finite rows only."""
     with torch.no_grad():
         means = params.means.detach().cpu().numpy().astype(np.float32)
         n = means.shape[0]
@@ -33,14 +37,17 @@ def to_columns(params: GaussianSet) -> Tuple[List[str], np.ndarray]:
         rest = params.features_rest.detach().transpose(1, 2).contiguous().cpu().numpy().reshape(n, -1)
         cols = [means, np.zeros_like(means), dc, rest, params.opacities.detach().cpu().numpy().reshape(n, 1),
                 params.scales.detach().cpu().numpy(), params.quats.detach().cpu().numpy()]
+        if semantic is not None:
+            cols.append(semantic.detach().cpu().numpy().reshape(n, -1))
     table = np.concatenate([c.astype(np.float32).reshape(n, -1) for c in cols], axis=1)
     table = table[np.isfinite(table).all(axis=1)]
-    return property_names(rest.shape[1]), table
+    return property_names(rest.shape[1], 0 if semantic is None else cols[-1].shape[1]), table
 
 
-def write_ply(path, params: GaussianSet) -> int:
-    """Writes ``point_cloud_<name>.ply`` for one sub-model; returns the number of exported Gaussians."""
-    names, table = to_columns(params)
+def write_ply(path, params: GaussianSet, semantic: Optional[torch.Tensor] = None) -> int:
+    """Writes ``point_cloud_<name>.ply`` for one sub-model; returns the number of exported Gaussians.  ``semantic``: the
+    sub-model's semantic logits [n, C], written as ``semantic_0..C-1`` after ``rot_3`` (None: no such columns)."""
+    names, table = to_columns(params, semantic)
     header = "ply\nformat binary_little_endian 1.0\nelement vertex %d\n" % table.shape[0]
     header += "".join(f"property float {k}\n" for k in names) + "end_header\n"
     with open(path, "wb") as f:
@@ -104,8 +111,19 @@ def read_ply(path, device="cpu") -> GaussianSet:
                        stack([f"f_dc_{i}" for i in range(3)]).reshape(n, 1, 3), rest, stack(["opacity"])).to(device)
 
 
+def read_semantic(path, device="cpu") -> Optional[torch.Tensor]:
+    """The ``semantic_0..C-1`` columns of a ``write_ply`` file as float32 [n, C], or None when the file has none."""
+    c = read_ply_columns(path)
+    C = sum(1 for k in c if k.startswith("semantic_"))
+    if C == 0:
+        return None
+    return torch.from_numpy(np.stack([c[f"semantic_{i}"].astype(np.float32) for i in range(C)], axis=1)).to(device)
+
+
 def export_model(model, output_dir) -> Dict[str, int]:
-    """exporter.py:131-137: one ``point_cloud_<sub-model>.ply`` per entry of ``all_models``."""
+    """exporter.py:131-137: one ``point_cloud_<sub-model>.ply`` per entry of ``all_models`` (with its semantic logits, when
+    the model has them)."""
     import os
     os.makedirs(output_dir, exist_ok=True)
-    return {k: write_ply(os.path.join(output_dir, f"point_cloud_{k}.ply"), sub.as_set()) for k, sub in model.all_models.items()}
+    return {k: write_ply(os.path.join(output_dir, f"point_cloud_{k}.ply"), sub.as_set(), getattr(sub, "semantic_logits", None))
+            for k, sub in model.all_models.items()}

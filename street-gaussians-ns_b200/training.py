@@ -39,10 +39,13 @@ class TrainStep:
         ``gradient_accumulation_steps``: name of one of the optimizer's extra tensors -> n, nerfstudio's trainer rule (the
         reference sets ``{"camera_opt": 100}``, sgn_config.py:30): the tensor's gradient is zeroed at the steps where
         ``step % n == 0``, summed over the steps in between, and the tensor is stepped where ``step % n == n - 1``.  None (or a
-        tensor not named): every step."""
+        tensor not named): every step.  A per-row group of the optimizer (``FusedAdam(rows=...)``; the reference sets
+        ``{"semantic": 10}``) follows the same rule per sub-model: a sub-model whose gradient is None at the due step is skipped,
+        and one that a refinement rebuilt in the middle of a cycle starts over from a zero gradient -- the refinement replaces
+        the Parameter, as nerfstudio's does, and the accumulated gradient goes with the old one."""
         self.model, self.optimizer, self.group = model, optimizer, group
         self.accumulate = dict(gradient_accumulation_steps or {})
-        unknown = sorted(set(self.accumulate) - set(optimizer.extra_tensors()))
+        unknown = sorted(set(self.accumulate) - set(optimizer.extra_tensors()) - set(optimizer.row_tensors()))
         if unknown or any(int(n) < 1 for n in self.accumulate.values()):
             raise ValueError(f"gradient_accumulation_steps names tensors the optimizer does not step ({unknown}) or a count < 1: "
                              f"{self.accumulate}")
@@ -86,11 +89,16 @@ class TrainStep:
             # refused before anything is rendered or exchanged: the gradient exchange covers the arena only
             raise NotImplementedError(f"data-parallel training does not exchange the gradients of {sorted(extras)}: the "
                                       "replicas would diverge")
+        if world > 1 and (m.config.semantic_classes > 0 or opt.row_tensors()):
+            raise NotImplementedError("data-parallel training does not exchange the gradients of the semantic logits: the "
+                                      "replicas would diverge")
         if world > 1:
             self._ensure_exchange()
         m.step = step                                     # step_cb (sgn_splatfacto.py:754-755)
         # accumulated tensors keep their gradient except where their cycle starts; they step where it ends
-        keep = {id(extras[k]) for k, n in self.accumulate.items() if step % n != 0}
+        keep = {id(extras[k]) for k, n in self.accumulate.items() if step % n != 0 and k in extras}
+        rows = opt.row_tensors()
+        keep |= {id(t) for k, n in self.accumulate.items() if step % n != 0 and k in rows for t in rows[k]}
         for p in m.parameters():                          # Optimizers.zero_grad_all()
             if id(p) not in keep:
                 p.grad = None
@@ -126,13 +134,18 @@ class TrainStep:
                 # a loss term of a further tensor (the camera regulariser) may still have left a gradient: that tensor steps
                 # on its own step count, as nerfstudio steps a group whatever was rendered
                 due = self._due_extra_grads(step, extras)
-                if due:
-                    opt.step(next(iter(due.values())), present=[], full_layout=True, extra_grads=due)
+                due_rows = self._due_row_grads(step)
+                base = next(iter(due.values()), None)
+                if base is None and due_rows:
+                    base = next(g for gs in due_rows.values() for g in gs if g is not None)
+                if base is not None:
+                    opt.step(base, present=[], full_layout=True, extra_grads=due or None, row_grads=due_rows or None)
                 self._maybe_refine(step)
                 return losses
             arena = m.zero_gradient_arena()
         # the further tensors of the optimizer (the sky cube map, sky.CubeMapSky.base) step with the gradient autograd left
         extra_grads = self._due_extra_grads(step, extras)
+        row_grads = self._due_row_grads(step)             # the per-row groups (the semantic logits), per sub-model
         if world > 1:
             present = sorted(set(i for cam in all_cameras for i in self.submodels_in_view(cam)))
         else:
@@ -145,7 +158,11 @@ class TrainStep:
         else:
             if world > 1:
                 dp.allreduce_gradients(arena, average=True, group=self.group)
-            opt.step(arena, present=None if everything else present, full_layout=full, extra_grads=extra_grads or None)
+            if row_grads:
+                opt.step(arena, present=None if everything else present, full_layout=full, extra_grads=extra_grads or None,
+                         row_grads=row_grads)
+            else:
+                opt.step(arena, present=None if everything else present, full_layout=full, extra_grads=extra_grads or None)
         if rendered:
             m.after_train(step)                           # AFTER_TRAIN_ITERATION callbacks, in the reference's order
         self._maybe_refine(step)
@@ -156,6 +173,19 @@ class TrainStep:
         the end of its cycle (``step % n == n - 1``)."""
         return {name: t.grad for name, t in extras.items()
                 if t.grad is not None and (name not in self.accumulate or step % self.accumulate[name] == self.accumulate[name] - 1)}
+
+    def _due_row_grads(self, step: int) -> Dict[str, List[Optional[torch.Tensor]]]:
+        """The per-row groups that step at ``step`` (every step, or at the end of their accumulation cycle): name -> the
+        sub-models' gradients (None = skipped); groups without any gradient are left out."""
+        out = {}
+        for name, ts in self.optimizer.row_tensors().items():
+            n = self.accumulate.get(name)
+            if n is not None and step % n != n - 1:
+                continue
+            gs = [t.grad for t in ts]
+            if any(g is not None for g in gs):
+                out[name] = gs
+        return out
 
     def _ensure_exchange(self) -> None:
         """(Re)allocates the symmetric gradient arena when the model's layout changed (first step, after a refinement).

@@ -26,7 +26,8 @@ sys.path.insert(0, ROOT)
 def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int = 100, start_step: int = 600,
         actor_range: float = 45.0, pipeline_chunks: int = 0, overlap: bool = False, resident_table: bool = True,
         async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True, sky: bool = False, metrics: bool = False,
-        bbox_opt: bool = False, camera_opt: bool = False, sky_view_grad: bool = False, lidar_depth: float = 0.0) -> dict:
+        bbox_opt: bool = False, camera_opt: bool = False, sky_view_grad: bool = False, lidar_depth: float = 0.0,
+        semantic: float = 0.0) -> dict:
     """One measurement.  torch.distributed must already be initialised when WORLD_SIZE > 1.  Returns the result dict on
     rank 0 (None elsewhere).  ``sky``: the reference's default learnable sky (use_sky_sphere, a 1024^2 cube map stepped by
     the same Adam launch at the ``sky_sphere`` group's lr 0.005, sgn_config.py:72-75).  ``metrics``: every step also computes
@@ -38,6 +39,10 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     ``camera_opt``): the sky also gives the camera rotation its gradient (CubeMapSky(view_grad=True)).  ``lidar_depth`` > 0: the
     lidar depth term at that weight (SceneGraphConfig.depth_loss_mult), against a synthetic sweep per step
     (``synthetic.street_points(170_000, seed=step)``, about one top-lidar sweep, all drawn onto the device before the first step)
+    ``semantic`` > 0: per-Gaussian semantic logits with 3 classes (the reference's SemanticType) and the cross-entropy term at
+    that weight (SceneGraphConfig.semantic_loss_mult), against synthetic labels drawn onto the device before timing; the logits
+    are the FusedAdam row group "semantic" at features_dc's lr 0.0025 (a choice: the reference config names no rate) with
+    the reference's gradient accumulation of 10
     projected with the step's camera."""
     import torch
     import torch.distributed as dist
@@ -67,7 +72,8 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     rs = RefineSettings(refine_every=refine_every)
     cfg = SceneGraphConfig(use_sky_sphere=sky, ssim_lambda=ssim_lambda, fused_loss=fused_loss, full_gradient_arena=world > 1, refine=rs, async_binning=async_binning,
                            object_refine=RefineSettings(refine_every=refine_every, cull_alpha_thresh=0.005),
-                           num_train_data=len(cams), refine_record=True, depth_loss_mult=lidar_depth)
+                           num_train_data=len(cams), refine_record=True, depth_loss_mult=lidar_depth,
+                           semantic_classes=3 if semantic > 0 else 0, semantic_loss_mult=semantic)
     env_map = None
     if sky:
         from street_gaussians_ns_b200.sky import CubeMapSky
@@ -93,7 +99,11 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     if camera_opt:
         extra["camera_opt.pose_adjustment"] = (cam_opt.pose_adjustment, 1e-3)
         accumulate = {"camera_opt.pose_adjustment": 100}
-    opt = FusedAdam(model.optimizer_params(), extra=extra, reserve_spare=True)  # no cudaMalloc of moment arenas inside the training loop
+    rows = None
+    if semantic > 0:
+        rows = {"semantic": (model.semantic_params(), 0.0025)}
+        accumulate = dict(accumulate or {}, semantic=10)
+    opt = FusedAdam(model.optimizer_params(), extra=extra, reserve_spare=True, rows=rows)  # no cudaMalloc of moment arenas inside the training loop
     step_fn = TrainStep(model, opt, refine_every=refine_every, pipeline_chunks=pipeline_chunks, overlap=overlap, metrics=metrics,
                         gradient_accumulation_steps=accumulate)
     g = torch.Generator().manual_seed(5)
@@ -135,6 +145,13 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
 
     # one sweep per step, drawn before the timed steps as a data loader would have prefetched them
     sweeps = [syn.street_points(170_000, seed=start_step + i).to(dev) for i in range(warmup + steps)] if lidar_depth > 0 else []
+    # synthetic segmentations (classes 0..2 and 5 % ignored pixels), drawn before the timed steps
+    gl = torch.Generator().manual_seed(6)
+    labels = []
+    for _ in range(4 if semantic > 0 else 0):
+        lab = torch.randint(0, 3, (H, W, 1), generator=gl)
+        lab[torch.rand(H, W, 1, generator=gl) < 0.05] = 255
+        labels.append(lab.to(dev))
 
     def one(i):
         step = start_step + i
@@ -144,6 +161,8 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         batch = {"image": gt}
         if lidar_depth > 0:
             batch["lidar_points"] = sweeps[i % len(sweeps)]
+        if semantic > 0:
+            batch["semantic"] = labels[i % len(labels)]
         return step_fn(step, mine[rank], batch, all_cameras=mine if world > 1 else None)
 
     def sync():
@@ -212,6 +231,8 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                    **({"camera_opt": "CameraPoseOptimizer(SO3xR3), Adam lr 1e-3, gradient accumulation 100"} if camera_opt else {}),
                    **({"sky_view_grad": "the sky's rotation cotangent reaches the camera"} if sky_view_grad else {}),
                    **({"lidar_depth": f"depth_loss_mult {lidar_depth}, street_points(170_000, seed=step) per step"} if lidar_depth > 0 else {}),
+                   **({"semantic": f"3 classes, semantic_loss_mult {semantic}, Adam lr 0.0025, gradient accumulation 10, synthetic labels"}
+                      if semantic > 0 else {}),
                    "loss": "fused kernels" if fused_loss else "torch ops", "metrics": "get_metrics_dict every step" if metrics else "none",
                    "start_step": start_step, "refine_every": refine_every,
                    "refinement_kernels_loaded_before_timing": refine_warm,
@@ -247,6 +268,8 @@ def main():
     ap.add_argument("--sky-view-grad", action="store_true", help="with --sky --camera-opt: the sky also trains the camera rotation")
     ap.add_argument("--lidar-depth", type=float, default=0.0, metavar="W",
                     help="> 0: the lidar depth term at weight W against a synthetic 170 k-point sweep per step")
+    ap.add_argument("--semantic", type=float, default=0.0, metavar="W",
+                    help="> 0: 3-class semantic logits and the cross-entropy term at weight W against synthetic labels")
     args = ap.parse_args()
     if args.sky_view_grad and not (args.sky and args.camera_opt):
         ap.error("--sky-view-grad needs --sky and --camera-opt")
@@ -262,7 +285,7 @@ def main():
     res = run(args.steps, args.warmup, args.scale, args.refine_every, args.start_step, args.actor_range, args.pipeline_chunks,
               args.overlap, not args.host_table, ssim_lambda=args.ssim_lambda, fused_loss=not args.torch_loss, sky=args.sky,
               metrics=args.metrics, bbox_opt=args.bbox_opt, camera_opt=args.camera_opt,
-              sky_view_grad=args.sky_view_grad, lidar_depth=args.lidar_depth)
+              sky_view_grad=args.sky_view_grad, lidar_depth=args.lidar_depth, semantic=args.semantic)
     if res is not None:
         print(json.dumps(res))
     if world > 1:
