@@ -3,9 +3,9 @@
 // gives every Gaussian a vector of class logits, alpha-blends them into a semantic map (sgn_blend_extra_fwd) and supervises it
 // with cross-entropy; the reference's loader carries the segmentation as batch["semantic"] (data/sgn_dataset.py:125).
 //
-// Loss: per valid pixel (0 <= label < C and mask != 0) CE = logsumexp(S) - S[label], in fp32 with the max subtracted; per-block
-// partials summed in fp64 (the pixel counts as int64), then added in a fixed order by a one-block finish kernel, as depth.cu:
-// the same bits every run.  The valid-pixel count stays on the device.
+// Loss: per valid pixel (0 <= label < C and mask != 0) CE = logsumexp(S) - S[label], in fp32 as (max - S[label]) + log1p of the
+// other classes' sum of exp(S - max); per-block partials summed in fp64 (the pixel counts as int64), then added in a fixed order
+// by a one-block finish kernel, as depth.cu: the same bits every run.  The valid-pixel count stays on the device.
 //
 // Metrics: one pass that counts (label, argmax) pairs in a per-block shared histogram, flushed with integer atomics (the
 // counts do not depend on the order of the adds).
@@ -72,10 +72,16 @@ __global__ void __launch_bounds__(SEM_THREADS) semantic_loss_fwd_kernel(const Se
         const int l = sem_label(p, i);
         if (l < 0) continue;
         const float* x = p.logits + i * p.C;
-        float m, z;
-        sem_softmax_stats(x, p.C, m, z);
-        const float lse = m + logf(z);
-        s += (double)(lse - x[l]);
+        float m = x[0];  // the max and the first class that attains it
+        int a = 0;
+        for (int c = 1; c < p.C; ++c)
+            if (x[c] > m) { m = x[c]; a = c; }
+        float z1 = 0.f;  // sum of exp(S - max) over the other classes: the max's own term is exactly 1
+        for (int c = 0; c < p.C; ++c)
+            if (c != a) z1 += expf(x[c] - m);
+        // (max - S[label]) + log(1 + z1): a confident pixel's CE is the small z1, not a difference of two large numbers
+        // (max + log z rounds log z away once max is large) and not log of a sum that rounded its small terms into 1
+        s += (double)((m - x[l]) + log1pf(z1));
         ++n;
     }
     const double a = sem_block_sum(s, s_red);
@@ -122,7 +128,7 @@ __global__ void __launch_bounds__(SEM_THREADS) semantic_loss_bwd_kernel(const Se
     }
 }
 
-// confusion[label * C + argmax] += 1 over the valid pixels; ties go to the lowest class index
+// confusion[label * C + argmax] += 1 over the valid pixels; ties go to the lowest class index, a NaN logit beats every number
 __global__ void __launch_bounds__(SEM_THREADS) semantic_confusion_kernel(const SemParams p, unsigned long long* __restrict__ confusion) {
     __shared__ unsigned s_hist[SEM_MAX_C * SEM_MAX_C];
     const int CC = p.C * p.C;
@@ -135,7 +141,7 @@ __global__ void __launch_bounds__(SEM_THREADS) semantic_confusion_kernel(const S
         int a = 0;
         float best = x[0];
         for (int c = 1; c < p.C; ++c)
-            if (x[c] > best) { best = x[c]; a = c; }
+            if (x[c] > best || (x[c] != x[c] && best == best)) { best = x[c]; a = c; }  // the first NaN wins, as torch.argmax
         atomicAdd(s_hist + l * p.C + a, 1u);
     }
     __syncthreads();

@@ -104,7 +104,7 @@ def semantic_loss_torch(logits: torch.Tensor, labels: torch.Tensor, mask: Option
 
 def semantic_confusion(logits: torch.Tensor, labels: torch.Tensor, mask: Optional[torch.Tensor] = None) -> torch.Tensor:
     """int64 [C, C] device tensor: entry (label, argmax logits) counts the valid pixels with that pair (ties to the lowest
-    class).  One launch; nothing is read back."""
+    class; the first NaN logit wins, as in torch.argmax).  One launch; nothing is read back."""
     s, H, W, Cn = _logits(logits)
     dev = s.device
     lab = _labels(labels, H, W, dev)

@@ -3,7 +3,17 @@ cotangent, the confusion matrix of eval with the metrics derived from it, and th
 
 Valid pixel: 0 <= label < C and (no mask or mask != 0).  loss = w * sum_valid (logsumexp(S[p]) - S[p, label]) / n_valid, 0 when
 n_valid = 0; v = g * w / n_valid * (softmax(S[p]) - onehot(label)) on the valid pixels, 0 elsewhere.  Argmax ties go to the
-lowest class.  The carry: output rows [survivors | split samples, sample-major | duplicates], each a copy of its source row;
+lowest class.
+
+Labels are int64 and compared whole: -1, C, 255, 2**31 or -2**40 are ignored like any label outside [0, C).  A mask of -0.0
+removes the pixel (-0.0 == 0); a fractional mask keeps it with weight 1.  Non-finite logits, per valid pixel:
+  * a -inf among finite logits contributes exp(-inf) = 0: its softmax entry is 0 and, when it holds the label, CE = +inf and the
+    label's cotangent is exactly -g w / n_valid;
+  * every logit -inf (logsumexp of -inf minus -inf) or any NaN: CE = NaN, so the loss is NaN, and the pixel's whole cotangent
+    row is NaN;
+  * the arg-max of the confusion matrix takes the first NaN when there is one (NaN beats every number, as torch.argmax and
+    np.argmax), else the first maximum, so a pixel whose logits are all -inf counts as class 0.
+The carry: output rows [survivors | split samples, sample-major | duplicates], each a copy of its source row;
 survivors keep their moments, new rows start at zero (what the refinement does to features_dc)."""
 from __future__ import annotations
 
@@ -31,9 +41,16 @@ def loss_ref64(logits: np.ndarray, labels: np.ndarray, mask: Optional[np.ndarray
     if n == 0:
         return 0.0, 0
     s, lab = S[ok], np.asarray(labels).reshape(-1)[ok].astype(np.int64)
-    m = s.max(axis=1, keepdims=True)
-    lse = m[:, 0] + np.log(np.exp(s - m).sum(axis=1))
-    return float(weight * (lse - s[np.arange(n), lab]).sum() / n), n
+    return float(weight * ce_ref64(s, lab).sum() / n), n
+
+
+def ce_ref64(s: np.ndarray, lab: np.ndarray) -> np.ndarray:
+    """Per-pixel CE float64 [n] of logits ``s`` [n, C] against in-range labels ``lab`` [n] (NaN and inf as the module states)."""
+    s = np.asarray(s, np.float64)
+    with np.errstate(invalid="ignore", over="ignore"):
+        m = s.max(axis=1, keepdims=True)
+        lse = m[:, 0] + np.log(np.exp(s - m).sum(axis=1))
+        return lse - s[np.arange(s.shape[0]), lab]
 
 
 def grad_ref64(logits: np.ndarray, labels: np.ndarray, mask: Optional[np.ndarray] = None, weight: float = 1.0,
@@ -46,8 +63,9 @@ def grad_ref64(logits: np.ndarray, labels: np.ndarray, mask: Optional[np.ndarray
     n = int(ok.sum())
     if n:
         s = S[ok]
-        e = np.exp(s - s.max(axis=1, keepdims=True))
-        p = e / e.sum(axis=1, keepdims=True)
+        with np.errstate(invalid="ignore"):
+            e = np.exp(s - s.max(axis=1, keepdims=True))
+            p = e / e.sum(axis=1, keepdims=True)
         p[np.arange(n), np.asarray(labels).reshape(-1)[ok].astype(np.int64)] -= 1.0
         v[ok] = grad_loss * weight / n * p
     return v.reshape(logits.shape)

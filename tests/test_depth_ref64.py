@@ -126,3 +126,49 @@ def test_metrics():
     assert m[3] == pytest.approx(np.sqrt(np.mean(np.log(d / t) ** 2)))
     assert list(m[4:7]) == [1 / 5, 3 / 5, 4 / 5]  # ratios 1, 1.25 (not < 1.25), 1e4, 1.3, 1.8
     assert r[1] == 1.25
+
+
+def test_non_finite_and_edge_rules():
+    """The rules oracle/depth_ref64.py states for targets, masks and depths that are not ordinary numbers."""
+    D = np.array([3.0, 3.0, 3.0, 3.0, 3.0, 3.0, 3.0, 7.5], np.float32)
+    T = np.array([-2.0, -0.0, np.nan, 2.0, 2.0, 2.0, 2.0, 7.5], np.float32)
+    M = np.array([1.0, 1.0, 1.0, -0.0, 0.25, np.nan, 1.0, 1.0], np.float32)
+    ok = [False, False, False, False, True, True, True, True]
+    from oracle.depth_ref64 import valid_ref64
+    assert valid_ref64(T, M).tolist() == ok
+    L, n = depth_loss_ref64(D, T, M, weight=2.0)
+    assert n == 4 and L == pytest.approx(2.0 * 3 / 4)
+    g = depth_loss_grad_ref64(D, T, M, weight=2.0, g=1.0)
+    assert g.tolist() == [0, 0, 0, 0, 0.5, 0.5, 0.5, 0.0]  # D == T: sign 0
+    Dn = D.copy()
+    Dn[4] = np.nan  # a NaN depth: the loss is NaN, its cotangent 0
+    assert np.isnan(depth_loss_ref64(Dn, T, M)[0])
+    gn = depth_loss_grad_ref64(Dn, T, M)
+    assert gn[4] == 0.0 and np.isfinite(gn).all()
+    # the metrics take fmax(D, 1e-3): a NaN depth counts as 1e-3
+    assert np.array_equal(depth_metrics_ref64(Dn, T, M), depth_metrics_ref64(np.where(np.isnan(Dn), np.float32(1e-3), Dn), T, M))
+
+
+def test_metric_thresholds_are_exclusive():
+    T = np.array([4.0, 5.0, 16.0, 25.0, 64.0, 125.0], np.float32)
+    D = np.array([5.0, 4.0, 25.0, 16.0, 125.0, 64.0], np.float32)  # r = 1.25, 1.25, 1.5625, 1.5625, 1.953125, 1.953125
+    m = depth_metrics_ref64(D, T)
+    assert list(m[4:8]) == [0.0, 2 / 6, 4 / 6, 6.0]
+    below = np.nextafter(D, np.float32(0)).astype(np.float32)
+    below[1::2] = D[1::2]
+    assert list(depth_metrics_ref64(below, T)[4:7] * 6) == [1.0, 3.0, 5.0]
+
+
+def test_map_clip_and_overflow_rules():
+    m, pix = dmap([[0, 0, CLIP], [0, 0, np.nextafter(np.float32(CLIP), np.float32(1))]])
+    assert pix[0] == -1 and pix[1] == 3 * W + 4
+    zero, pix = lidar_depth_map_ref64(np.array([[0, 0, 0.0], [0, 0, -0.0]]), EYE, F, F, CX, CY, W, H, 0.0)
+    assert (pix == -1).all() and not zero.any()
+    # NaN and infinite coordinates drop the point
+    _, pix = dmap([[np.nan, 0, 3.0], [0, 0, np.nan], [np.inf, 0, 3.0], [0, 0, np.inf], [0, 0, -np.inf]])
+    assert (pix == -1).all()
+    # a depth that overflows float32 (6e38) is no return, like the map's +inf empty marker
+    A = EYE.copy()
+    A[2, 2] = 2.0
+    m, pix = dmap([[0, 0, 3e38], [1.0, 0.5, 3.0]], A)
+    assert pix[0] == -1 and m[3, 4] == 0.0 and m[3, 5] == 6.0

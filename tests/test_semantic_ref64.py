@@ -286,3 +286,27 @@ def test_model_refinement_carries_the_logits(host_backend, monkeypatch):
         sm, sv = opt.row_moment_views("semantic", i)
         assert torch.equal(sm[:, 0], m[:, 0, 0]) and torch.equal(sv[:, 0], v[:, 0, 0])
         assert opt.row_tensors()["semantic"][i] is sub.semantic_logits
+
+
+def test_label_mask_and_non_finite_rules():
+    """The rules tests/semantic_cases.py states: int64 labels outside [0, C) and a -0.0 mask leave the pixel out; -inf and
+    NaN logits give the stated loss, cotangent and arg-max."""
+    C = 4
+    lab = np.array([-1, C, 255, 2 ** 31, -2 ** 40, 2, 1], np.int64)
+    mask = np.array([1, 1, 1, 1, 1, -0.0, 0.5], np.float32)
+    assert ref.valid_ref(lab, C, mask).tolist() == [False] * 6 + [True]
+    x = np.zeros((1, 5, C))
+    x[0, 0, 0] = -np.inf                 # off the label (1): a zero softmax entry
+    x[0, 1, 1] = -np.inf                 # on the label: CE = +inf, cotangent -1 there
+    x[0, 2, :] = -np.inf                 # all -inf: NaN
+    x[0, 3, 2] = np.nan                  # NaN: NaN
+    labels = np.array([[1, 1, 1, 1, 1]])
+    ce = ref.ce_ref64(x.reshape(-1, C), labels.reshape(-1))
+    assert ce[0] == pytest.approx(np.log(3.0)) and ce[1] == np.inf and np.isnan(ce[2]) and np.isnan(ce[3])
+    assert ce[4] == pytest.approx(np.log(4.0))
+    v = ref.grad_ref64(x[:, :2], labels[:, :2])
+    assert v[0, 0, 0] == 0.0 and v[0, 1, 1] == -0.5  # g w / n_valid = 1 / 2
+    for bad in (x[:, 2:3], x[:, 3:4]):
+        assert np.isnan(ref.loss_ref64(bad, labels[:, :1])[0]) and np.isnan(ref.grad_ref64(bad, labels[:, :1])).all()
+    conf = ref.confusion_ref64(x, labels)
+    assert conf[1].tolist() == [3, 1, 1, 0]  # argmax: 1, 0, 0 (all -inf), 2 (the NaN), 0 (all tie)
