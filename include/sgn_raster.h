@@ -45,10 +45,12 @@ typedef enum sgn_status {
  *   [0] x  [1] y            pixel centre            == gsplat project_gaussians `xys`
  *   [2] a  [3] b  [4] c     conic (inverse cov2d)   == `conics`
  *   [5] opacity             sigmoid(logit)          (sgn_splatfacto.py:946-949)
+ *                           antialiased mode: sigmoid(logit) * comp
  *   [6] r  [7] g  [8] b     clamp(SH+0.5, min 0)    (sgn_splatfacto.py:939-940)
  *   [9] depth               view-space z            == `depths`
  *   [10] aux (int bits)     bits 0-2: colour clamp pass mask, bit 3: object class, bit 4: visible
- *   [11] unused
+ *   [11] comp               antialiased mode: sqrt(max(0, det(cov2d) / det(cov2d + 0.3 I))) of a visible row (cov2d before
+ *                           the blur), 0 otherwise; classic mode: 0
  * xys / conics / depths handed back to Python are strided views of this array. */
 
 /* One visible sub-model of the scene graph for one frame (sgn_splatfacto_scene_graph.py:332-360).
@@ -95,6 +97,9 @@ typedef struct sgn_camera {
     int32_t block_width;      /* config.block_width; binning semantics (tile AABB) */
     int32_t sh_degree;        /* coefficients stored */
     int32_t sh_degree_to_use; /* min(step//interval, sh_degree) train, sh_degree eval (:936-938) */
+    int32_t antialiased;      /* rasterize_mode (sgn_splatfacto.py:214-223): 0 "classic", 1 "antialiased" -- the record's
+                                 opacity is scaled by the blur compensation, forward and backward (gsplat's antialiased
+                                 mode; the reference leaves the multiply commented out, :946-949) */
 } sgn_camera;
 
 /* Blend settings. */
@@ -146,7 +151,11 @@ int sgn_upload(const void* host, size_t bytes, void* dev, void* stream);
  * xmin,ymin,xmax,ymax in tiles), tiles_touched[N] i32 = number of AABB tiles the Gaussian can really
  * reach (exact test, see sgn_bin_count), touch_mask[N] u32 = one bit per AABB tile when the AABB has at
  * most 32 tiles.  Work is split into 128-row chunks that never straddle segments:
- * num_chunks = sum over segments of ceil(count/128), sgn_segment.chunk0 = the segment's first chunk. */
+ * num_chunks = sum over segments of ceil(count/128), sgn_segment.chunk0 = the segment's first chunk.
+ * cam->antialiased: record [5] is sigmoid(logit) * comp and [11] is comp (layout above), and the touch test uses that
+ * opacity, tau = ln(255 o comp), so a row with comp == 0 reaches no tile.  The backward (every form below, with the same
+ * camera) then sends the opacity cotangent to the logit as v * comp * s (1 - s) and, through comp, to cov2d and from
+ * there to means, scales, quats and the pose / view partials. */
 int sgn_project_fwd(const sgn_segment* segs_dev, int nseg, int N, int num_chunks, const sgn_camera* cam,
                     float* records, int32_t* radii, int32_t* num_tiles_hit, uint16_t* tile_bbox,
                     int32_t* tiles_touched, uint32_t* touch_mask, void* stream);
@@ -226,6 +235,13 @@ int sgn_l1_project_fwd(int N, const float* means, const float* scales, float glo
 int sgn_l1_project_bwd(int N, const float* means, const float* scales, float glob_scale, const float* quats,
                        const sgn_camera* cam, const int32_t* radii, const float* v_xys, const float* v_depths,
                        const float* v_conics, float* v_means, float* v_scales, float* v_quats, void* stream);
+/* The same backward with a cotangent of `compensation` too (v_compensation may be NULL: then the outputs are
+ * sgn_l1_project_bwd's).  comp = sqrt(max(0, det(cov2d) / det(cov2d + 0.3 I))) reaches means, scales and quats through
+ * cov2d; a row whose comp is 0 (the clamp) passes no cotangent through it. */
+int sgn_l1_project_bwd_comp(int N, const float* means, const float* scales, float glob_scale, const float* quats,
+                            const sgn_camera* cam, const int32_t* radii, const float* v_xys, const float* v_depths,
+                            const float* v_conics, const float* v_compensation, float* v_means, float* v_scales,
+                            float* v_quats, void* stream);
 /* gsplat.spherical_harmonics(degrees_to_use, viewdirs[N,3], coeffs[N,K,3]) (call site :939): forward when
  * `colors` is non-NULL, backward (v_coeffs = Y_k * v_colors) when `v_coeffs` is non-NULL. */
 int sgn_l1_sh(int N, int K, int degree, const float* viewdirs, const float* coeffs, const float* v_colors,

@@ -45,6 +45,7 @@ class CameraStruct(C.Structure):
         ("clip_thresh", C.c_float),
         ("block_width", C.c_int32),
         ("sh_degree", C.c_int32), ("sh_degree_to_use", C.c_int32),
+        ("antialiased", C.c_int32),  # rasterize_mode: 0 classic (zero-initialised), 1 antialiased
     ]
 
 
@@ -124,7 +125,7 @@ _lib = None
 
 EXPORTS = [
     "sgn_last_error", "sgn_abi_version", "sgn_launch_count", "sgn_sizeof_segment", "sgn_sizeof_segment_grads", "sgn_sizeof_camera",
-    "sgn_upload", "sgn_bin_count", "sgn_project_fwd", "sgn_project_bwd", "sgn_l1_project_fwd", "sgn_l1_project_bwd", "sgn_l1_sh", "sgn_bin_scan_scratch_bytes", "sgn_bin_scan",
+    "sgn_upload", "sgn_bin_count", "sgn_project_fwd", "sgn_project_bwd", "sgn_l1_project_fwd", "sgn_l1_project_bwd", "sgn_l1_project_bwd_comp", "sgn_l1_sh", "sgn_bin_scan_scratch_bytes", "sgn_bin_scan",
     "sgn_bin_sort_scratch_bytes", "sgn_bin_sort", "sgn_bin_class_scratch_bytes", "sgn_bin_class_lists", "sgn_blend_sched_ints",
     "sgn_blend_fwd", "sgn_blend_bwd", "sgn_sizeof_adam_tensor", "sgn_adam_chunk_elems", "sgn_adam_step",
     "sgn_loss_scratch_bytes", "sgn_loss_fwd", "sgn_loss_bwd", "sgn_ssim_workspace_bytes", "sgn_ssim_fwd", "sgn_ssim_bwd",
@@ -191,8 +192,9 @@ def load():
     fl = C.c_float
     L.sgn_l1_project_fwd.argtypes = [i32, vp, vp, fl, vp, C.POINTER(CameraStruct), vp, vp, vp, vp, vp, vp, vp, vp]
     L.sgn_l1_project_bwd.argtypes = [i32, vp, vp, fl, vp, C.POINTER(CameraStruct), vp, vp, vp, vp, vp, vp, vp, vp]
+    L.sgn_l1_project_bwd_comp.argtypes = [i32, vp, vp, fl, vp, C.POINTER(CameraStruct), vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.sgn_l1_sh.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, vp]
-    for f in ("sgn_l1_project_fwd", "sgn_l1_project_bwd", "sgn_l1_sh"):
+    for f in ("sgn_l1_project_fwd", "sgn_l1_project_bwd", "sgn_l1_project_bwd_comp", "sgn_l1_sh"):
         getattr(L, f).restype = C.c_int
     L.sgn_bin_scan_scratch_bytes.argtypes = [i32]
     L.sgn_bin_scan_scratch_bytes.restype = sz

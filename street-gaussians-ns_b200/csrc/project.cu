@@ -128,10 +128,10 @@ project_fwd_direct_kernel(const sgn_segment* __restrict__ segs, int nseg, const 
         q[0] = qq.x; q[1] = qq.y; q[2] = qq.z; q[3] = qq.w;
     }
     SgnProj st;
-    vis = sgn_project_exact(sg, cam, m, ls, q, st);
+    vis = sgn_project_exact(sg, cam, m, ls, q, st, true, 1.f, cam.antialiased != 0);
 
     float rgb[3] = {0.f, 0.f, 0.f};
-    float opac = 0.f;
+    float opac = 0.f, comp = 0.f;
     int aux = 0;
     if (vis) {
         // colour: Fourier DC (scene graph :239-247), SH (sgn_splatfacto.py:933-940)
@@ -165,6 +165,10 @@ project_fwd_direct_kernel(const sgn_segment* __restrict__ segs, int nseg, const 
             for (int ch = 0; ch < 3; ++ch) { rgb[ch] = 1.f / (1.f + expf(-c0[ch])); aux |= (1 << ch); }
         }
         opac = 1.f / (1.f + expf(-__ldg(sg.opacities + i)));
+        if (cam.antialiased) {  // warp-uniform
+            comp = st.comp;
+            opac = opac * comp;
+        }
         aux |= SGN_AUX_VISIBLE;
     }
     if (sg.cls == 1) aux |= SGN_AUX_OBJECT;
@@ -172,7 +176,7 @@ project_fwd_direct_kernel(const sgn_segment* __restrict__ segs, int nseg, const 
     float4* rec = records + 3 * g;
     rec[0] = make_float4(st.xy[0], st.xy[1], st.conic[0], st.conic[1]);
     rec[1] = make_float4(st.conic[2], opac, rgb[0], rgb[1]);
-    rec[2] = make_float4(rgb[2], vis ? st.pv[2] : 0.f, __int_as_float(aux), 0.f);
+    rec[2] = make_float4(rgb[2], vis ? st.pv[2] : 0.f, __int_as_float(aux), comp);
     radii[g] = st.radius;
     num_tiles_hit[g] = vis ? (st.tmax[0] - st.tmin[0]) * (st.tmax[1] - st.tmin[1]) : 0;
     bb = make_ushort4((unsigned short)st.tmin[0], (unsigned short)st.tmin[1],
@@ -180,7 +184,8 @@ project_fwd_direct_kernel(const sgn_segment* __restrict__ segs, int nseg, const 
     tile_bbox[g] = bb;
     if (vis) tc = make_touch_ctx(make_float4(st.xy[0], st.xy[1], st.conic[0], st.conic[1]), make_float4(st.conic[2], opac, 0.f, 0.f));
     }  // active
-    // tiles the Gaussian can really reach (exact ellipse-vs-tile test, sgn_touch.cuh); binning lists only those
+    // tiles the Gaussian can really reach (exact ellipse-vs-tile test, sgn_touch.cuh) with the opacity the blend draws --
+    // compensated in the antialiased mode, where comp == 0 gives tau = -inf and no tile; binning lists only those
     uint32_t mask;
     const int nt = count_touched_tiles(vis, tc, bb, cam.width, cam.height, cam.block_width, mask);
     if (active) {
@@ -204,7 +209,7 @@ project_fwd_staged_kernel(const sgn_segment* __restrict__ segs, int nseg, const 
     __shared__ __align__(16) float s_dc[CH * MAX_DC];
     __shared__ __align__(16) float s_means[CH * 3];
     __shared__ __align__(16) float s_scales[CH * 3];
-    __shared__ float s_geo[CH][9];  // per visible row (compact index): xy, conic, depth, world mean
+    __shared__ float s_geo[CH][10];  // per visible row (compact index): xy, conic, depth, world mean, comp
     __shared__ int s_row[CH];       // compact index -> row of the chunk
     __shared__ int s_warp_base[CH / 32 + 1];
     for (int i = threadIdx.x; i < nseg; i += blockDim.x) s_chunk0[i] = segs[i].chunk0;
@@ -231,7 +236,7 @@ project_fwd_staged_kernel(const sgn_segment* __restrict__ segs, int nseg, const 
         const float ls[3] = {s_scales[3 * tid], s_scales[3 * tid + 1], s_scales[3 * tid + 2]};
         const float4 qq = __ldg(reinterpret_cast<const float4*>(sg.quats) + r0 + tid);
         const float q[4] = {qq.x, qq.y, qq.z, qq.w};
-        vis = sgn_project_exact(sg, cam, m, ls, q, st);
+        vis = sgn_project_exact(sg, cam, m, ls, q, st, true, 1.f, cam.antialiased != 0);
         radii[g] = st.radius;
         num_tiles_hit[g] = vis ? (st.tmax[0] - st.tmin[0]) * (st.tmax[1] - st.tmin[1]) : 0;
         tile_bbox[g] = make_ushort4((unsigned short)st.tmin[0], (unsigned short)st.tmin[1],
@@ -262,6 +267,7 @@ project_fwd_staged_kernel(const sgn_segment* __restrict__ segs, int nseg, const 
         float* ge = s_geo[c];
         ge[0] = st.xy[0]; ge[1] = st.xy[1]; ge[2] = st.conic[0]; ge[3] = st.conic[1]; ge[4] = st.conic[2];
         ge[5] = st.pv[2]; ge[6] = st.mw[0]; ge[7] = st.mw[1]; ge[8] = st.mw[2];
+        ge[9] = st.comp;
     }
     __syncthreads();
     if (nvis == 0) return;
@@ -338,10 +344,11 @@ project_fwd_staged_kernel(const sgn_segment* __restrict__ segs, int nseg, const 
 #pragma unroll
             for (int ch = 0; ch < 3; ++ch) { rgb[ch] = 1.f / (1.f + expf(-c0[ch])); aux |= (1 << ch); }
         }
-        const float opac = 1.f / (1.f + expf(-__ldg(sg.opacities + r0 + row)));
+        float opac = 1.f / (1.f + expf(-__ldg(sg.opacities + r0 + row)));
+        if (cam.antialiased) opac = opac * ge[9];  // warp-uniform
         float4* rec = records + 3 * gb;
         rec[1] = make_float4(ge[4], opac, rgb[0], rgb[1]);
-        rec[2] = make_float4(rgb[2], ge[5], __int_as_float(aux), 0.f);
+        rec[2] = make_float4(rgb[2], ge[5], __int_as_float(aux), ge[9]);
         bb = tile_bbox[gb];  // written by this block in phase A (visible to the block after the barriers above)
         tc = make_touch_ctx(make_float4(ge[0], ge[1], ge[2], ge[3]), make_float4(ge[4], opac, 0.f, 0.f));
     }
@@ -415,10 +422,14 @@ extern "C" int sgn_project_fwd(const sgn_segment* segs_dev, int nseg, int N, int
 // p_c = W p_w + c and covariance S_c = W S_w W^T: v_W = v_pc p_w^T + 2 G W S_w, v_c = v_pc, where v_pc (vpv below) is the
 // complete cotangent of p_c (xy, depth and the Jacobian's dependence on p_c) and G = J^T g J that of S_c; 2 G W S_w = J^T vT
 // since T = J W and vT = 2 g T S_w.
+// with_comp (a warp-uniform flag): also the cotangent v_comp of comp (the forward's sgn_compensation), through cov2d.  Its
+// un-blurred diagonal is rebuilt from st.T and st.S (the forward's bits), so that it does not stay live from the projection
+// to here.
 template <bool VIEW = false>
 __device__ __forceinline__ void sgn_project_vjp(const sgn_camera& cam, const SgnProj& st, const float v_xy[2], float v_depth,
                                                 const float v_conic[3], float vmw[3], float vs[3], float vqr[4],
-                                                float* vview = nullptr) {
+                                                float* vview = nullptr, bool with_comp = false, float comp = 0.f,
+                                                float v_comp = 0.f) {
     const float* W = cam.viewmat;
     const float fx = cam.fx, fy = cam.fy;
     float vpv[3];
@@ -438,6 +449,13 @@ __device__ __forceinline__ void sgn_project_vjp(const sgn_camera& cam, const Sgn
         vA = -(a00 * X0 + a01 * X1);
         vB = -(a00 * X1 + a01 * X2) - (a10 * X0 + a11 * X1);
         vC = -(a10 * X1 + a11 * X2);
+    }
+    if (with_comp) {
+        xf T[6], S[6], a, b, c, c00, c11;
+#pragma unroll
+        for (int k = 0; k < 6; ++k) { T[k] = xf(st.T[k]); S[k] = xf(st.S[k]); }
+        sgn_cov2d_blur(T, S, a, b, c, c00, c11);
+        sgn_compensation_vjp(c00.v, c11.v, a.v, b.v, c.v, comp, v_comp, vA, vB, vC);
     }
     const float g00 = vA, g01 = 0.5f * vB, g11 = vC;
     const float* T = st.T;
@@ -577,7 +595,7 @@ project_bwd_kernel(const sgn_segment* __restrict__ segs, const sgn_segment_grads
         const float v_depth = v2.y;
         const float4 r1 = records[3 * g + 1], r2 = records[3 * g + 2];
         const int aux = __float_as_int(r2.z);
-        {   // opacity: sigmoid backward
+        if (!cam.antialiased) {  // opacity: sigmoid backward (the antialiased mode's below)
             const float o = r1.y;
             gr.opacities[i] = v_opac * o * (1.f - o);
         }
@@ -623,9 +641,18 @@ project_bwd_kernel(const sgn_segment* __restrict__ segs, const sgn_segment_grads
                 for (int ch = 0; ch < 3; ++ch) gdc[f * 3 + ch] = w * vc[ch];
             }
         }
+        // antialiased mode: record [5] = s comp with s = sigmoid(logit) and comp in record [11]; v_comp = v_opac s goes on
+        // through cov2d (sgn_project_vjp)
+        float v_comp = 0.f, comp = 0.f;
+        if (cam.antialiased) {  // warp-uniform
+            const float s = 1.f / (1.f + expf(-__ldg(sg.opacities + i)));  // the forward's sigmoid, not record [5]
+            v_comp = v_opac * s;
+            gr.opacities[i] = v_opac * r2.w * s * (1.f - s);
+            comp = __ldg(reinterpret_cast<const float*>(records) + 12 * g + 11);  // read again here: nothing stays live
+        }
         if (vis && radii[g] > 0) {
             float vmw[3], vs[3], vqr[4];
-            sgn_project_vjp<VIEW>(cam, st, v_xy, v_depth, v_conic, vmw, vs, vqr, vv);
+            sgn_project_vjp<VIEW>(cam, st, v_xy, v_depth, v_conic, vmw, vs, vqr, vv, cam.antialiased != 0, comp, v_comp);
 #pragma unroll
             for (int c = 0; c < 3; ++c) gs[c] = vs[c] * st.s[c];  // through exp
             if (sg.has_pose) {
@@ -833,20 +860,14 @@ l1_project_fwd_kernel(int N, const float* __restrict__ means, const float* __res
     const float sc[3] = {scales[3 * g], scales[3 * g + 1], scales[3 * g + 2]};
     const float q[4] = {quats[4 * g], quats[4 * g + 1], quats[4 * g + 2], quats[4 * g + 3]};
     SgnProj st;
-    const bool vis = sgn_project_exact(sg, cam, m, sc, q, st, false, glob_scale);
+    const bool vis = sgn_project_exact(sg, cam, m, sc, q, st, false, glob_scale, true);
     const bool clipped = st.pv[2] <= cam.clip_thresh;
     xys[2 * g] = st.xy[0]; xys[2 * g + 1] = st.xy[1];
     depths[g] = vis ? st.pv[2] : 0.f;
     radii[g] = st.radius;
     conics[3 * g] = st.conic[0]; conics[3 * g + 1] = st.conic[1]; conics[3 * g + 2] = st.conic[2];
     num_tiles_hit[g] = vis ? (st.tmax[0] - st.tmin[0]) * (st.tmax[1] - st.tmin[1]) : 0;
-    float c = 0.f;
-    if (vis) {
-        const float det_orig = (st.a - 0.3f) * (st.c - 0.3f) - st.b * st.b;
-        const float det_blur = st.a * st.c - st.b * st.b;
-        c = sqrtf(fmaxf(0.f, det_orig / det_blur));
-    }
-    comp[g] = c;
+    comp[g] = vis ? st.comp : 0.f;
 #pragma unroll
     for (int k = 0; k < 6; ++k) cov3d[6 * g + k] = clipped ? 0.f : st.S[k];
 }
@@ -869,7 +890,8 @@ __global__ void __launch_bounds__(PROJ_THREADS)
 l1_project_bwd_kernel(int N, const float* __restrict__ means, const float* __restrict__ scales, float glob_scale,
                       const float* __restrict__ quats, const sgn_camera cam, const int32_t* __restrict__ radii,
                       const float* __restrict__ v_xys, const float* __restrict__ v_depths, const float* __restrict__ v_conics,
-                      float* __restrict__ v_means, float* __restrict__ v_scales, float* __restrict__ v_quats) {
+                      const float* __restrict__ v_comp, float* __restrict__ v_means, float* __restrict__ v_scales,
+                      float* __restrict__ v_quats) {
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= N) return;
     float gm[3] = {0.f, 0.f, 0.f}, gs[3] = {0.f, 0.f, 0.f}, gq[4] = {0.f, 0.f, 0.f, 0.f};
@@ -880,12 +902,14 @@ l1_project_bwd_kernel(int N, const float* __restrict__ means, const float* __res
         const float sc[3] = {scales[3 * g], scales[3 * g + 1], scales[3 * g + 2]};
         const float q[4] = {quats[4 * g], quats[4 * g + 1], quats[4 * g + 2], quats[4 * g + 3]};
         SgnProj st;
-        if (sgn_project_exact(sg, cam, m, sc, q, st, false, glob_scale)) {
+        if (sgn_project_exact(sg, cam, m, sc, q, st, false, glob_scale, v_comp != nullptr)) {
             const float vxy[2] = {v_xys ? v_xys[2 * g] : 0.f, v_xys ? v_xys[2 * g + 1] : 0.f};
             const float vc[3] = {v_conics ? v_conics[3 * g] : 0.f, v_conics ? v_conics[3 * g + 1] : 0.f,
                                  v_conics ? v_conics[3 * g + 2] : 0.f};
             float vs[3];
-            sgn_project_vjp(cam, st, vxy, v_depths ? v_depths[g] : 0.f, vc, gm, vs, gq);
+            const bool with_comp = v_comp != nullptr;  // uniform: a NULL cotangent is sgn_l1_project_bwd, unchanged
+            sgn_project_vjp(cam, st, vxy, v_depths ? v_depths[g] : 0.f, vc, gm, vs, gq, nullptr, with_comp, st.comp,
+                            with_comp ? v_comp[g] : 0.f);
 #pragma unroll
             for (int k = 0; k < 3; ++k) gs[k] = vs[k] * glob_scale;
         }
@@ -896,16 +920,33 @@ l1_project_bwd_kernel(int N, const float* __restrict__ means, const float* __res
     for (int k = 0; k < 4; ++k) v_quats[4 * g + k] = gq[k];
 }
 
+static int l1_project_bwd_launch(const char* what, int N, const float* means, const float* scales, float glob_scale,
+                                 const float* quats, const sgn_camera* cam, const int32_t* radii, const float* v_xys,
+                                 const float* v_depths, const float* v_conics, const float* v_comp, float* v_means,
+                                 float* v_scales, float* v_quats, void* stream) {
+    SGN_REQUIRE(means && scales && quats && cam && radii && v_means && v_scales && v_quats, "%s: null pointer", what);
+    if (N == 0) return SGN_OK;
+    l1_project_bwd_kernel<<<(N + PROJ_THREADS - 1) / PROJ_THREADS, PROJ_THREADS, 0, (cudaStream_t)stream>>>(
+        N, means, scales, glob_scale, quats, *cam, radii, v_xys, v_depths, v_conics, v_comp, v_means, v_scales, v_quats);
+    SGN_CHECK_LAUNCH("l1_project_bwd_kernel");
+    return SGN_OK;
+}
+
 extern "C" int sgn_l1_project_bwd(int N, const float* means, const float* scales, float glob_scale, const float* quats,
                                   const sgn_camera* cam, const int32_t* radii, const float* v_xys, const float* v_depths,
                                   const float* v_conics, float* v_means, float* v_scales, float* v_quats, void* stream) {
     SGN_RANGE("sgn_l1_project_bwd");
-    SGN_REQUIRE(means && scales && quats && cam && radii && v_means && v_scales && v_quats, "sgn_l1_project_bwd: null pointer");
-    if (N == 0) return SGN_OK;
-    l1_project_bwd_kernel<<<(N + PROJ_THREADS - 1) / PROJ_THREADS, PROJ_THREADS, 0, (cudaStream_t)stream>>>(
-        N, means, scales, glob_scale, quats, *cam, radii, v_xys, v_depths, v_conics, v_means, v_scales, v_quats);
-    SGN_CHECK_LAUNCH("l1_project_bwd_kernel");
-    return SGN_OK;
+    return l1_project_bwd_launch("sgn_l1_project_bwd", N, means, scales, glob_scale, quats, cam, radii, v_xys, v_depths,
+                                 v_conics, nullptr, v_means, v_scales, v_quats, stream);
+}
+
+extern "C" int sgn_l1_project_bwd_comp(int N, const float* means, const float* scales, float glob_scale, const float* quats,
+                                       const sgn_camera* cam, const int32_t* radii, const float* v_xys, const float* v_depths,
+                                       const float* v_conics, const float* v_compensation, float* v_means, float* v_scales,
+                                       float* v_quats, void* stream) {
+    SGN_RANGE("sgn_l1_project_bwd_comp");
+    return l1_project_bwd_launch("sgn_l1_project_bwd_comp", N, means, scales, glob_scale, quats, cam, radii, v_xys, v_depths,
+                                 v_conics, v_compensation, v_means, v_scales, v_quats, stream);
 }
 
 // gsplat spherical_harmonics(degrees_to_use, viewdirs[N,3], coeffs[N,K,3]) -> colors[N,3]

@@ -24,6 +24,7 @@ struct SgnProj {
     int clampx, clampy;
     float T[6];
     float a, b, c;
+    float comp;  // blur compensation (sgn_compensation), when sgn_project_exact was asked for it; 0 otherwise
     float conic[3];
     float xy[2];
     int radius;
@@ -71,12 +72,35 @@ __device__ __forceinline__ int sgn_f2i_sat(float x) {
     return (int)x;
 }
 
+// The blurred screen covariance [[a, b], [b, c]] = T S T^T + 0.3 I from T = J W (2x3) and S = Sigma3D (upper triangle 00 01 02
+// 11 12 22), in the exact section's order, and its un-blurred diagonal c00, c11.  The backward calls it again on SgnProj's
+// T and S for the same bits.
+__device__ __forceinline__ void sgn_cov2d_blur(const xf T[6], const xf S[6], xf& a, xf& b, xf& c, xf& c00, xf& c11) {
+    xf TS[6];
+    TS[0] = (T[0] * S[0] + T[1] * S[1]) + T[2] * S[2];
+    TS[1] = (T[0] * S[1] + T[1] * S[3]) + T[2] * S[4];
+    TS[2] = (T[0] * S[2] + T[1] * S[4]) + T[2] * S[5];
+    TS[3] = (T[3] * S[0] + T[4] * S[1]) + T[5] * S[2];
+    TS[4] = (T[3] * S[1] + T[4] * S[3]) + T[5] * S[4];
+    TS[5] = (T[3] * S[2] + T[4] * S[4]) + T[5] * S[5];
+    c00 = (TS[0] * T[0] + TS[1] * T[1]) + TS[2] * T[2];
+    const xf c01 = (TS[0] * T[3] + TS[1] * T[4]) + TS[2] * T[5];
+    c11 = (TS[3] * T[3] + TS[4] * T[4]) + TS[5] * T[5];
+    a = c00 + xf(0.3f);
+    b = c01;
+    c = c11 + xf(0.3f);
+}
+
+__device__ __forceinline__ float sgn_compensation(const SgnProj& st);
+
 // Returns st.visible.  `m`, `ls`, `q` are this Gaussian's raw parameters.
 // log_scales: `ls` holds log-scales (the model's parameters) -> exp is applied here; otherwise `ls` holds
 // activated scales (gsplat's project_gaussians argument) multiplied by glob_scale.
+// with_comp (warp-uniform): also st.comp = sgn_compensation(st), computed here while its inputs are live.
 __device__ __forceinline__ bool sgn_project_exact(const sgn_segment& sg, const sgn_camera& cam, const float m_[3],
                                                   const float ls[3], const float q_[4], SgnProj& st,
-                                                  const bool log_scales = true, const float glob_scale = 1.f) {
+                                                  const bool log_scales = true, const float glob_scale = 1.f,
+                                                  const bool with_comp = false) {
     xf W[12];
 #pragma unroll
     for (int k = 0; k < 12; ++k) W[k] = xf(cam.viewmat[k]);
@@ -86,6 +110,7 @@ __device__ __forceinline__ bool sgn_project_exact(const sgn_segment& sg, const s
     st.conic[0] = st.conic[1] = st.conic[2] = 0.f;
     st.tmin[0] = st.tmin[1] = st.tmax[0] = st.tmax[1] = 0;
     st.clampx = st.clampy = 0;
+    st.comp = 0.f;
     const xf m[3] = {xf(m_[0]), xf(m_[1]), xf(m_[2])};
     xf mw[3], qr[4];
     if (sg.has_pose) {
@@ -182,20 +207,10 @@ __device__ __forceinline__ bool sgn_project_exact(const sgn_segment& sg, const s
         }
 #pragma unroll
         for (int k = 0; k < 6; ++k) st.T[k] = T[k].v;
-        xf TS[6];
-        TS[0] = (T[0] * S[0] + T[1] * S[1]) + T[2] * S[2];
-        TS[1] = (T[0] * S[1] + T[1] * S[3]) + T[2] * S[4];
-        TS[2] = (T[0] * S[2] + T[1] * S[4]) + T[2] * S[5];
-        TS[3] = (T[3] * S[0] + T[4] * S[1]) + T[5] * S[2];
-        TS[4] = (T[3] * S[1] + T[4] * S[3]) + T[5] * S[4];
-        TS[5] = (T[3] * S[2] + T[4] * S[4]) + T[5] * S[5];
-        const xf c00 = (TS[0] * T[0] + TS[1] * T[1]) + TS[2] * T[2];
-        const xf c01 = (TS[0] * T[3] + TS[1] * T[4]) + TS[2] * T[5];
-        const xf c11 = (TS[3] * T[3] + TS[4] * T[4]) + TS[5] * T[5];
-        a = c00 + xf(0.3f);
-        b = c01;
-        c = c11 + xf(0.3f);
+        xf c00, c11;
+        sgn_cov2d_blur(T, S, a, b, c, c00, c11);
         st.a = a.v; st.b = b.v; st.c = c.v;
+        if (with_comp) st.comp = sgn_compensation(st);
     }
     const xf det = a * c - b * b;
     if (det.v == 0.f) return false;
@@ -229,6 +244,45 @@ __device__ __forceinline__ bool sgn_project_exact(const sgn_segment& sg, const s
     st.xy[1] = cyp.v;
     st.visible = true;
     return true;
+}
+
+// ---- blur compensation (the antialiased rasterize mode, and the Level-1 `compensation` output) ---------------------
+// comp = sqrt(max(0, det(cov2d) / det(cov2d + 0.3 I))): the factor by which the 0.3 px^2 blur spreads the Gaussian's
+// integrated density, gsplat's antialiased-mode opacity scale.  det(cov2d) of cov2d = P P^T, P = T M (2x3), M = R diag(s), is
+// taken as the sum of the squared 2x2 minors of P (Cauchy-Binet): each minor is s_i s_j times a cross product of two
+// columns of T R, so it keeps its accuracy for needles and sub-pixel Gaussians, where c00 c11 - c01^2 -- or (a - 0.3)
+// (c - 0.3) - b^2 from the blurred entries -- cancels to rounding noise.  A Gaussian of rank one on the screen has comp 0.
+// Individually rounded (xf) from SgnProj's T, Rg, s, a, b, c, so the forward and the backward compute the same bits.
+__device__ __forceinline__ float sgn_compensation(const SgnProj& st) {
+    xf P0[3], P1[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const xf m0 = xf(st.Rg[c]) * xf(st.s[c]), m1 = xf(st.Rg[3 + c]) * xf(st.s[c]), m2 = xf(st.Rg[6 + c]) * xf(st.s[c]);
+        P0[c] = (xf(st.T[0]) * m0 + xf(st.T[1]) * m1) + xf(st.T[2]) * m2;
+        P1[c] = (xf(st.T[3]) * m0 + xf(st.T[4]) * m1) + xf(st.T[5]) * m2;
+    }
+    const xf m01 = P0[0] * P1[1] - P0[1] * P1[0], m02 = P0[0] * P1[2] - P0[2] * P1[0], m12 = P0[1] * P1[2] - P0[2] * P1[1];
+    const xf det_orig = (m01 * m01 + m02 * m02) + m12 * m12;
+    const xf det_blur = xf(st.a) * xf(st.c) - xf(st.b) * xf(st.b);
+    return xsqrt(xmax(xf(0.f), det_orig / det_blur)).v;
+}
+
+// Cotangent of comp -> cotangents of the blurred a, b (the one off-diagonal parameter), c, ADDED to vA, vB, vC.  With
+// r = det_orig / det_blur and det_blur - det_orig = 0.3 (a + c) - 0.09:
+//   dr/da = 0.3 (c c11 + b^2) / det_blur^2,  dr/dc = 0.3 (a c00 + b^2) / det_blur^2,
+//   dr/db = -2 b (0.3 (a + c) - 0.09) / det_blur^2,  d comp = dr / (2 comp),
+// with c00, c11 the un-blurred diagonal (not a - 0.3, c - 0.3, which lose a sub-pixel Gaussian's covariance).  The blur is a
+// constant, so these are also the cotangents of the un-blurred cov2d.  comp == 0 (det_orig <= 0, clamped) passes nothing: the
+// clamp is flat there, and 1 / (2 comp) would be inf.
+__device__ __forceinline__ void sgn_compensation_vjp(float c00, float c11, float a, float b, float c, float comp, float v_comp,
+                                                     float& vA, float& vB, float& vC) {
+    if (!(comp > 0.f)) return;
+    const float inv = 1.f / (a * c - b * b);
+    const float w = (0.5f * v_comp) / comp * inv * inv;
+    const float b2 = b * b;
+    vA += w * (0.3f * (c * c11 + b2));
+    vC += w * (0.3f * (a * c00 + b2));
+    vB -= w * (2.f * b * (0.3f * (a + c) - 0.09f));
 }
 
 // ---- SH basis (gsplat "poly" SH, Appendix A.7); not part of the exact section -------------------

@@ -12,7 +12,8 @@ from ._common import camera_struct, need_cuda, ptr, stream
 def project_gaussians(means3d, scales, glob_scale: float, quats, viewmat, fx: float, fy: float, cx: float, cy: float,
                       img_height: int, img_width: int, block_width: int, clip_thresh: float = 0.01) -> Tuple:
     """-> (xys[N,2], depths[N], radii[N] int32, conics[N,3], compensation[N], num_tiles_hit[N] int32, cov3d[N,6]).
-    Differentiable w.r.t. means3d, scales and quats (through xys, depths and conics)."""
+    Differentiable w.r.t. means3d, scales and quats (through xys, depths, conics and compensation: the antialiased
+    mode's ``opacities * comp[:, None]`` trains the geometry through comp, as gsplat's does)."""
     assert block_width > 1 and block_width <= 16, "block_width must be between 2 and 16"
     assert (quats.norm(dim=-1) - 1 < 1e-6).all(), "quats must be normalized"
     return _ProjectGaussians.apply(means3d.contiguous(), scales.contiguous(), glob_scale, quats.contiguous(), viewmat,
@@ -54,7 +55,13 @@ class _ProjectGaussians(Function):
         c = lambda t: None if t is None else t.contiguous()
         v_xys, v_depths, v_conics = c(v_xys), c(v_depths), c(v_conics)
         v_means, v_scales, v_quats = torch.empty_like(means3d), torch.empty_like(scales), torch.empty_like(quats)
-        _lib.check(L.sgn_l1_project_bwd(N, ptr(means3d), ptr(scales), ctx.glob_scale, ptr(quats), C.byref(ctx.cs), ptr(radii),
-                                        ptr(v_xys), ptr(v_depths), ptr(v_conics), ptr(v_means), ptr(v_scales), ptr(v_quats),
-                                        stream()), "sgn_l1_project_bwd")
+        if v_comp is None:
+            _lib.check(L.sgn_l1_project_bwd(N, ptr(means3d), ptr(scales), ctx.glob_scale, ptr(quats), C.byref(ctx.cs), ptr(radii),
+                                            ptr(v_xys), ptr(v_depths), ptr(v_conics), ptr(v_means), ptr(v_scales), ptr(v_quats),
+                                            stream()), "sgn_l1_project_bwd")
+        else:  # compensation was used (the antialiased mode): its cotangent reaches the geometry through cov2d
+            v_comp = v_comp.contiguous()
+            _lib.check(L.sgn_l1_project_bwd_comp(N, ptr(means3d), ptr(scales), ctx.glob_scale, ptr(quats), C.byref(ctx.cs),
+                                                 ptr(radii), ptr(v_xys), ptr(v_depths), ptr(v_conics), ptr(v_comp), ptr(v_means),
+                                                 ptr(v_scales), ptr(v_quats), stream()), "sgn_l1_project_bwd_comp")
         return (v_means, v_scales, None, v_quats) + (None,) * 9

@@ -81,6 +81,11 @@ class SceneGraphConfig:
     full_gradient_arena: bool = False
     # no host read-back of the intersection count inside get_outputs (raster.RenderSettings.async_binning); None -> SGN_ASYNC_BIN
     async_binning: Optional[bool] = None
+    # the reference's rasterize_mode (sgn_splatfacto.py:214-223): "classic", or "antialiased" -- every render blends
+    # sigmoid(opacity) * comp, the EWA blur's compensation (raster.RenderSettings.rasterize_mode).  The reference leaves the
+    # multiply commented out, so its "antialiased" renders like "classic"; here the mode does what its docstring says.  The
+    # refinement's opacity cull / reset and the metrics keep reading sigmoid(opacity), as the reference's do
+    rasterize_mode: str = "classic"
 
     # ``stop_split_at`` of the BACKGROUND sub-model: what the reference's entropy gate reads
     # (``config.background_model.stop_split_at``, scene graph :386).  One source: ``refine.stop_split_at``.
@@ -329,6 +334,7 @@ class SceneGraphRasterModel(torch.nn.Module):
                  camera_optimizer: Optional[torch.nn.Module] = None):
         super().__init__()
         self.config = config or SceneGraphConfig()
+        raster.rasterize_mode_flag(self.config.rasterize_mode)  # an unknown mode raises ValueError, as the reference's does
         # trainable camera poses (camera_pose.CameraPoseOptimizer, nerfstudio's attribute name).  None, or one in mode "off":
         # every camera is rendered as given, by the same calls as without it
         if camera_optimizer is not None and camera_optimizer.mode != "off" and sky is not None:
@@ -531,7 +537,8 @@ class SceneGraphRasterModel(torch.nn.Module):
         n = min(self.step // c.sh_degree_interval, c.sh_degree) if self.training else c.sh_degree
         return raster.RenderSettings(sh_degree=c.sh_degree, sh_degree_to_use=n, block_width=c.block_width,
                                      alpha_clamp_fwd=c.alpha_clamp_fwd, alpha_clamp_bwd=c.alpha_clamp_bwd,
-                                     class_streams=class_streams, training=self.training, async_binning=c.async_binning)
+                                     class_streams=class_streams, training=self.training, async_binning=c.async_binning,
+                                     rasterize_mode=c.rasterize_mode)
 
     def _box_poses(self, frame: Frame) -> Optional[torch.Tensor]:
         """The corrected poses of the frame's actors, [actors, 16], from ``bbox_optimizer`` -- in training and in eval alike,

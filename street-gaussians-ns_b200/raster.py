@@ -43,6 +43,11 @@ class RenderSettings:
     # A frame whose count exceeds the capacity renders truncated lists; it is detected with the NEXT frame (warning,
     # ``raster.ASYNC_STATS``), the capacity grows.  None -> the SGN_ASYNC_BIN environment variable.  Off: exact, one sync.
     async_binning: Optional[bool] = None
+    # "classic" or "antialiased" (the reference's rasterize_mode, sgn_splatfacto.py:214-223): antialiased scales every
+    # visible Gaussian's opacity by comp = sqrt(det(cov2d) / det(cov2d + 0.3 I)), so that the 0.3 px^2 blur of the EWA
+    # projection does not inflate sub-pixel Gaussians -- gsplat's antialiased mode.  Every stream that blends the records
+    # (rgb, accumulation, depth, the class streams, the extra channels, the sky composite) follows, forward and backward
+    rasterize_mode: str = "classic"
 
 
 class StageTimer:
@@ -104,7 +109,18 @@ def camera_struct(cam: Camera, s: RenderSettings) -> _lib.CameraStruct:
     cs.block_width = s.block_width
     cs.sh_degree = s.sh_degree
     cs.sh_degree_to_use = s.sh_degree if s.sh_degree_to_use is None else s.sh_degree_to_use
+    cs.antialiased = rasterize_mode_flag(s.rasterize_mode)
     return cs
+
+
+RASTERIZE_MODES = ("classic", "antialiased")
+
+
+def rasterize_mode_flag(mode: str) -> int:
+    '''sgn_camera.antialiased for a rasterize_mode name; any other name raises ValueError.'''
+    if mode not in RASTERIZE_MODES:
+        raise ValueError(f"Unknown rasterize_mode: {mode}")
+    return int(mode == "antialiased")
 
 
 def _check_param(t: torch.Tensor, name: str, device) -> None:

@@ -27,7 +27,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         actor_range: float = 45.0, pipeline_chunks: int = 0, overlap: bool = False, resident_table: bool = True,
         async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True, sky: bool = False, metrics: bool = False,
         bbox_opt: bool = False, camera_opt: bool = False, sky_view_grad: bool = False, lidar_depth: float = 0.0,
-        semantic: float = 0.0) -> dict:
+        semantic: float = 0.0, antialiased: bool = False) -> dict:
     """One measurement.  torch.distributed must already be initialised when WORLD_SIZE > 1.  Returns the result dict on
     rank 0 (None elsewhere).  ``sky``: the reference's default learnable sky (use_sky_sphere, a 1024^2 cube map stepped by
     the same Adam launch at the ``sky_sphere`` group's lr 0.005, sgn_config.py:72-75).  ``metrics``: every step also computes
@@ -43,7 +43,8 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     that weight (SceneGraphConfig.semantic_loss_mult), against synthetic labels drawn onto the device before timing; the logits
     are the FusedAdam row group "semantic" at features_dc's lr 0.0025 (a choice: the reference config names no rate) with
     the reference's gradient accumulation of 10
-    projected with the step's camera."""
+    projected with the step's camera.  ``antialiased``: rasterize_mode "antialiased" (the opacity scaled by the blur
+    compensation, forward and backward)."""
     import torch
     import torch.distributed as dist
 
@@ -73,7 +74,8 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     cfg = SceneGraphConfig(use_sky_sphere=sky, ssim_lambda=ssim_lambda, fused_loss=fused_loss, full_gradient_arena=world > 1, refine=rs, async_binning=async_binning,
                            object_refine=RefineSettings(refine_every=refine_every, cull_alpha_thresh=0.005),
                            num_train_data=len(cams), refine_record=True, depth_loss_mult=lidar_depth,
-                           semantic_classes=3 if semantic > 0 else 0, semantic_loss_mult=semantic)
+                           semantic_classes=3 if semantic > 0 else 0, semantic_loss_mult=semantic,
+                           rasterize_mode="antialiased" if antialiased else "classic")
     env_map = None
     if sky:
         from street_gaussians_ns_b200.sky import CubeMapSky
@@ -233,6 +235,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                    **({"lidar_depth": f"depth_loss_mult {lidar_depth}, street_points(170_000, seed=step) per step"} if lidar_depth > 0 else {}),
                    **({"semantic": f"3 classes, semantic_loss_mult {semantic}, Adam lr 0.0025, gradient accumulation 10, synthetic labels"}
                       if semantic > 0 else {}),
+                   **({"rasterize_mode": "antialiased"} if antialiased else {}),
                    "loss": "fused kernels" if fused_loss else "torch ops", "metrics": "get_metrics_dict every step" if metrics else "none",
                    "start_step": start_step, "refine_every": refine_every,
                    "refinement_kernels_loaded_before_timing": refine_warm,
@@ -270,6 +273,7 @@ def main():
                     help="> 0: the lidar depth term at weight W against a synthetic 170 k-point sweep per step")
     ap.add_argument("--semantic", type=float, default=0.0, metavar="W",
                     help="> 0: 3-class semantic logits and the cross-entropy term at weight W against synthetic labels")
+    ap.add_argument("--antialiased", action="store_true", help="rasterize_mode 'antialiased': opacities scaled by the blur compensation")
     args = ap.parse_args()
     if args.sky_view_grad and not (args.sky and args.camera_opt):
         ap.error("--sky-view-grad needs --sky and --camera-opt")
@@ -285,7 +289,7 @@ def main():
     res = run(args.steps, args.warmup, args.scale, args.refine_every, args.start_step, args.actor_range, args.pipeline_chunks,
               args.overlap, not args.host_table, ssim_lambda=args.ssim_lambda, fused_loss=not args.torch_loss, sky=args.sky,
               metrics=args.metrics, bbox_opt=args.bbox_opt, camera_opt=args.camera_opt,
-              sky_view_grad=args.sky_view_grad, lidar_depth=args.lidar_depth, semantic=args.semantic)
+              sky_view_grad=args.sky_view_grad, lidar_depth=args.lidar_depth, semantic=args.semantic, antialiased=args.antialiased)
     if res is not None:
         print(json.dumps(res))
     if world > 1:
