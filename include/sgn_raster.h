@@ -671,6 +671,22 @@ int sgn_refine_carry(int n, const sgn_refine_config* cfg, const uint8_t* flags, 
                      const float* src, float* dst, int width, const float* src_m, const float* src_v, float* dst_m, float* dst_v,
                      void* stream);
 
+/* ---- scale regularisation (nerfstudio's use_scale_regularization, which the reference's config sets, sgn_splatfacto.py:206-211)
+ * Over the N rows of the segment table (read in place, 128-row chunks as sgn_project_fwd), with s = exp(scales):
+ *   *out = 0.1 * mean_rows(max(amax(s) / amin(s), max_ratio) - max_ratio)
+ * expf / division / max in fp32 per row, sums in fp64 per block added in a fixed order (bit-identical run to run), the mean rounded
+ * once to fp32, then * 0.1f.  N = 0 gives NaN, as torch's mean of nothing.  No host synchronisation.
+ * The backward ADDS d out / d scales * (*v_out) into grads_dev[k].scales (v_out: device scalar), following torch autograd of the
+ * expression in fp32: the gradient is halved at amax / amin == max_ratio (torch.maximum's tie) and split evenly between tied
+ * elements of the max and of the min.  Rows with amax / amin < max_ratio are not written.  Elementwise: deterministic.
+ * A null table with nseg > 0, a null out / scratch / v_out, chunks without segments (SGN_ERR_INVALID) or a short scratch
+ * (SGN_ERR_WORKSPACE) launch nothing. */
+size_t sgn_scale_reg_scratch_bytes(void);
+int sgn_scale_reg_fwd(const sgn_segment* table_dev, int nseg, int N, int num_chunks, float max_ratio, float* out, void* scratch,
+                      size_t scratch_bytes, void* stream);
+int sgn_scale_reg_bwd(const sgn_segment* table_dev, const sgn_segment_grads* grads_dev, int nseg, int N, int num_chunks, float max_ratio,
+                      const float* v_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

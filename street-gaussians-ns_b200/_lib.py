@@ -141,6 +141,7 @@ EXPORTS = [
     "sgn_sky_rot_scratch_bytes", "sgn_sky_bwd_view_rot", "sgn_sky_bwd_det_view_rot", "sgn_knn_scratch_bytes", "sgn_knn",
     "sgn_lidar_depth_map", "sgn_depth_scratch_bytes", "sgn_depth_loss_fwd", "sgn_depth_loss_bwd", "sgn_depth_metrics",
     "sgn_semantic_scratch_bytes", "sgn_semantic_loss_fwd", "sgn_semantic_loss_bwd", "sgn_semantic_metrics", "sgn_refine_carry",
+    "sgn_scale_reg_scratch_bytes", "sgn_scale_reg_fwd", "sgn_scale_reg_bwd",
 ]
 VIEW_FLOATS = 12  # SGN_VIEW_FLOATS: the view's cotangent, viewmat[12] row-major; the device view itself is 12 + 3 (cam_pos) floats
 POSE_FLOATS = 16  # SGN_POSE_FLOATS: a segment's pose (and its cotangent) as R[9] row-major, t[3], q[4]
@@ -280,6 +281,10 @@ def load():
     L.sgn_refine_carry.argtypes = [i32, C.POINTER(RefineConfig), vp, vp, C.POINTER(C.c_int32), vp, vp, i32, vp, vp, vp, vp, vp]
     for f in ("sgn_semantic_loss_fwd", "sgn_semantic_loss_bwd", "sgn_semantic_metrics", "sgn_refine_carry"):
         getattr(L, f).restype = C.c_int
+    L.sgn_scale_reg_scratch_bytes.restype = sz
+    L.sgn_scale_reg_fwd.argtypes = [vp, i32, i32, i32, fl, vp, vp, sz, vp]
+    L.sgn_scale_reg_bwd.argtypes = [vp, vp, i32, i32, i32, fl, vp, vp]
+    L.sgn_scale_reg_fwd.restype = L.sgn_scale_reg_bwd.restype = C.c_int
     L.sgn_sizeof_adam_tensor.restype = sz
     L.sgn_adam_chunk_elems.restype = C.c_int
     L.sgn_adam_step.argtypes = [vp, i32, i32, vp, vp, vp, vp]

@@ -34,6 +34,7 @@ SOURCES = {
     "knn.cu": [],  # distances through explicit _rn intrinsics: the box bound must not exceed a point's distance
     "depth.cu": [],  # the lidar projection is the projection's xf arithmetic; IEEE log / division in the metrics
     "semantic.cu": [],  # IEEE expf / logf / division in the cross-entropy; the carry only copies
+    "scale_reg.cu": [],  # IEEE expf; the gradient chain through explicit _rn intrinsics, as torch autograd rounds it
 }
 
 

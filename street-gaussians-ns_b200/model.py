@@ -86,6 +86,12 @@ class SceneGraphConfig:
     # multiply commented out, so its "antialiased" renders like "classic"; here the mode does what its docstring says.  The
     # refinement's opacity cull / reset and the metrics keep reading sigmoid(opacity), as the reference's do
     rasterize_mode: str = "classic"
+    # nerfstudio's scale regularisation (PhysGaussian), which the reference's config turns on (use_scale_regularization = True,
+    # max_gauss_ratio = 10, sgn_splatfacto.py:206-211) and its loss never computes: every tenth step, losses["scale_reg"] =
+    # 0.1 * mean(max(amax(exp(scales)) / amin(exp(scales)), max_gauss_ratio) - max_gauss_ratio) over the visible rows.  Off here
+    # by default; the 0.1 weight and the 10-step cadence are nerfstudio's constants
+    use_scale_regularization: bool = False
+    max_gauss_ratio: float = 10.0
 
     # ``stop_split_at`` of the BACKGROUND sub-model: what the reference's entropy gate reads
     # (``config.background_model.stop_split_at``, scene graph :386).  One source: ``refine.stop_split_at``.
@@ -223,13 +229,34 @@ class _GradSink:
     allocator = None  # optional callable(total, device) -> float32 tensor: where the persistent arena lives (data parallel: a
     #                   symmetric allocation the exchange kernel can address on every replica)
 
-    def target(self, static: dict, device):
+    def _ensure_arena(self, static: dict, device) -> None:
         sizes, _, _ = raster.arena_layout(static)
         total = sum(sizes)
         if self.arena is None or self.arena.numel() != total or self.arena.device != device:
             self.arena = self.allocator(total, device) if self.allocator is not None else torch.empty(total, device=device, dtype=torch.float32)
             assert self.arena.numel() == total and self.arena.dtype == torch.float32
             self.views = raster.arena_views(self.arena, static)
+
+    def collect(self, static: dict, device) -> tuple:
+        """The persistent arena made to hold every bound parameter's ``.grad`` (which then points at its slice), for a fused
+        optimizer that reads the arena: needed after a backward in which a gradient reached the parameters outside the render
+        (a torch loss term of the parameters themselves), so that ``.grad`` was set before the render's backward ran and the
+        render added its share through a temporary arena.  A parameter without a gradient gets a zero slice.  Returns (arena,
+        the PARAM_NAMES positions that have a gradient in some bound parameter)."""
+        self._ensure_arena(static, device)
+        kinds = set()
+        for i, (p, v) in enumerate(zip(self.params, self.views)):
+            if p.grad is None:
+                v.zero_()
+                continue
+            kinds.add(i % 6)
+            if p.grad.data_ptr() != v.data_ptr():
+                v.copy_(p.grad)
+                p.grad = v
+        return self.arena, sorted(kinds)
+
+    def target(self, static: dict, device):
+        self._ensure_arena(static, device)
         for p in self.params:
             if p.grad is not None:
                 return None  # accumulate: render into a temporary arena, add in publish()
@@ -297,14 +324,26 @@ class _FullArenaSink(_GradSink):
         chunks = arena.split_with_sizes([int(x) for x in self.sizes])
         self.all_views = [c[:int(np.prod(shp))].view(shp) for c, shp in zip(chunks, self.all_shapes)]
 
-    def target(self, static: dict, device):
+    def _ensure_arena(self, static: dict, device) -> None:
         total = int(self.sizes.sum())
         if self.arena is None or self.arena.numel() != total or self.arena.device != device:
             self.set_arena(torch.zeros(total, device=device, dtype=torch.float32))
         self.views = [self.all_views[t] for t in self._tensor_ids()]
+
+    def collect(self, static: dict, device) -> tuple:
+        arena, kinds = super().collect(static, device)
+        self._zero_absent()
+        return arena, kinds
+
+    def target(self, static: dict, device):
+        self._ensure_arena(static, device)
         for p in self.params:
             if p.grad is not None:
                 return None  # accumulate: render into a temporary arena (frame layout), add in publish()
+        self._zero_absent()
+        return self.arena
+
+    def _zero_absent(self) -> None:
         # zero the sub-models that are not in this frame (runs of absent sub-models are contiguous in the arena);
         # after an all-reduce they hold the other replicas' gradients
         nsub = len(self.sizes) // 6
@@ -321,7 +360,6 @@ class _FullArenaSink(_GradSink):
             hi = int(self.offsets[6 * (j - 1) + 5] + self.sizes[6 * (j - 1) + 5])
             self.arena[lo:hi].zero_()
             i = j
-        return self.arena
 
 
 _MODEL_SERIAL = itertools.count()
@@ -595,13 +633,20 @@ class SceneGraphRasterModel(torch.nn.Module):
                 anchor = self._anchor
         pose = self._box_poses(frame)
         extra = self._semantic_rows(frame)
-        if extra is None:
-            out, holder = raster.render_frame(frame, self._settings(class_streams=True), sky=sky, grad_sink=sink, anchor=anchor,
-                                              pose=pose, view=view)
-        else:
-            out, holder = raster.render_frame(frame, self._settings(class_streams=True), sky=sky, grad_sink=sink, anchor=anchor,
-                                              extra=extra, pose=pose, view=view)
+        kw = {}
+        if extra is not None:
+            kw["extra"] = extra
+        # the scale regularisation of this step comes out of the render (raster.render_frame, scale_reg=); get_loss_dict takes it
+        # from here, so ``outputs`` keeps its keys
+        self.__dict__["_scale_reg"] = None
+        if self._fused_scale_reg_due():
+            kw["scale_reg"] = self.config.max_gauss_ratio
+        out, holder = raster.render_frame(frame, self._settings(class_streams=True), sky=sky, grad_sink=sink, anchor=anchor,
+                                          pose=pose, view=view, **kw)
+        if extra is not None:
             out["semantic"] = out.pop("extra")
+        if "scale_reg" in kw:
+            self.__dict__["_scale_reg"] = out.pop("scale_reg")
         self._holder = holder
         self._publish_side_effects(frame, holder)
         if isinstance(holder.M, raster.LazyCount):
@@ -631,6 +676,35 @@ class SceneGraphRasterModel(torch.nn.Module):
                     # (scene graph :264-267), which get_outputs publishes as object_rgb AND object_depth (:371-372)
                     out["object_depth"] = torch.zeros(H, W, 1, device=self.device)
         return out
+
+    def _fused_scale_reg_due(self) -> bool:
+        """Whether this step's scale regularisation comes out of the render: switched on, a step that is a multiple of 10 (as
+        nerfstudio's), the fused loss path (``fused_loss=False`` computes it with torch ops in get_loss_dict), and a training
+        render that records gradients (an eval loss takes the value alone, see ``_scale_reg_loss``)."""
+        c = self.config
+        return (c.use_scale_regularization and self.step % 10 == 0 and c.fused_loss and self.training
+                and torch.is_grad_enabled())
+
+    def _scale_reg_loss(self, fused: bool) -> torch.Tensor:
+        """losses["scale_reg"] (SplatfactoModel.get_loss_dict of nerfstudio 1.0) over the visible sub-models' rows, in the frame's
+        concatenation order; a zero without gradient on the steps that are not a multiple of 10."""
+        c = self.config
+        if self.step % 10 != 0:
+            return torch.zeros((), device=self.device)
+        if fused:
+            reg = self.__dict__.get("_scale_reg")
+            if reg is not None:
+                return reg
+            h = self._holder
+            if (self.training and torch.is_grad_enabled()) or h is None or h.table is None:
+                raise RuntimeError("the scale regularisation of this step was not rendered: call get_outputs at the same model.step "
+                                   "before get_loss_dict")
+            return raster.scale_reg_fwd(h.table, c.max_gauss_ratio)  # eval / no_grad: the value alone, from the last frame's rows
+        scales = torch.cat([self.all_models._modules[n].gauss_params["scales"] for n in self.visible_model_names])
+        scale_exp = torch.exp(scales)
+        scale_reg = torch.maximum(scale_exp.amax(dim=-1) / scale_exp.amin(dim=-1),
+                                  torch.tensor(c.max_gauss_ratio, device=scales.device)) - c.max_gauss_ratio
+        return 0.1 * scale_reg.mean()
 
     def _semantic_rows(self, frame: Frame) -> Optional[torch.Tensor]:
         """The frame's semantic logits [N, C] in its row order (the visible sub-models' ``semantic_logits``, concatenated in
@@ -892,7 +966,12 @@ class SceneGraphRasterModel(torch.nn.Module):
         Sky-labelled pixels are supervised like any other class: the semantic map there is the blend of whatever Gaussians the
         pixel sees, and ``sky_accumulation`` separately pushes their accumulation towards 0, which also shrinks the blended logits
         (weights sum to the accumulation).  The two terms therefore pull against each other on sky pixels; nothing special-cases
-        that, as a segmentation with a sky class gives both signals."""
+        that, as a segmentation with a sky class gives both signals.
+
+        With ``use_scale_regularization``, ``scale_reg`` is present on every call, as nerfstudio emits it: at a step that is a
+        multiple of 10, 0.1 * mean(max(amax(s) / amin(s), max_gauss_ratio) - max_gauss_ratio) with s = exp(scales) over the rows
+        of the visible sub-models (the render computed it, sgn_scale_reg_fwd; torch ops over ``torch.cat`` of their scales
+        with ``fused_loss=False``), and a zero without gradient on the other steps."""
         c = self.config
         want_sky = "semantic" in batch and c.sky_acc_loss_mult > 0
         want_ent = c.object_acc_entropy_loss_mult > 0.0 and self.step > c.refine.stop_split_at  # background_model.stop_split_at (:386)
@@ -955,6 +1034,8 @@ class SceneGraphRasterModel(torch.nn.Module):
             from .semantic import fused_semantic_loss, semantic_loss_torch
             term = fused_semantic_loss if fused else semantic_loss_torch
             losses["semantic_loss"] = term(outputs["semantic"], batch["semantic"], batch.get("mask"), c.semantic_loss_mult)
+        if c.use_scale_regularization:
+            losses["scale_reg"] = self._scale_reg_loss(fused)
         co = self.camera_optimizer
         if self.training and co is not None and co.mode != "off":
             terms = getattr(self, "_camera_terms", None)

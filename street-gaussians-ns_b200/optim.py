@@ -167,11 +167,15 @@ class FusedAdam:
     # ---- the step -------------------------------------------------------------------------------------------
     def step_table(self, present: Optional[Sequence[int]] = None, full_layout: bool = False, grad_arena: Optional[torch.Tensor] = None,
                    extra_grads: Optional[Dict[str, torch.Tensor]] = None,
-                   row_grads: Optional[Dict[str, Sequence[Optional[torch.Tensor]]]] = None) -> np.ndarray:
+                   row_grads: Optional[Dict[str, Sequence[Optional[torch.Tensor]]]] = None,
+                   kinds: Optional[Sequence[int]] = None) -> np.ndarray:
         """Advance the step counts of the tensors that have a gradient and return their sgn_adam_tensor rows.
         ``present``: indices of the sub-models that have a gradient this step (None = all).  The gradient arena
         either holds exactly those, back to back in that order (a frame's arena, the default), or has the optimizer's
-        own layout with the absent sub-models' slices unused (``full_layout``: the data-parallel arena, model.py)."""
+        own layout with the absent sub-models' slices unused (``full_layout``: the data-parallel arena, model.py).
+        ``kinds``: which of a present sub-model's six tensors (PARAM_NAMES positions) have a gradient (None = all six); the
+        arena keeps its layout, the other tensors are skipped -- moments, step counts and values untouched, as torch.optim.Adam
+        skips a parameter whose ``grad`` is None."""
         extras = []
         if self.extra_index:  # rows of the extra tensors that have a gradient this step
             assert not extra_grads or grad_arena is not None, "extra_grads need grad_arena (their offsets are relative to it)"
@@ -195,21 +199,28 @@ class FusedAdam:
                     delta = g.data_ptr() - grad_arena.data_ptr()
                     assert delta % 4 == 0
                     extras.append((i, delta // 4))
-        if present is None and not self.extra_index and not self.row_index:
+        if present is None and not self.extra_index and not self.row_index and kinds is None:
             idx = slice(None)
             tab = self.table  # grad_offset == arena_offset, chunk0 as installed
         else:
             present = list(range(self.num_segments)) if present is None else list(present)
             assert len(set(present)) == len(present) and all(0 <= s < self.num_segments for s in present), present
             idx = (np.asarray(present, np.int64)[:, None] * 6 + np.arange(6)[None, :]).reshape(-1)
+            goff = self.table["grad_offset"][idx]
+            if not full_layout and len(present) < self.num_segments:
+                goff = np.concatenate([[0], np.cumsum(self.sizes[idx])[:-1]])
+            if kinds is not None:  # the arena's layout holds all six tensors: offsets first, then the selection
+                assert all(0 <= k < 6 for k in kinds), kinds
+                keep = np.isin(idx % 6, np.asarray(list(kinds), np.int64))
+                idx, goff = idx[keep], goff[keep]
+            n_own = len(idx)
             idx = np.concatenate([idx, np.asarray([i for i, _ in extras], np.int64)]) if extras else idx
             tab = self.table[idx]
-            sz, ch = self.sizes[idx], self.chunks[idx]
-            if not full_layout and len(present) < self.num_segments:
-                tab["grad_offset"][:6 * len(present)] = np.concatenate([[0], np.cumsum(sz[:6 * len(present)])[:-1]])
+            ch = self.chunks[idx]
+            tab["grad_offset"][:n_own] = goff
             for r, (_, off) in enumerate(extras):
-                tab["grad_offset"][6 * len(present) + r] = off
-            tab["chunk0"] = np.concatenate([[0], np.cumsum(ch)[:-1]])
+                tab["grad_offset"][n_own + r] = off
+            tab["chunk0"] = np.concatenate([[0], np.cumsum(ch)[:-1]]) if len(idx) else []
 
         self.steps[idx] += 1
         st = self.steps[idx].astype(np.float64)
@@ -220,11 +231,11 @@ class FusedAdam:
 
     def step(self, grad_arena: torch.Tensor, present: Optional[Sequence[int]] = None, full_layout: bool = False,
              extra_grads: Optional[Dict[str, torch.Tensor]] = None,
-             row_grads: Optional[Dict[str, Sequence[Optional[torch.Tensor]]]] = None) -> None:
+             row_grads: Optional[Dict[str, Sequence[Optional[torch.Tensor]]]] = None, kinds: Optional[Sequence[int]] = None) -> None:
         self.step_count += 1
         # the launch is asynchronous: keep the gradient tensors alive until the next step
         self._keep = extra_grads if row_grads is None else (extra_grads, row_grads)
-        self.launch(self.step_table(present, full_layout, grad_arena, extra_grads, row_grads), grad_arena)
+        self.launch(self.step_table(present, full_layout, grad_arena, extra_grads, row_grads, kinds), grad_arena)
 
     def launch(self, tab: np.ndarray, grad_arena: torch.Tensor) -> None:
         """One ``sgn_adam_step`` over the rows of ``tab`` (from step_table, possibly cut by rows_in_range)."""

@@ -631,6 +631,54 @@ def arena_views(arena: torch.Tensor, static: dict) -> List[torch.Tensor]:
     return [c[:n].view(shp) if n != c.shape[0] else c.view(shp) for c, n, shp in zip(chunks, numels, shapes)]
 
 
+def _arena_grads_table(arena: torch.Tensor, static: dict, device, out_offsets: Optional[np.ndarray] = None) -> torch.Tensor:
+    """The sgn_segment_grads rows of a frame into ``arena``: back to back in the frame's layout, or at ``out_offsets``
+    (floats, one per parameter tensor, multiples of 4) inside a larger arena."""
+    flat_sizes, _, _ = arena_layout(static)
+    if out_offsets is None:
+        assert arena.numel() == sum(flat_sizes)
+        return _grads_table(arena, static, device)
+    assert len(out_offsets) == len(flat_sizes)
+    off = np.asarray(out_offsets, np.int64)
+    assert (off % 4 == 0).all() and int((off + np.asarray(flat_sizes, np.int64)).max()) <= arena.numel()
+    return torch.from_numpy((np.uint64(arena.data_ptr()) + (off * 4).astype(np.uint64)).view(np.uint8)).to(device, non_blocking=True)
+
+
+def scale_reg_fwd(table: SegmentTable, max_ratio: float) -> torch.Tensor:
+    """The scale regularisation over the frame's rows, 0.1 * mean(max(amax(s) / amin(s), max_ratio) - max_ratio) with
+    s = exp(scales): a 0-d float32 tensor on the device, no read-back (sgn_scale_reg_fwd)."""
+    L = _lib.load()
+    device = table.dev.device
+    out = torch.empty((), device=device, dtype=torch.float32)
+    sb = L.sgn_scale_reg_scratch_bytes()
+    scratch = torch.empty(sb, device=device, dtype=torch.uint8)
+    with _timed("scale_reg_fwd"):
+        _lib.check(L.sgn_scale_reg_fwd(_ptr(table.dev), table.nseg, table.N, table.num_chunks, float(max_ratio), _ptr(out), _ptr(scratch),
+                                       sb, _stream()), "sgn_scale_reg_fwd")
+    return out
+
+
+def scale_reg_bwd(table: SegmentTable, arena: torch.Tensor, max_ratio: float, v_out: torch.Tensor,
+                  out_offsets: Optional[np.ndarray] = None) -> None:
+    """ADDS the scale regularisation's gradient times ``v_out`` (a float32 device scalar) into the scales slices of the
+    gradient arena (laid out as project_bwd's, ``out_offsets`` likewise); sgn_scale_reg_bwd."""
+    L = _lib.load()
+    v_out = v_out.detach().reshape(()).to(torch.float32).contiguous()
+    gt = _arena_grads_table(arena, table.static, arena.device, out_offsets)
+    with _timed("scale_reg_bwd"):
+        _lib.check(L.sgn_scale_reg_bwd(_ptr(table.dev), _ptr(gt), table.nseg, table.N, table.num_chunks, float(max_ratio), _ptr(v_out),
+                                       _stream()), "sgn_scale_reg_bwd")
+
+
+def _zero_arena(static: dict, device, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The gradient arena of a backward with no image-space cotangent: ``out`` zeroed (all of it, also the slices of sub-models
+    outside the frame when ``out`` has the layout of the whole model), or a new zero arena in the frame's layout."""
+    if out is None:
+        flat_sizes, _, _ = arena_layout(static)
+        return torch.zeros(sum(flat_sizes), device=device, dtype=torch.float32)
+    return out.zero_()
+
+
 def project_bwd(table: SegmentTable, params: List[List[torch.Tensor]], cs, records, radii, v_records, make_views: bool = True,
                 out: Optional[torch.Tensor] = None, out_offsets: Optional[np.ndarray] = None, chunk_ranges=None, after_range=None,
                 v_pose: Optional[torch.Tensor] = None, view: Optional[torch.Tensor] = None, v_view: Optional[torch.Tensor] = None):
@@ -650,13 +698,8 @@ def project_bwd(table: SegmentTable, params: List[List[torch.Tensor]], cs, recor
     arena = out if out is not None else torch.empty(sum(flat_sizes), device=device, dtype=torch.float32)
     assert arena.dtype == torch.float32 and arena.is_contiguous()
     if out_offsets is not None:
-        assert out is not None and not make_views and len(out_offsets) == len(flat_sizes)
-        off = np.asarray(out_offsets, np.int64)
-        assert (off % 4 == 0).all() and int((off + np.asarray(flat_sizes, np.int64)).max()) <= arena.numel()
-        gt = torch.from_numpy((np.uint64(arena.data_ptr()) + (off * 4).astype(np.uint64)).view(np.uint8)).to(device, non_blocking=True)
-    else:
-        assert arena.numel() == sum(flat_sizes)
-        gt = _grads_table(arena, st, device)
+        assert out is not None and not make_views
+    gt = _arena_grads_table(arena, st, device, out_offsets)
     flat = arena_views(arena, st) if make_views else None
     partials = None
     if v_pose is not None:
@@ -722,12 +765,16 @@ class _Holder:
         # model path: an object with target(static) -> arena-or-None and publish(arena, static); the parameter
         # gradients are then delivered through it instead of through 6 x segments autograd leaves
         self.grad_sink = None
+        # the last backward had no image-space cotangent (only the scale regularisation's): the blend and projection were
+        # skipped, and the arena holds zeros but for the scales
+        self.params_only = False
 
 
 class _SceneGraphRasterize(torch.autograd.Function):
     @staticmethod
     def forward(ctx, frame: Frame, settings: RenderSettings, holder: _Holder, sky: Optional[torch.Tensor],
-                extra: Optional[torch.Tensor], pose: Optional[torch.Tensor], view: Optional[torch.Tensor], *flat):
+                extra: Optional[torch.Tensor], pose: Optional[torch.Tensor], view: Optional[torch.Tensor], scale_reg: Optional[float],
+                *flat):
         # unused outputs must reach backward as None, not as zero tensors: the kernels specialise on
         # which cotangents exist (depth / background_acc have none in training)
         ctx.set_materialize_grads(False)
@@ -783,18 +830,29 @@ class _SceneGraphRasterize(torch.autograd.Function):
             extra = extra.contiguous()
             ctx.extra = extra.detach()
             outs.append(blend_extra_fwd(cs, bo, records, sorted_ids, tile_bins, out["final_T"], out["final_idx"], ctx.extra))
+        ctx.scale_reg = scale_reg
+        if scale_reg is not None:  # the scale regularisation: a term of the parameters alone, from the frame's table
+            outs.append(scale_reg_fwd(table, scale_reg))
         return tuple(outs)
 
     @staticmethod
     def backward(ctx, *v):
-        v_extra_img = None
+        v_scale_reg = v_extra_img = None
+        if ctx.scale_reg is not None:
+            v, v_scale_reg = v[:-1], v[-1]
         if ctx.extra is not None:
             v, v_extra_img = v[:-1], v[-1]
         names = ["rgb", "accumulation", "depth", "object_acc", "background_acc"][: len(v)]
         vd = {k: t for k, t in zip(names, v)}
-        v_records, v_sky = blend_bwd(ctx.cs, ctx.bo, ctx.records, ctx.sorted_ids, ctx.tile_bins, ctx.saved, ctx.sky, vd,
-                                     ctx.sky_needs_grad, ctx.obj_ids, ctx.obj_bins, deterministic=ctx.settings.deterministic)
-        v_extra = None
+        # only the scale regularisation has a cotangent (nothing in view, or a backward of that term alone): every image-space
+        # gradient is zero, so the blend and the projection are skipped and the arena starts from zeros
+        params_only = ctx.scale_reg is not None and v_extra_img is None and all(t is None for t in vd.values())
+        v_extra = v_sky = None
+        if params_only:
+            v_records = torch.zeros_like(ctx.records)
+        else:
+            v_records, v_sky = blend_bwd(ctx.cs, ctx.bo, ctx.records, ctx.sorted_ids, ctx.tile_bins, ctx.saved, ctx.sky, vd,
+                                         ctx.sky_needs_grad, ctx.obj_ids, ctx.obj_bins, deterministic=ctx.settings.deterministic)
         if v_extra_img is not None:  # adds the extra channels' share of the geometry gradients to v_records before project_bwd
             v_extra = blend_extra_bwd(ctx.cs, ctx.bo, ctx.records, ctx.sorted_ids, ctx.tile_bins, ctx.saved["final_T"],
                                       ctx.saved["final_idx"], ctx.extra, v_extra_img, v_records,
@@ -812,18 +870,32 @@ class _SceneGraphRasterize(torch.autograd.Function):
         if sink is not None:
             target = sink.target(ctx.table.static, v_records.device)
             offsets = sink.grad_offsets(ctx.table.static) if target is not None else None  # None: the frame's own layout
-            chunk_ranges = after_range = None
-            plan = getattr(sink, "exchange_plan", None)  # data parallel: the arena is produced and exchanged range by range
-            if plan is not None and target is not None:
-                chunk_ranges, after_range = plan(ctx.table)
-            _, arena = project_bwd(ctx.table, ctx.params, ctx.cs, ctx.records, ctx.radii, v_records, make_views=False,
-                                   out=target, out_offsets=offsets, chunk_ranges=chunk_ranges, after_range=after_range, v_pose=v_pose,
-                                   view=view, v_view=v_view)
+            if params_only:
+                arena = _zero_arena(ctx.table.static, v_records.device, target)
+            else:
+                chunk_ranges = after_range = None
+                plan = getattr(sink, "exchange_plan", None)  # data parallel: the arena is produced and exchanged range by range
+                if plan is not None and target is not None:
+                    chunk_ranges, after_range = plan(ctx.table)
+                _, arena = project_bwd(ctx.table, ctx.params, ctx.cs, ctx.records, ctx.radii, v_records, make_views=False,
+                                       out=target, out_offsets=offsets, chunk_ranges=chunk_ranges, after_range=after_range,
+                                       v_pose=v_pose, view=view, v_view=v_view)
+            if v_scale_reg is not None:  # project_bwd overwrote the arena: the term's gradient is added after it
+                scale_reg_bwd(ctx.table, arena, ctx.scale_reg, v_scale_reg, offsets)
             sink.publish(arena, ctx.table.static)
             flat = (None,)
         else:
-            flat, arena = project_bwd(ctx.table, ctx.params, ctx.cs, ctx.records, ctx.radii, v_records, v_pose=v_pose, view=view,
-                                      v_view=v_view)
+            if params_only:
+                arena = _zero_arena(ctx.table.static, v_records.device)
+                flat = arena_views(arena, ctx.table.static)
+            else:
+                flat, arena = project_bwd(ctx.table, ctx.params, ctx.cs, ctx.records, ctx.radii, v_records, v_pose=v_pose, view=view,
+                                          v_view=v_view)
+            if v_scale_reg is not None:
+                scale_reg_bwd(ctx.table, arena, ctx.scale_reg, v_scale_reg)
+        if params_only:  # no image term reached the poses or the view
+            v_pose = v_view = None
+        h.params_only = params_only
         h.v_records, h.grad_arena, h.v_pose, h.v_view = v_records, arena, v_pose, v_view
         if v_pose is not None:
             g_pose = v_pose[posed_rows(ctx.table)[0]]
@@ -832,16 +904,18 @@ class _SceneGraphRasterize(torch.autograd.Function):
         h.xys.grad = v_records[:, 0:2]
         if h.post_backward is not None:
             h.post_backward(h)
-        return (None, None, None, v_sky, v_extra, g_pose, g_view if ctx.view_needs_grad else None, *flat)
+        return (None, None, None, v_sky, v_extra, g_pose, g_view if ctx.view_needs_grad and not params_only else None, None, *flat)
 
 
 def forward_backward(frame: Frame, settings: RenderSettings, cotangents: Dict[str, Optional[torch.Tensor]],
                      sky: Optional[torch.Tensor] = None, want_param_grads: bool = False, grad_out: Optional[torch.Tensor] = None,
-                     chunk_ranges=None, after_range=None, after_project=None):
+                     chunk_ranges=None, after_range=None, after_project=None, scale_reg: Optional[float] = None):
     """One frame, forward AND backward, straight through the C-ABI stages (no autograd graph).
 
-    ``cotangents`` maps output names (rgb, accumulation, depth, object_acc, background_acc) to their
-    cotangent tensors (missing / None = no gradient from that output).  Returns (outputs, holder);
+    ``cotangents`` maps output names (rgb, accumulation, depth, object_acc, background_acc, and scale_reg with ``scale_reg``) to
+    their cotangent tensors (missing / None = no gradient from that output).  ``scale_reg`` (max_ratio, None = off): the outputs
+    also hold the scale regularisation (see ``render_frame``); its cotangent, a device scalar, adds the term's gradient to the
+    arena after project_bwd.  Returns (outputs, holder);
     ``holder.grad_arena`` is the flat dense gradient arena (what the data-parallel all-reduce and a
     fused optimizer consume), ``holder.v_records[:, 0:2]`` the pixel-space mean gradients the
     densification statistics read.  With ``want_param_grads`` the per-parameter views are returned in
@@ -864,11 +938,23 @@ def forward_backward(frame: Frame, settings: RenderSettings, cotangents: Dict[st
     if settings.class_streams:
         cls_ids, cls_bins = class_lists(cs, M, sorted_ids, tile_bins)
     out = blend_fwd(cs, bo, records, sorted_ids, tile_bins, sky, cls_ids, cls_bins)
+    reg = scale_reg_fwd(table, scale_reg) if scale_reg is not None else None
     v = {k: cotangents.get(k) for k in ("rgb", "accumulation", "depth", "object_acc", "background_acc")}
-    v_records, v_sky = blend_bwd(cs, bo, records, sorted_ids, tile_bins, out, sky, v, sky is not None, cls_ids, cls_bins,
-                                 deterministic=settings.deterministic)
-    flat, arena = project_bwd(table, params, cs, records, radii, v_records, make_views=want_param_grads, out=grad_out,
-                              chunk_ranges=chunk_ranges, after_range=after_range)
+    v_scale_reg = cotangents.get("scale_reg")
+    assert v_scale_reg is None or scale_reg is not None, "a scale_reg cotangent needs scale_reg (max_ratio)"
+    # the term's gradient is added after project_bwd: with ranges, the exchange of a range may already be reading it
+    assert scale_reg is None or (chunk_ranges is None and after_range is None), "scale_reg does not combine with ranged exchange"
+    if scale_reg is not None and all(t is None for t in v.values()):  # as the render's backward: nothing image-space to propagate
+        v_records, v_sky = torch.zeros_like(records), None
+        arena = _zero_arena(table.static, device, grad_out)
+        flat = arena_views(arena, table.static) if want_param_grads else None
+    else:
+        v_records, v_sky = blend_bwd(cs, bo, records, sorted_ids, tile_bins, out, sky, v, sky is not None, cls_ids, cls_bins,
+                                     deterministic=settings.deterministic)
+        flat, arena = project_bwd(table, params, cs, records, radii, v_records, make_views=want_param_grads, out=grad_out,
+                                  chunk_ranges=chunk_ranges, after_range=after_range)
+    if v_scale_reg is not None:
+        scale_reg_bwd(table, arena, scale_reg, v_scale_reg)
     holder = _Holder()
     holder.records, holder.radii, holder.num_tiles_hit, holder.M = records, radii, tiles_hit, M
     holder.xys, holder.conics, holder.depths = records[:, 0:2], records[:, 2:5], records[:, 9]
@@ -877,6 +963,8 @@ def forward_backward(frame: Frame, settings: RenderSettings, cotangents: Dict[st
     holder.param_grads = flat
     holder.tile_bins, holder.tile_depth = tile_bins, out["tile_depth"]  # diagnostics (tools/depth_stats.py)
     res = {k: out[k] for k in ("rgb", "accumulation", "depth", "object_acc", "background_acc") if k in out}
+    if scale_reg is not None:
+        res["scale_reg"] = reg
     return res, holder
 
 
@@ -918,8 +1006,16 @@ def blend_extra_bwd(cs, bo, records, sorted_ids, tile_bins, final_T, final_idx, 
 
 def render_frame(frame: Frame, settings: Optional[RenderSettings] = None, sky: Optional[torch.Tensor] = None,
                  grad_sink=None, anchor: Optional[torch.Tensor] = None, extra: Optional[torch.Tensor] = None,
-                 pose: Optional[torch.Tensor] = None, view: Optional[torch.Tensor] = None):
+                 pose: Optional[torch.Tensor] = None, view: Optional[torch.Tensor] = None, scale_reg: Optional[float] = None):
     """Render one camera.  Returns (outputs dict, holder).  Segment parameters must be CUDA tensors.
+
+    ``scale_reg`` (max_ratio; None = off, and the call sequence is unchanged): ``out["scale_reg"]`` is nerfstudio's scale
+    regularisation over the frame's rows, 0.1 * mean(max(amax(s) / amin(s), max_ratio) - max_ratio) with s = exp(scales), a
+    0-d device tensor (sgn_scale_reg_fwd).  It is an output of the render node rather than a function of its own because
+    project_bwd OVERWRITES the gradient arena: as an output, the render's backward waits for the term's cotangent and adds
+    its gradient (sgn_scale_reg_bwd) into the arena after project_bwd, before the arena is handed on.  When the term is the
+    only output with a cotangent (nothing in view, or a backward of the term alone) the blend and projection backward are
+    skipped and the arena holds zeros plus the term's gradient.
 
     ``view`` [15] (float32, on the device): the world->camera view to project with -- viewmat 3x4 row-major, then cam_pos
     (the SH view directions' origin) -- in place of the one ``frame.camera`` gives; intrinsics and image size still come
@@ -947,7 +1043,10 @@ def render_frame(frame: Frame, settings: Optional[RenderSettings] = None, sky: O
     holder = _Holder()
     holder.grad_sink = grad_sink
     flat = [anchor] if grad_sink is not None else [t for seg in frame.segments for t in seg.params.tensors()]
-    outs = _SceneGraphRasterize.apply(frame, settings, holder, sky, extra, pose, view, *flat)
+    outs = _SceneGraphRasterize.apply(frame, settings, holder, sky, extra, pose, view, scale_reg, *flat)
+    reg = None
+    if scale_reg is not None:
+        outs, reg = outs[:-1], outs[-1]
     extra_img = None
     if extra is not None:
         outs, extra_img = outs[:-1], outs[-1]
@@ -955,6 +1054,8 @@ def render_frame(frame: Frame, settings: Optional[RenderSettings] = None, sky: O
     out = {k: t for k, t in zip(names, outs)}
     if extra_img is not None:
         out["extra"] = extra_img
+    if reg is not None:
+        out["scale_reg"] = reg
     if sky is not None:
         out["sky"] = sky
     return out, holder

@@ -24,7 +24,7 @@ import torch.distributed as dist
 from . import dp
 from .model import SceneGraphRasterModel, _FullArenaSink
 from .optim import FusedAdam
-from .scene import Camera
+from .scene import PARAM_NAMES, Camera
 
 
 class TrainStep:
@@ -92,6 +92,11 @@ class TrainStep:
         if world > 1 and (m.config.semantic_classes > 0 or opt.row_tensors()):
             raise NotImplementedError("data-parallel training does not exchange the gradients of the semantic logits: the "
                                       "replicas would diverge")
+        if world > 1 and m.config.use_scale_regularization:
+            # the term's gradient reaches background rows no replica saw, which the exchange leaves out, and every replica
+            # would normalise by its own visible row count
+            raise NotImplementedError("data-parallel training does not exchange the gradient of the scale regularisation: the "
+                                      "replicas would diverge")
         if world > 1:
             self._ensure_exchange()
         m.step = step                                     # step_cb (sgn_splatfacto.py:754-755)
@@ -120,13 +125,25 @@ class TrainStep:
         losses = m.get_loss_dict(out, batch)
         total = sum(losses.values())
         rendered = isinstance(total, torch.Tensor) and total.requires_grad
+        kinds = None  # which of the six tensors of a sub-model have a gradient (None: all of them)
         if rendered:
             total.backward()
+            h, sink = m._holder, getattr(m, "_grad_sink", None)
+            # a loss term of the parameters themselves (the scale regularisation with fused_loss=False) sets .grad before the
+            # render's backward runs: the render then adds its share into .grad through a temporary arena, and the arena the
+            # optimizer reads is rebuilt from .grad
+            outside = (sink is not None and getattr(h, "grad_sink", None) is sink and h.table is not None
+                       and (h.grad_arena is None or h.grad_arena is not sink.arena) and any(p.grad is not None for p in sink.params))
+            if outside:
+                arena, got = sink.collect(h.table.static, m.device)
+                kinds = None if len(got) == 6 else got
+            elif h is not None and h.grad_arena is not None:
+                arena = h.grad_arena
+                if getattr(h, "params_only", False):  # only the scale regularisation reached the render (nothing in view): only the scales step
+                    kinds = [PARAM_NAMES.index("scales")]
             # with nothing in view a loss term of another tensor (the camera regulariser) can still carry a gradient
-            rendered = m._holder is not None and m._holder.grad_arena is not None
-        if rendered:
-            arena = m._holder.grad_arena
-        else:
+            rendered = outside or (h is not None and h.grad_arena is not None)
+        if not rendered:
             # nothing in view on this replica (the reference's early-out, sgn_splatfacto.py:878-886): no gradient here.
             # A single replica skips backward / optimizer / after_train only: the refinement callbacks still run
             # (nerfstudio fires them on the step count, whatever was rendered)
@@ -158,12 +175,16 @@ class TrainStep:
         else:
             if world > 1:
                 dp.allreduce_gradients(arena, average=True, group=self.group)
+            kw = {"kinds": kinds} if kinds is not None else {}
             if row_grads:
                 opt.step(arena, present=None if everything else present, full_layout=full, extra_grads=extra_grads or None,
-                         row_grads=row_grads)
+                         row_grads=row_grads, **kw)
             else:
-                opt.step(arena, present=None if everything else present, full_layout=full, extra_grads=extra_grads or None)
-        if rendered:
+                opt.step(arena, present=None if everything else present, full_layout=full, extra_grads=extra_grads or None, **kw)
+        # a frame with nothing in view (rendered only for the scale regularisation's gradient) has no densification statistics;
+        # a count left on the device (async binning) is not read back for this
+        M = getattr(m._holder, "M", None)
+        if rendered and not (type(M) is int and M == 0):
             m.after_train(step)                           # AFTER_TRAIN_ITERATION callbacks, in the reference's order
         self._maybe_refine(step)
         return losses

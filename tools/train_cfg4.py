@@ -27,7 +27,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         actor_range: float = 45.0, pipeline_chunks: int = 0, overlap: bool = False, resident_table: bool = True,
         async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True, sky: bool = False, metrics: bool = False,
         bbox_opt: bool = False, camera_opt: bool = False, sky_view_grad: bool = False, lidar_depth: float = 0.0,
-        semantic: float = 0.0, antialiased: bool = False) -> dict:
+        semantic: float = 0.0, antialiased: bool = False, scale_reg: bool = False) -> dict:
     """One measurement.  torch.distributed must already be initialised when WORLD_SIZE > 1.  Returns the result dict on
     rank 0 (None elsewhere).  ``sky``: the reference's default learnable sky (use_sky_sphere, a 1024^2 cube map stepped by
     the same Adam launch at the ``sky_sphere`` group's lr 0.005, sgn_config.py:72-75).  ``metrics``: every step also computes
@@ -44,7 +44,9 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     are the FusedAdam row group "semantic" at features_dc's lr 0.0025 (a choice: the reference config names no rate) with
     the reference's gradient accumulation of 10
     projected with the step's camera.  ``antialiased``: rasterize_mode "antialiased" (the opacity scaled by the blur
-    compensation, forward and backward)."""
+    compensation, forward and backward).  ``scale_reg``: nerfstudio's scale regularisation (use_scale_regularization,
+    max_gauss_ratio 10, every tenth step); the result then reports the fraction of rows whose max / min scale ratio is above
+    10 before and after the run."""
     import torch
     import torch.distributed as dist
 
@@ -75,7 +77,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                            object_refine=RefineSettings(refine_every=refine_every, cull_alpha_thresh=0.005),
                            num_train_data=len(cams), refine_record=True, depth_loss_mult=lidar_depth,
                            semantic_classes=3 if semantic > 0 else 0, semantic_loss_mult=semantic,
-                           rasterize_mode="antialiased" if antialiased else "classic")
+                           rasterize_mode="antialiased" if antialiased else "classic", use_scale_regularization=scale_reg)
     env_map = None
     if sky:
         from street_gaussians_ns_b200.sky import CubeMapSky
@@ -111,6 +113,12 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     g = torch.Generator().manual_seed(5)
     gt = (torch.rand(H, W, 3, generator=g) * 255).to(torch.uint8).to(dev)  # get_loss_dict consumes uint8 directly
     counts0 = [sub.num_points for sub in model.all_models.values()]
+
+    def needle_fraction():  # rows whose max / min scale ratio is above max_gauss_ratio, over every sub-model
+        with torch.no_grad():
+            s = torch.exp(torch.cat([sub.gauss_params["scales"] for sub in model.all_models.values()]))
+            return float(((s.amax(-1) / s.amin(-1)) > cfg.max_gauss_ratio).float().mean())
+    needles0 = needle_fraction()
     times = [float(f) for f in range(num_frames)]
     if resident_table:
         model.prepare_frames(times)
@@ -236,6 +244,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                    **({"semantic": f"3 classes, semantic_loss_mult {semantic}, Adam lr 0.0025, gradient accumulation 10, synthetic labels"}
                       if semantic > 0 else {}),
                    **({"rasterize_mode": "antialiased"} if antialiased else {}),
+                   **({"scale_reg": "use_scale_regularization, max_gauss_ratio 10, every tenth step"} if scale_reg else {}),
                    "loss": "fused kernels" if fused_loss else "torch ops", "metrics": "get_metrics_dict every step" if metrics else "none",
                    "start_step": start_step, "refine_every": refine_every,
                    "refinement_kernels_loaded_before_timing": refine_warm,
@@ -247,6 +256,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         "gaussians_before": int(sum(counts0)), "gaussians_after": int(sum(counts1)),
         "submodels_changed": int(sum(a != b for a, b in zip(counts0, counts1))),
         "loss_first": first, "loss_last": last, "replicas_identical": replicas_identical,
+        "ratio_above_10_before": needles0, "ratio_above_10_after": needle_fraction(),
         **({"metrics_last": {k: (v if isinstance(v, int) else float(v)) for k, v in step_fn.metrics.items()}} if metrics else {}),
         "step_ms_rank0": step_ms, "host_ms_rank0": [round(x, 3) for x in host_ms]}
 
@@ -274,6 +284,7 @@ def main():
     ap.add_argument("--semantic", type=float, default=0.0, metavar="W",
                     help="> 0: 3-class semantic logits and the cross-entropy term at weight W against synthetic labels")
     ap.add_argument("--antialiased", action="store_true", help="rasterize_mode 'antialiased': opacities scaled by the blur compensation")
+    ap.add_argument("--scale-reg", action="store_true", help="nerfstudio's scale regularisation (max_gauss_ratio 10, every tenth step)")
     args = ap.parse_args()
     if args.sky_view_grad and not (args.sky and args.camera_opt):
         ap.error("--sky-view-grad needs --sky and --camera-opt")
@@ -289,7 +300,8 @@ def main():
     res = run(args.steps, args.warmup, args.scale, args.refine_every, args.start_step, args.actor_range, args.pipeline_chunks,
               args.overlap, not args.host_table, ssim_lambda=args.ssim_lambda, fused_loss=not args.torch_loss, sky=args.sky,
               metrics=args.metrics, bbox_opt=args.bbox_opt, camera_opt=args.camera_opt,
-              sky_view_grad=args.sky_view_grad, lidar_depth=args.lidar_depth, semantic=args.semantic, antialiased=args.antialiased)
+              sky_view_grad=args.sky_view_grad, lidar_depth=args.lidar_depth, semantic=args.semantic, antialiased=args.antialiased,
+              scale_reg=args.scale_reg)
     if res is not None:
         print(json.dumps(res))
     if world > 1:
