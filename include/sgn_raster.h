@@ -46,6 +46,7 @@ typedef enum sgn_status {
  *   [2] a  [3] b  [4] c     conic (inverse cov2d)   == `conics`
  *   [5] opacity             sigmoid(logit)          (sgn_splatfacto.py:946-949)
  *                           antialiased mode: sigmoid(logit) * comp
+ *                           with a 3D filter (sgn_camera.filter_3d): sigmoid(logit) * coef [* comp]
  *   [6] r  [7] g  [8] b     clamp(SH+0.5, min 0)    (sgn_splatfacto.py:939-940)
  *   [9] depth               view-space z            == `depths`
  *   [10] aux (int bits)     bits 0-2: colour clamp pass mask, bit 3: object class, bit 4: visible
@@ -100,6 +101,10 @@ typedef struct sgn_camera {
     int32_t antialiased;      /* rasterize_mode (sgn_splatfacto.py:214-223): 0 "classic", 1 "antialiased" -- the record's
                                  opacity is scaled by the blur compensation, forward and backward (gsplat's antialiased
                                  mode; the reference leaves the multiply commented out, :946-949) */
+    const float* const* filter_3d; /* NULL: off.  Otherwise a DEVICE array of nseg pointers, one per segment of the table the
+                                      call is given, each to that segment's count per-row 3D filter sizes sigma (Mip-Splatting's
+                                      3D smoothing filter, sgn_filter3d): the projection uses s' = sqrt(s^2 + sigma^2) and scales
+                                      the opacity by coef = prod_k sqrt(s_k^2 / (s_k^2 + sigma^2)), forward and backward */
 } sgn_camera;
 
 /* Blend settings. */
@@ -155,7 +160,12 @@ int sgn_upload(const void* host, size_t bytes, void* dev, void* stream);
  * cam->antialiased: record [5] is sigmoid(logit) * comp and [11] is comp (layout above), and the touch test uses that
  * opacity, tau = ln(255 o comp), so a row with comp == 0 reaches no tile.  The backward (every form below, with the same
  * camera) then sends the opacity cotangent to the logit as v * comp * s (1 - s) and, through comp, to cov2d and from
- * there to means, scales, quats and the pose / view partials. */
+ * there to means, scales, quats and the pose / view partials.
+ * cam->filter_3d (non-NULL): every row i of segment k is projected with the scales s' = sqrt(s^2 + sigma^2), sigma =
+ * cam->filter_3d[k][i], and its opacity is multiplied by coef = prod_k sqrt(r_k), r_k = s_k^2 / (s_k^2 + sigma^2) (then by comp
+ * in the antialiased mode, computed from the filtered covariance).  sigma is a constant: the backward sends the scales' cotangent
+ * through d log s' / d log s = r and d coef / d log s_k = coef (1 - r_k), with coef recomputed from the parameters and sigma, and
+ * the opacity cotangent to the logit as v * coef [* comp] * s (1 - s).  NULL: the outputs are those of a camera without the field. */
 int sgn_project_fwd(const sgn_segment* segs_dev, int nseg, int N, int num_chunks, const sgn_camera* cam,
                     float* records, int32_t* radii, int32_t* num_tiles_hit, uint16_t* tile_bbox,
                     int32_t* tiles_touched, uint32_t* touch_mask, void* stream);
@@ -686,6 +696,35 @@ int sgn_scale_reg_fwd(const sgn_segment* table_dev, int nseg, int N, int num_chu
                       size_t scratch_bytes, void* stream);
 int sgn_scale_reg_bwd(const sgn_segment* table_dev, const sgn_segment_grads* grads_dev, int nseg, int N, int num_chunks, float max_ratio,
                       const float* v_out, void* stream);
+
+/* ---- 3D smoothing filter sizes (Mip-Splatting, Yu et al. 2024, eq. 7: compute_3D_filter)
+ * For every row i of sub-model m (nsub sub-models; subs_dev[m] = its means [count,3], its output sigma [count], its count and
+ * its first 128-row chunk, chunk0 = sum over earlier sub-models of ceil(count/128); num_chunks the total):
+ *   nu_i = max over views v with xforms[v * nsub + m].present of max(fx, fy) / z, over the views where
+ *          p = M[0:3,0:3] mu_i + M[:,3] (M = xforms[v * nsub + m].M, row-major 3x4, object -> camera) has z > near and
+ *          u = fx x / z + cx in [-0.15 W, 1.15 W], w = fy y / z + cy in [-0.15 H, 1.15 H] (bounds inclusive);
+ *   sigma_i = sqrt(variance) / nu_i.
+ * Rows no view samples get the largest sigma of the sampled rows; with none sampled, every sigma is 0.  The transform and tests
+ * are evaluated in fp64.  stats (device, 2 x int32, overwritten): [0] the number of sampled rows, [1] the bits of the largest
+ * sampled sigma.  No float atomics, no host synchronisation: two launches and one memset. */
+typedef struct sgn_filter_view {
+    float fx, fy, cx, cy;
+    int32_t width, height;
+} sgn_filter_view;
+typedef struct sgn_filter_xform {
+    double M[12];    /* object -> camera: the view matrix composed with the sub-model's object -> world pose at the view's time */
+    int32_t present; /* 0: the sub-model is not in this view (an actor without a box at the view's timestamp) */
+    int32_t pad;
+} sgn_filter_xform;
+typedef struct sgn_filter_sub {
+    const float* means; /* [count,3] */
+    float* out;         /* [count] sigma */
+    int32_t count;
+    int32_t chunk0;
+} sgn_filter_sub;
+size_t sgn_sizeof_filter_xform(void);
+int sgn_filter3d(const sgn_filter_sub* subs_dev, int nsub, int num_chunks, const sgn_filter_view* views_dev, int V,
+                 const sgn_filter_xform* xforms_dev, double variance, double near, int32_t* stats, void* stream);
 
 #ifdef __cplusplus
 }

@@ -46,7 +46,21 @@ class CameraStruct(C.Structure):
         ("block_width", C.c_int32),
         ("sh_degree", C.c_int32), ("sh_degree_to_use", C.c_int32),
         ("antialiased", C.c_int32),  # rasterize_mode: 0 classic (zero-initialised), 1 antialiased
+        ("filter_3d", C.c_void_p),   # device array of per-segment 3D filter pointers; NULL (zero-initialised) = off
     ]
+
+
+class FilterView(C.Structure):
+    _fields_ = [("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float),
+                ("width", C.c_int32), ("height", C.c_int32)]
+
+
+class FilterXform(C.Structure):
+    _fields_ = [("M", C.c_double * 12), ("present", C.c_int32), ("pad", C.c_int32)]
+
+
+class FilterSub(C.Structure):
+    _fields_ = [("means", C.c_void_p), ("out", C.c_void_p), ("count", C.c_int32), ("chunk0", C.c_int32)]
 
 
 class BlendOpts(C.Structure):
@@ -141,7 +155,7 @@ EXPORTS = [
     "sgn_sky_rot_scratch_bytes", "sgn_sky_bwd_view_rot", "sgn_sky_bwd_det_view_rot", "sgn_knn_scratch_bytes", "sgn_knn",
     "sgn_lidar_depth_map", "sgn_depth_scratch_bytes", "sgn_depth_loss_fwd", "sgn_depth_loss_bwd", "sgn_depth_metrics",
     "sgn_semantic_scratch_bytes", "sgn_semantic_loss_fwd", "sgn_semantic_loss_bwd", "sgn_semantic_metrics", "sgn_refine_carry",
-    "sgn_scale_reg_scratch_bytes", "sgn_scale_reg_fwd", "sgn_scale_reg_bwd",
+    "sgn_scale_reg_scratch_bytes", "sgn_scale_reg_fwd", "sgn_scale_reg_bwd", "sgn_sizeof_filter_xform", "sgn_filter3d",
 ]
 VIEW_FLOATS = 12  # SGN_VIEW_FLOATS: the view's cotangent, viewmat[12] row-major; the device view itself is 12 + 3 (cam_pos) floats
 POSE_FLOATS = 16  # SGN_POSE_FLOATS: a segment's pose (and its cotangent) as R[9] row-major, t[3], q[4]
@@ -163,8 +177,10 @@ def load():
     L.sgn_last_error.restype = C.c_char_p
     L.sgn_abi_version.restype = C.c_int
     L.sgn_launch_count.restype = C.c_longlong
-    for f in ("sgn_sizeof_segment", "sgn_sizeof_segment_grads", "sgn_sizeof_camera"):
+    for f in ("sgn_sizeof_segment", "sgn_sizeof_segment_grads", "sgn_sizeof_camera", "sgn_sizeof_filter_xform"):
         getattr(L, f).restype = sz
+    L.sgn_filter3d.argtypes = [vp, i32, i32, vp, i32, vp, C.c_double, C.c_double, vp, vp]
+    L.sgn_filter3d.restype = C.c_int
     L.sgn_upload.argtypes = [vp, sz, vp, vp]
     L.sgn_project_fwd.argtypes = [vp, i32, i32, i32, C.POINTER(CameraStruct), vp, vp, vp, vp, vp, vp, vp]
     L.sgn_project_bwd.argtypes = [vp, vp, i32, i32, i32, C.POINTER(CameraStruct), vp, vp, vp, vp]

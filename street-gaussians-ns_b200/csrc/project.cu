@@ -127,8 +127,10 @@ project_fwd_direct_kernel(const sgn_segment* __restrict__ segs, int nseg, const 
         const float4 qq = __ldg(reinterpret_cast<const float4*>(sg.quats) + i);
         q[0] = qq.x; q[1] = qq.y; q[2] = qq.z; q[3] = qq.w;
     }
+    const bool filt = cam.filter_3d != nullptr;  // uniform: the 3D smoothing filter
+    const float sigma = filt ? __ldg(cam.filter_3d[si] + i) : 0.f;
     SgnProj st;
-    vis = sgn_project_exact(sg, cam, m, ls, q, st, true, 1.f, cam.antialiased != 0);
+    vis = sgn_project_exact(sg, cam, m, ls, q, st, true, 1.f, cam.antialiased != 0, filt, sigma);
 
     float rgb[3] = {0.f, 0.f, 0.f};
     float opac = 0.f, comp = 0.f;
@@ -165,6 +167,7 @@ project_fwd_direct_kernel(const sgn_segment* __restrict__ segs, int nseg, const 
             for (int ch = 0; ch < 3; ++ch) { rgb[ch] = 1.f / (1.f + expf(-c0[ch])); aux |= (1 << ch); }
         }
         opac = 1.f / (1.f + expf(-__ldg(sg.opacities + i)));
+        if (filt) opac = opac * st.coef;
         if (cam.antialiased) {  // warp-uniform
             comp = st.comp;
             opac = opac * comp;
@@ -209,7 +212,7 @@ project_fwd_staged_kernel(const sgn_segment* __restrict__ segs, int nseg, const 
     __shared__ __align__(16) float s_dc[CH * MAX_DC];
     __shared__ __align__(16) float s_means[CH * 3];
     __shared__ __align__(16) float s_scales[CH * 3];
-    __shared__ float s_geo[CH][10];  // per visible row (compact index): xy, conic, depth, world mean, comp
+    __shared__ float s_geo[CH][11];  // per visible row (compact index): xy, conic, depth, world mean, comp, filter coef
     __shared__ int s_row[CH];       // compact index -> row of the chunk
     __shared__ int s_warp_base[CH / 32 + 1];
     for (int i = threadIdx.x; i < nseg; i += blockDim.x) s_chunk0[i] = segs[i].chunk0;
@@ -236,7 +239,9 @@ project_fwd_staged_kernel(const sgn_segment* __restrict__ segs, int nseg, const 
         const float ls[3] = {s_scales[3 * tid], s_scales[3 * tid + 1], s_scales[3 * tid + 2]};
         const float4 qq = __ldg(reinterpret_cast<const float4*>(sg.quats) + r0 + tid);
         const float q[4] = {qq.x, qq.y, qq.z, qq.w};
-        vis = sgn_project_exact(sg, cam, m, ls, q, st, true, 1.f, cam.antialiased != 0);
+        const bool filt = cam.filter_3d != nullptr;  // uniform: the 3D smoothing filter
+        const float sigma = filt ? __ldg(cam.filter_3d[si] + r0 + tid) : 0.f;
+        vis = sgn_project_exact(sg, cam, m, ls, q, st, true, 1.f, cam.antialiased != 0, filt, sigma);
         radii[g] = st.radius;
         num_tiles_hit[g] = vis ? (st.tmax[0] - st.tmin[0]) * (st.tmax[1] - st.tmin[1]) : 0;
         tile_bbox[g] = make_ushort4((unsigned short)st.tmin[0], (unsigned short)st.tmin[1],
@@ -268,6 +273,7 @@ project_fwd_staged_kernel(const sgn_segment* __restrict__ segs, int nseg, const 
         ge[0] = st.xy[0]; ge[1] = st.xy[1]; ge[2] = st.conic[0]; ge[3] = st.conic[1]; ge[4] = st.conic[2];
         ge[5] = st.pv[2]; ge[6] = st.mw[0]; ge[7] = st.mw[1]; ge[8] = st.mw[2];
         ge[9] = st.comp;
+        ge[10] = st.coef;
     }
     __syncthreads();
     if (nvis == 0) return;
@@ -345,6 +351,7 @@ project_fwd_staged_kernel(const sgn_segment* __restrict__ segs, int nseg, const 
             for (int ch = 0; ch < 3; ++ch) { rgb[ch] = 1.f / (1.f + expf(-c0[ch])); aux |= (1 << ch); }
         }
         float opac = 1.f / (1.f + expf(-__ldg(sg.opacities + r0 + row)));
+        if (cam.filter_3d) opac = opac * ge[10];   // uniform
         if (cam.antialiased) opac = opac * ge[9];  // warp-uniform
         float4* rec = records + 3 * gb;
         rec[1] = make_float4(ge[4], opac, rgb[0], rgb[1]);
@@ -595,7 +602,8 @@ project_bwd_kernel(const sgn_segment* __restrict__ segs, const sgn_segment_grads
         const float v_depth = v2.y;
         const float4 r1 = records[3 * g + 1], r2 = records[3 * g + 2];
         const int aux = __float_as_int(r2.z);
-        if (!cam.antialiased) {  // opacity: sigmoid backward (the antialiased mode's below)
+        const bool filt = cam.filter_3d != nullptr;  // uniform: the 3D smoothing filter
+        if (!cam.antialiased && !filt) {  // opacity: sigmoid backward (the antialiased mode's and the filter's below)
             const float o = r1.y;
             gr.opacities[i] = v_opac * o * (1.f - o);
         }
@@ -606,8 +614,9 @@ project_bwd_kernel(const sgn_segment* __restrict__ segs, const sgn_segment_grads
             const float4 qq = __ldg(reinterpret_cast<const float4*>(sg.quats) + i);
             q[0] = qq.x; q[1] = qq.y; q[2] = qq.z; q[3] = qq.w;
         }
+        const float sigma = filt ? __ldg(cam.filter_3d[si] + i) : 0.f;
         SgnProj st;
-        const bool vis = sgn_project_exact(sg, cam, m, ls, q, st);
+        const bool vis = sgn_project_exact(sg, cam, m, ls, q, st, true, 1.f, false, filt, sigma);
         // colour backward (compute_sh_backward + clamp mask + Fourier DC) into the staging rows
         {
             float vc[3];
@@ -643,18 +652,36 @@ project_bwd_kernel(const sgn_segment* __restrict__ segs, const sgn_segment_grads
         }
         // antialiased mode: record [5] = s comp with s = sigmoid(logit) and comp in record [11]; v_comp = v_opac s goes on
         // through cov2d (sgn_project_vjp)
-        float v_comp = 0.f, comp = 0.f;
-        if (cam.antialiased) {  // warp-uniform
+        // 3D filter: record [5] = s coef [comp]; v_coef = v_opac s [comp] reaches the log-scales through coef, and the scales'
+        // cotangent passes d s' / d log s = r s' (coef and r recomputed from the parameters and sigma, as the forward has them)
+        float v_comp = 0.f, comp = 0.f, v_coef = 0.f;
+        if (cam.antialiased || filt) {  // warp-uniform
             const float s = 1.f / (1.f + expf(-__ldg(sg.opacities + i)));  // the forward's sigmoid, not record [5]
-            v_comp = v_opac * s;
-            gr.opacities[i] = v_opac * r2.w * s * (1.f - s);
-            comp = __ldg(reinterpret_cast<const float*>(records) + 12 * g + 11);  // read again here: nothing stays live
+            float f = 1.f;  // the factors of the opacity beyond the sigmoid
+            if (cam.antialiased) {
+                v_comp = v_opac * s;
+                f = r2.w;
+                comp = __ldg(reinterpret_cast<const float*>(records) + 12 * g + 11);  // read again here: nothing stays live
+            }
+            if (filt) {
+                v_coef = v_opac * s * f;
+                v_comp = v_comp * st.coef;
+                f = f * st.coef;
+            }
+            gr.opacities[i] = v_opac * f * s * (1.f - s);
         }
         if (vis && radii[g] > 0) {
             float vmw[3], vs[3], vqr[4];
             sgn_project_vjp<VIEW>(cam, st, v_xy, v_depth, v_conic, vmw, vs, vqr, vv, cam.antialiased != 0, comp, v_comp);
 #pragma unroll
             for (int c = 0; c < 3; ++c) gs[c] = vs[c] * st.s[c];  // through exp
+            if (filt) {
+                float r[3];
+                sgn_filter_ratios(ls, sigma, r);
+                const float vc = v_coef * st.coef;
+#pragma unroll
+                for (int c = 0; c < 3; ++c) gs[c] = gs[c] * r[c] + vc * (1.f - r[c]);
+            }
             if (sg.has_pose) {
                 const float* R = sg.R;
 #pragma unroll

@@ -25,6 +25,7 @@ struct SgnProj {
     float T[6];
     float a, b, c;
     float comp;  // blur compensation (sgn_compensation), when sgn_project_exact was asked for it; 0 otherwise
+    float coef;  // opacity factor of the 3D smoothing filter (sgn_filter_coef), when asked for; 1 otherwise
     float conic[3];
     float xy[2];
     int radius;
@@ -93,14 +94,43 @@ __device__ __forceinline__ void sgn_cov2d_blur(const xf T[6], const xf S[6], xf&
 
 __device__ __forceinline__ float sgn_compensation(const SgnProj& st);
 
+// ---- 3D smoothing filter (Mip-Splatting): s' = sqrt(s^2 + sigma^2) on one axis, and r = s^2 / (s^2 + sigma^2) ----------------
+// Individually rounded (xf), so that the forward and the backward (which recomputes r from the parameters) get the same bits.
+// s^2 + sigma^2 == 0 (sigma 0 and s^2 below the smallest float) keeps r = 1: the filter is then the identity.
+__device__ __forceinline__ xf sgn_filter_axis(xf s, xf sigma, xf& r) {
+    const xf s2 = s * s;
+    const xf v = s2 + sigma * sigma;
+    r = v.v > 0.f ? s2 / v : xf(1.f);
+    return xsqrt(v);
+}
+
+// coef = prod_k sqrt(r_k), the filter's opacity factor, as a product of per-axis ratios: prod s^2 / prod (s^2 + sigma^2)
+// underflows in fp32 for small scales
+__device__ __forceinline__ float sgn_filter_coef(const float r[3]) {
+    return ((xsqrt(xf(r[0])) * xsqrt(xf(r[1]))) * xsqrt(xf(r[2]))).v;
+}
+
+// the ratios r_k of the log-scales ls (the model's parameters) under the filter sigma, recomputed as sgn_project_exact does
+__device__ __forceinline__ void sgn_filter_ratios(const float ls[3], float sigma, float r[3]) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        xf rk;
+        sgn_filter_axis(xf(sgn_expf_exact(ls[k])), xf(sigma), rk);
+        r[k] = rk.v;
+    }
+}
+
 // Returns st.visible.  `m`, `ls`, `q` are this Gaussian's raw parameters.
 // log_scales: `ls` holds log-scales (the model's parameters) -> exp is applied here; otherwise `ls` holds
 // activated scales (gsplat's project_gaussians argument) multiplied by glob_scale.
 // with_comp (warp-uniform): also st.comp = sgn_compensation(st), computed here while its inputs are live.
+// with_filter (warp-uniform): the 3D smoothing filter of size `sigma` -- st.s and the covariance use s' = sqrt(s^2 + sigma^2),
+// and st.coef = sgn_filter_coef of the ratios (1 otherwise).
 __device__ __forceinline__ bool sgn_project_exact(const sgn_segment& sg, const sgn_camera& cam, const float m_[3],
                                                   const float ls[3], const float q_[4], SgnProj& st,
                                                   const bool log_scales = true, const float glob_scale = 1.f,
-                                                  const bool with_comp = false) {
+                                                  const bool with_comp = false, const bool with_filter = false,
+                                                  const float sigma = 0.f) {
     xf W[12];
 #pragma unroll
     for (int k = 0; k < 12; ++k) W[k] = xf(cam.viewmat[k]);
@@ -111,6 +141,7 @@ __device__ __forceinline__ bool sgn_project_exact(const sgn_segment& sg, const s
     st.tmin[0] = st.tmin[1] = st.tmax[0] = st.tmax[1] = 0;
     st.clampx = st.clampy = 0;
     st.comp = 0.f;
+    st.coef = 1.f;
     const xf m[3] = {xf(m_[0]), xf(m_[1]), xf(m_[2])};
     xf mw[3], qr[4];
     if (sg.has_pose) {
@@ -151,10 +182,19 @@ __device__ __forceinline__ bool sgn_project_exact(const sgn_segment& sg, const s
     }
     xf sc[3];
 #pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        sc[k] = log_scales ? xf(sgn_expf_exact(ls[k])) : xf(ls[k]) * xf(glob_scale);
-        st.s[k] = sc[k].v;
+    for (int k = 0; k < 3; ++k) sc[k] = log_scales ? xf(sgn_expf_exact(ls[k])) : xf(ls[k]) * xf(glob_scale);
+    if (with_filter) {
+        float r[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            xf rk;
+            sc[k] = sgn_filter_axis(sc[k], xf(sigma), rk);
+            r[k] = rk.v;
+        }
+        st.coef = sgn_filter_coef(r);
     }
+#pragma unroll
+    for (int k = 0; k < 3; ++k) st.s[k] = sc[k].v;
     xf S[6];
     {
         const xf w = qn[0], x = qn[1], y = qn[2], z = qn[3];

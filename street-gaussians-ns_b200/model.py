@@ -92,6 +92,16 @@ class SceneGraphConfig:
     # by default; the 0.1 weight and the 10-step cadence are nerfstudio's constants
     use_scale_regularization: bool = False
     max_gauss_ratio: float = 10.0
+    # Mip-Splatting's 3D smoothing filter (filter3d.py): every Gaussian is rendered convolved with an isotropic 3D Gaussian whose
+    # size comes from the highest rate at which a training camera sampled it, sigma = sqrt(filter_3d_variance) / max(f / z),
+    # over the views where z > filter_3d_near and the projection is inside the image with a 15 % margin.  The sizes are a
+    # per-sub-model buffer (``filter_3d``, in the state dict only with the filter on) that ``compute_filter_3d`` fills;
+    # TrainStep(filter_cameras=...) recomputes it after every refinement that changed a row count and every filter_3d_every
+    # steps.  The refinement, densification statistics, metrics and scale regularisation keep reading the raw parameters
+    filter_3d: bool = False
+    filter_3d_variance: float = 0.2
+    filter_3d_near: float = 0.2
+    filter_3d_every: int = 100
 
     # ``stop_split_at`` of the BACKGROUND sub-model: what the reference's entropy gate reads
     # (``config.background_model.stop_split_at``, scene graph :386).  One source: ``refine.stop_split_at``.
@@ -153,7 +163,7 @@ class GaussianSubModel(torch.nn.Module):
     conics = _FrameSlice("conics")
     num_tiles_hit = _FrameSlice("num_tiles_hit")
 
-    def __init__(self, params: GaussianSet, semantic_classes: int = 0):
+    def __init__(self, params: GaussianSet, semantic_classes: int = 0, filter_3d: bool = False):
         super().__init__()
         self.gauss_params = torch.nn.ParameterDict(
             {k: torch.nn.Parameter(getattr(params, k).detach().clone()) for k in
@@ -166,6 +176,12 @@ class GaussianSubModel(torch.nn.Module):
                                                                   device=params.means.device, dtype=torch.float32))
         else:
             self.semantic_logits = None
+        # the 3D smoothing filter's per-row sizes [n] (SceneGraphConfig.filter_3d): a buffer, so it is saved with the model;
+        # zeros (no smoothing) until SceneGraphRasterModel.compute_filter_3d fills it
+        if filter_3d:
+            self.register_buffer("filter_3d", torch.zeros(params.means.shape[0], device=params.means.device, dtype=torch.float32))
+        else:
+            self.filter_3d = None
         self.xys = self.depths = self.radii = self.conics = self.num_tiles_hit = None
         self.last_size = None
         # densification statistics (sgn_splatfacto.py:513-541), created by the first after_train
@@ -200,6 +216,10 @@ class GaussianSubModel(torch.nn.Module):
             want = state_dict.get("semantic_logits")
             if sem is not None and want is not None and tuple(sem.shape) != tuple(want.shape):
                 self.semantic_logits = torch.nn.Parameter(torch.zeros(tuple(want.shape), device=sem.device, dtype=sem.dtype))
+            f3 = self.filter_3d
+            want = state_dict.get("filter_3d")
+            if f3 is not None and want is not None and tuple(f3.shape) != tuple(want.shape):
+                self.filter_3d = torch.zeros(tuple(want.shape), device=f3.device, dtype=f3.dtype)
             d = self.__dict__
             d["xys_grad_norm"] = d["vis_counts"] = d["max_2Dsize"] = None  # statistics of the old rows are meaningless
         return super().load_state_dict(state_dict, **kwargs)
@@ -386,9 +406,10 @@ class SceneGraphRasterModel(torch.nn.Module):
         self.bbox_optimizer = bbox_optimizer
         self.all_models = torch.nn.ModuleDict()
         C = int(self.config.semantic_classes)
-        self.all_models["background"] = GaussianSubModel(background, C)
+        f3 = bool(self.config.filter_3d)
+        self.all_models["background"] = GaussianSubModel(background, C, f3)
         for obj_id, ps in actors.items():
-            self.all_models[self.get_object_model_name(obj_id)] = GaussianSubModel(ps, C)
+            self.all_models[self.get_object_model_name(obj_id)] = GaussianSubModel(ps, C, f3)
         self.poses_at = poses_at or (lambda t: [])
         # the learnable sky (EnvLight, sgn_splatfacto.py:109-150): sky.CubeMapSky on this library's kernels, or any callable
         # (camera, train) -> [H, W, 3] such as the reference's EnvLight on nvdiffrast
@@ -410,7 +431,7 @@ class SceneGraphRasterModel(torch.nn.Module):
     @classmethod
     def from_points(cls, background=None, actors: Optional[Dict[str, tuple]] = None, config: Optional[SceneGraphConfig] = None,
                     generator: Optional[torch.Generator] = None, replay_scene_graph_init: bool = True, device=None,
-                    **model_kwargs) -> "SceneGraphRasterModel":
+                    cameras: Optional[Sequence[Camera]] = None, **model_kwargs) -> "SceneGraphRasterModel":
         """A model initialised from seed points, as ``SplatfactoSceneGraphModel.populate_modules`` builds its sub-models
         (sgn_splatfacto_scene_graph.py:49-96, each one by ``SplatfactoModel.populate_modules``, see populate.py).
 
@@ -418,6 +439,9 @@ class SceneGraphRasterModel(torch.nn.Module):
         None for the reference's random initialisation of 50 000 points in a cube of side 10.  ``actors``: ``{track_id:
         (xyz, rgb)}``, one aggregated lidar cloud per tracked actor, with ``config.fourier_features_dim``, in the given order.
         Every sub-model uses ``config.sh_degree``.  The initial scales come from the GPU nearest-neighbour search (knn.py).
+
+        ``cameras`` (a sequence of scene.Camera): with ``config.filter_3d``, the 3D smoothing filter is computed from them once
+        the model is built (``compute_filter_3d``).
 
         Draws come from ``generator`` (default: torch's default CPU generator) in the reference's order.  With
         ``replay_scene_graph_init`` (the default) the draws of the scene graph's own random initialisation, which the reference
@@ -438,7 +462,10 @@ class SceneGraphRasterModel(torch.nn.Module):
         acts = {tid: populate.gaussians_from_points(xyz, rgb, sh_degree=config.sh_degree, fourier_dim=config.fourier_features_dim,
                                                     generator=generator, device=device)
                 for tid, (xyz, rgb) in (actors or {}).items()}
-        return cls(bg, acts, config=config, **model_kwargs)
+        model = cls(bg, acts, config=config, **model_kwargs)
+        if cameras is not None and config.filter_3d:
+            model.compute_filter_3d(cameras)
+        return model
 
     @staticmethod
     def get_object_model_name(object_id) -> str:
@@ -491,6 +518,43 @@ class SceneGraphRasterModel(torch.nn.Module):
         frame = self._build_frame(camera, poses)
         frame._table_slot = self._remember_frame(camera.time, digest, frame, None)
         return frame
+
+    def compute_filter_3d(self, cameras: Sequence[Camera]) -> int:
+        """Mip-Splatting's 3D filter sizes from the training ``cameras`` (filter3d.py, one sweep of every row against every
+        view on the device): fills every sub-model's ``filter_3d`` buffer in place, resizing the ones whose row count changed.
+        Each camera's view is its ``c2w`` as given, actors are placed by ``poses_at(camera.time)`` (box corrections are not
+        applied).  Returns the number of rows some view samples (also kept as ``filter_3d_sampled``); when it is 0, no view
+        sees any Gaussian and every sigma is 0."""
+        from . import filter3d
+        c = self.config
+        if not c.filter_3d:
+            raise ValueError("the model was built without the 3D filter (SceneGraphConfig.filter_3d = False)")
+        resized = False
+        for sub in self.all_models._modules.values():
+            n = sub.num_points
+            if sub.filter_3d is None or sub.filter_3d.shape[0] != n or sub.filter_3d.device != self.device:
+                sub.filter_3d = torch.zeros(n, device=self.device, dtype=torch.float32)
+                resized = True
+        if resized:  # the frames' segments hold the old buffers
+            self.invalidate_frames()
+        n = filter3d.compute(self, list(cameras), c.filter_3d_variance, c.filter_3d_near)
+        self.filter_3d_sampled = n
+        if n == 0:
+            import warnings
+            warnings.warn("compute_filter_3d: no camera samples any Gaussian; every filter size is 0")
+        return n
+
+    def _filter_of(self, name: str) -> Optional[torch.Tensor]:
+        """The sub-model's 3D filter sizes for a frame's segment (None with the filter off)."""
+        if not self.config.filter_3d:
+            return None
+        sub = self.all_models._modules[name]
+        f = sub.filter_3d
+        if f is None or f.shape[0] != sub.num_points:
+            raise RuntimeError(f"the 3D filter of {name} has {None if f is None else f.shape[0]} rows, the sub-model "
+                               f"{sub.num_points}: call compute_filter_3d after changing the rows (TrainStep(filter_cameras=...) "
+                               "does it after every refinement)")
+        return f
 
     def invalidate_frames(self) -> None:
         """Drop the per-timestamp segment rows (call after replacing parameter tensors by hand; ``refinement_after`` and
@@ -547,7 +611,7 @@ class SceneGraphRasterModel(torch.nn.Module):
         return g
 
     def _build_frame(self, camera: Camera, poses) -> Frame:
-        segs = [Segment(self._set_of("background"), CLS_BACKGROUND, name="background")]
+        segs = [Segment(self._set_of("background"), CLS_BACKGROUND, name="background", filter_3d=self._filter_of("background"))]
         names = ["background"]
         kept = []
         for pose in poses:
@@ -561,7 +625,7 @@ class SceneGraphRasterModel(torch.nn.Module):
             if F > 1:
                 t = fourier_time(pose.frame, pose.frame_list, self.config.fourier_features_scale)
                 basis = idft_basis(t, F)
-            segs.append(Segment(ps, CLS_OBJECT, rot=pose.rot, center=pose.center, idft=basis, name=name))
+            segs.append(Segment(ps, CLS_OBJECT, rot=pose.rot, center=pose.center, idft=basis, name=name, filter_3d=self._filter_of(name)))
             names.append(name)
             kept.append(pose)
         self.visible_model_names = names
@@ -864,9 +928,12 @@ class SceneGraphRasterModel(torch.nn.Module):
                         ms, md = adapter.row_moments("semantic", i)
                         refine_carry(p, old_sem[i], new_sem[i], ms, md)
                         subs[i].semantic_logits = torch.nn.Parameter(new_sem[i])
+                    if subs[i].filter_3d is not None:  # sized to the new rows; compute_filter_3d fills it (TrainStep does, next)
+                        subs[i].filter_3d = torch.zeros(p.out_rows, device=self.device, dtype=torch.float32)
             adapter.commit([[sub.gauss_params[k] for k in PARAM_NAMES] for sub in subs], changed,
                            {"semantic": [sub.semantic_logits for sub in subs]} if sem else None)
             self.invalidate_frames()
+        self.__dict__["refine_changed_rows"] = any(p is not None for p in plans)
         for i, st in enumerate(resets):
             if st is not None:  # opacity reset on the survivors (:629-642); the semantic logits are left alone
                 subs[i].gauss_params["opacities"].data.clamp_(max=refine.opacity_reset_logit(st))

@@ -11,6 +11,12 @@ opacity as logit, scales as log, rotation un-normalised wxyz; rows with any non-
 
 A sub-model with semantic logits [n, C] (``SceneGraphConfig.semantic_classes``) appends ``semantic_0..C-1`` after ``rot_3``;
 ``read_semantic`` reads them back.  Files without semantics are byte for byte what they were before.
+
+A model with the 3D smoothing filter (``SceneGraphConfig.filter_3d``) exports either way Mip-Splatting does:
+``filter_3d="bake"`` folds the filter into the parameters -- scales log(sqrt(exp(s)^2 + sigma^2)) and opacity
+logit(sigmoid(o) * coef), coef = prod_k sqrt(exp(s_k)^2 / (exp(s_k)^2 + sigma^2)) -- so that a viewer without the filter
+renders what the model renders with it; ``filter_3d="column"`` writes the raw parameters plus a ``filter_3D`` property,
+which ``read_filter_3d`` reads back.
 """
 from __future__ import annotations
 
@@ -28,8 +34,28 @@ def property_names(n_rest: int, n_semantic: int = 0) -> List[str]:
             + [f"semantic_{i}" for i in range(n_semantic)])
 
 
-def to_columns(params: GaussianSet, semantic: Optional[torch.Tensor] = None) -> Tuple[List[str], np.ndarray]:
-    """[n, n_props] float32 table in the exporter's column order (+ the semantic logits [n, C], when given), finite rows only."""
+def bake_filter_3d(params: GaussianSet, filter_3d: torch.Tensor) -> GaussianSet:
+    """The parameters with the 3D smoothing filter folded in (Mip-Splatting's fused export), evaluated in float64 and rounded
+    once to float32: scales log(s') with s' = sqrt(s^2 + sigma^2), opacity logit(sigmoid(o) * coef) with coef =
+    prod_k sqrt(s_k^2 / (s_k^2 + sigma^2)), s = exp(scales).  Means, rotations and colours are unchanged."""
+    with torch.no_grad():
+        ls = params.scales.detach().double()
+        sig2 = filter_3d.detach().double().reshape(-1, 1).to(ls.device) ** 2
+        s2 = torch.exp(2.0 * ls)
+        v = s2 + sig2
+        r = torch.where(v > 0, s2 / torch.where(v > 0, v, torch.ones_like(v)), torch.ones_like(v))
+        coef = torch.sqrt(r).prod(1, keepdim=True)
+        o = torch.sigmoid(params.opacities.detach().double()) * coef
+        logit = torch.log(o) - torch.log1p(-o)
+        scales = torch.where(v > 0, 0.5 * torch.log(torch.where(v > 0, v, torch.ones_like(v))), ls)
+        return GaussianSet(params.means, scales.float().contiguous(), params.quats, params.features_dc, params.features_rest,
+                           logit.float().contiguous())
+
+
+def to_columns(params: GaussianSet, semantic: Optional[torch.Tensor] = None,
+               filter_3d: Optional[torch.Tensor] = None) -> Tuple[List[str], np.ndarray]:
+    """[n, n_props] float32 table in the exporter's column order (+ the semantic logits [n, C], when given, + the 3D filter
+    sizes as ``filter_3D``, when given), finite rows only."""
     with torch.no_grad():
         means = params.means.detach().cpu().numpy().astype(np.float32)
         n = means.shape[0]
@@ -37,17 +63,22 @@ def to_columns(params: GaussianSet, semantic: Optional[torch.Tensor] = None) -> 
         rest = params.features_rest.detach().transpose(1, 2).contiguous().cpu().numpy().reshape(n, -1)
         cols = [means, np.zeros_like(means), dc, rest, params.opacities.detach().cpu().numpy().reshape(n, 1),
                 params.scales.detach().cpu().numpy(), params.quats.detach().cpu().numpy()]
+        n_sem = 0
         if semantic is not None:
             cols.append(semantic.detach().cpu().numpy().reshape(n, -1))
+            n_sem = cols[-1].shape[1]
+        if filter_3d is not None:
+            cols.append(filter_3d.detach().cpu().numpy().reshape(n, 1))
     table = np.concatenate([c.astype(np.float32).reshape(n, -1) for c in cols], axis=1)
     table = table[np.isfinite(table).all(axis=1)]
-    return property_names(rest.shape[1], 0 if semantic is None else cols[-1].shape[1]), table
+    return property_names(rest.shape[1], n_sem) + (["filter_3D"] if filter_3d is not None else []), table
 
 
-def write_ply(path, params: GaussianSet, semantic: Optional[torch.Tensor] = None) -> int:
+def write_ply(path, params: GaussianSet, semantic: Optional[torch.Tensor] = None, filter_3d: Optional[torch.Tensor] = None) -> int:
     """Writes ``point_cloud_<name>.ply`` for one sub-model; returns the number of exported Gaussians.  ``semantic``: the
-    sub-model's semantic logits [n, C], written as ``semantic_0..C-1`` after ``rot_3`` (None: no such columns)."""
-    names, table = to_columns(params, semantic)
+    sub-model's semantic logits [n, C], written as ``semantic_0..C-1`` after ``rot_3`` (None: no such columns).
+    ``filter_3d``: the 3D filter sizes [n], written as the last property ``filter_3D`` (None: no such column)."""
+    names, table = to_columns(params, semantic, filter_3d)
     header = "ply\nformat binary_little_endian 1.0\nelement vertex %d\n" % table.shape[0]
     header += "".join(f"property float {k}\n" for k in names) + "end_header\n"
     with open(path, "wb") as f:
@@ -120,10 +151,32 @@ def read_semantic(path, device="cpu") -> Optional[torch.Tensor]:
     return torch.from_numpy(np.stack([c[f"semantic_{i}"].astype(np.float32) for i in range(C)], axis=1)).to(device)
 
 
-def export_model(model, output_dir) -> Dict[str, int]:
+def read_filter_3d(path, device="cpu") -> Optional[torch.Tensor]:
+    """The ``filter_3D`` column of a ``write_ply(..., filter_3d=...)`` file as float32 [n], or None when the file has none."""
+    c = read_ply_columns(path)
+    if "filter_3D" not in c:
+        return None
+    return torch.from_numpy(c["filter_3D"].astype(np.float32)).to(device)
+
+
+def export_model(model, output_dir, filter_3d: Optional[str] = None) -> Dict[str, int]:
     """exporter.py:131-137: one ``point_cloud_<sub-model>.ply`` per entry of ``all_models`` (with its semantic logits, when
-    the model has them)."""
+    the model has them).  ``filter_3d`` (a model with ``SceneGraphConfig.filter_3d``): None writes the raw parameters alone,
+    "bake" the parameters with the filter folded in (``bake_filter_3d``), "column" the raw parameters plus ``filter_3D``."""
     import os
+    if filter_3d not in (None, "bake", "column"):
+        raise ValueError(f"filter_3d must be None, 'bake' or 'column' (got {filter_3d!r})")
     os.makedirs(output_dir, exist_ok=True)
-    return {k: write_ply(os.path.join(output_dir, f"point_cloud_{k}.ply"), sub.as_set(), getattr(sub, "semantic_logits", None))
-            for k, sub in model.all_models.items()}
+    out = {}
+    for k, sub in model.all_models.items():
+        params, column = sub.as_set(), None
+        if filter_3d is not None:
+            f = getattr(sub, "filter_3d", None)
+            if f is None:
+                raise ValueError(f"sub-model {k} has no 3D filter (SceneGraphConfig.filter_3d is off)")
+            if filter_3d == "bake":
+                params = bake_filter_3d(params, f)
+            else:
+                column = f
+        out[k] = write_ply(os.path.join(output_dir, f"point_cloud_{k}.ply"), params, getattr(sub, "semantic_logits", None), column)
+    return out

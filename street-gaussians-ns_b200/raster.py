@@ -155,6 +155,7 @@ class SegmentTable:
         if pre is not None and pre.dev is not None and pre.dev.device == device:
             # a row block of the device-resident (frame, actor) table (model.prepare_frames): nothing to build, nothing to copy
             self.host, self.N, self.num_chunks, self.nseg, self.static, self.dev = pre.host, pre.N, pre.num_chunks, pre.nseg, pre.static, pre.dev
+            self.filter_dev = filter_table(frame, self.static, device)
             return
         n = len(frame.segments)
         # the per-model part is cached on the parameter storage addresses -- or on a key the model vouches for
@@ -222,9 +223,44 @@ class SegmentTable:
         self.nseg = n
         self.static = st
         self.dev = torch.from_numpy(host.view(np.uint8).reshape(-1)).to(device, non_blocking=True) if upload else None
+        self.filter_dev = filter_table(frame, st, device)
         slot = getattr(frame, "_table_slot", None)
         if slot is not None and upload:  # the model keeps a timestamp's rows (validated by content, model._frame)
             slot["table"] = self
+
+
+def filter_table(frame: Frame, static: dict, device) -> Optional[torch.Tensor]:
+    """The device array of per-segment 3D filter pointers (sgn_camera.filter_3d) of ``frame``'s segments, or None when no
+    segment carries a filter.  Cached with the segment rows' static part, on the filter tensors' addresses."""
+    fl = [s.filter_3d for s in frame.segments]
+    if all(f is None for f in fl):
+        return None
+    if any(f is None for f in fl):
+        raise _lib.SgnError("only some segments of the frame carry a 3D filter: give every segment one, or none")
+    key = tuple(f.data_ptr() for f in fl)
+    cache = static.setdefault("filter_tables", {})
+    hit = cache.get(key)
+    if hit is None:
+        for i, (f, seg) in enumerate(zip(fl, frame.segments)):
+            n = seg.params.num_points
+            if not (f.is_cuda and f.device == device and f.dtype == torch.float32 and f.is_contiguous() and tuple(f.shape) == (n,)):
+                raise _lib.SgnError(f"segment {i} filter_3d must be a contiguous float32 [{n}] tensor on {device}; got {f.dtype} "
+                                    f"{tuple(f.shape)} on {f.device}")
+        if len(cache) > 16:
+            cache.clear()
+        hit = cache[key] = torch.from_numpy(np.array(key, np.uint64).view(np.uint8)).to(device, non_blocking=True)
+    return hit
+
+
+def with_filter(cs: _lib.CameraStruct, table: "SegmentTable") -> _lib.CameraStruct:
+    """``cs`` for a projection call over ``table``: a copy that points at the table's 3D filter array, or ``cs`` itself when
+    the table has none (the field stays as the caller set it, NULL by default)."""
+    fd = getattr(table, "filter_dev", None)
+    if fd is None:
+        return cs
+    out = _lib.CameraStruct.from_buffer_copy(cs)
+    out.filter_3d = fd.data_ptr()
+    return out
 
 
 def _grads_table(arena: torch.Tensor, static: dict, device) -> torch.Tensor:
@@ -294,6 +330,7 @@ def project_fwd(table: SegmentTable, cs: _lib.CameraStruct, device, view: Option
     """``view``: a device view (check_view) in place of the camera's (sgn_project_fwd_view)."""
     L = _lib.load()
     N = table.N
+    cs = with_filter(cs, table)
     records = torch.empty(N, _lib.RECORD_FLOATS, device=device, dtype=torch.float32)
     ints = torch.empty(4, max(N, 1), device=device, dtype=torch.int32)  # radii, num_tiles_hit, tiles_touched, touch_mask
     bbox = torch.empty(N, 4, device=device, dtype=torch.int16)
@@ -692,6 +729,7 @@ def project_bwd(table: SegmentTable, params: List[List[torch.Tensor]], cs, recor
     sgn_view_grad_reduce.  The arena is the same bits as sgn_project_bwd_range's with that view."""
     assert (view is None) == (v_view is None), "view and v_view go together"
     L = _lib.load()
+    cs = with_filter(cs, table)
     device = records.device
     st = table.static
     flat_sizes, _, _ = arena_layout(st)

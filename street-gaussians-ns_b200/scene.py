@@ -177,6 +177,10 @@ class Segment:
     center: Optional[np.ndarray] = None  # [3] (Box.center)
     idft: Optional[np.ndarray] = None  # [F] float32; None -> [1, 0, ...]
     name: str = ""
+    # per-row 3D smoothing filter sizes sigma [count] (float32, on the parameters' device; model.compute_filter_3d): the
+    # projection renders every row with scales sqrt(s^2 + sigma^2) and its opacity times coef (include/sgn_raster.h,
+    # sgn_camera.filter_3d).  None: no filter.  A frame's segments carry one all together or none at all
+    filter_3d: Optional[torch.Tensor] = None
 
     @property
     def has_pose(self) -> bool:

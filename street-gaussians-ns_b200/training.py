@@ -31,7 +31,7 @@ class TrainStep:
     def __init__(self, model: SceneGraphRasterModel, optimizer: FusedAdam, refine_every: Optional[int] = None,
                  group: Optional[dist.ProcessGroup] = None, pipeline_chunks: int = 0, refine_seed: int = 0,
                  check_replicas: bool = True, overlap: bool = False, exchange: str = "auto", metrics: bool = False,
-                 gradient_accumulation_steps: Optional[Dict[str, int]] = None):
+                 gradient_accumulation_steps: Optional[Dict[str, int]] = None, filter_cameras: Optional[Sequence[Camera]] = None):
         """``pipeline_chunks`` > 0 (data parallel only): all-reduce and Adam are pipelined over that many ranges of the
         arena (dp.allreduce_and_step) instead of running one after the other.  ``metrics``: every step calls
         ``model.get_metrics_dict`` between ``get_outputs`` and ``get_loss_dict`` (nerfstudio's order,
@@ -42,7 +42,11 @@ class TrainStep:
         tensor not named): every step.  A per-row group of the optimizer (``FusedAdam(rows=...)``; the reference sets
         ``{"semantic": 10}``) follows the same rule per sub-model: a sub-model whose gradient is None at the due step is skipped,
         and one that a refinement rebuilt in the middle of a cycle starts over from a zero gradient -- the refinement replaces
-        the Parameter, as nerfstudio's does, and the accumulated gradient goes with the old one."""
+        the Parameter, as nerfstudio's does, and the accumulated gradient goes with the old one.
+        ``filter_cameras`` (a model with ``SceneGraphConfig.filter_3d``): the training cameras the 3D smoothing filter is
+        computed from -- on the first step, right after every refinement that changed a row count, and every
+        ``filter_3d_every`` steps otherwise (Mip-Splatting's schedule).  Under data parallelism every replica computes the same
+        filter from the same full list, so nothing is exchanged."""
         self.model, self.optimizer, self.group = model, optimizer, group
         self.accumulate = dict(gradient_accumulation_steps or {})
         unknown = sorted(set(self.accumulate) - set(optimizer.extra_tensors()) - set(optimizer.row_tensors()))
@@ -58,6 +62,10 @@ class TrainStep:
         # None: every sub-model on its own ``refine_every`` (the reference registers one callback per sub-model with
         # ``update_every_num_iters = config.refine_every``); a number: one cadence for all of them
         self.refine_every = refine_every
+        self.filter_cameras = list(filter_cameras) if filter_cameras is not None else None
+        if self.filter_cameras is not None and not model.config.filter_3d:
+            raise ValueError("filter_cameras needs a model with SceneGraphConfig(filter_3d=True)")
+        self._filter_step = None  # the step the filter was last computed at
         assert optimizer.num_segments == len(model.all_models), "build FusedAdam over model.optimizer_params()"
 
     def world_size(self) -> int:
@@ -100,6 +108,8 @@ class TrainStep:
         if world > 1:
             self._ensure_exchange()
         m.step = step                                     # step_cb (sgn_splatfacto.py:754-755)
+        if self.filter_cameras is not None and self._filter_step is None:
+            self._update_filter(step)
         # accumulated tensors keep their gradient except where their cycle starts; they step where it ends
         keep = {id(extras[k]) for k, n in self.accumulate.items() if step % n != 0 and k in extras}
         rows = opt.row_tensors()
@@ -301,8 +311,11 @@ class TrainStep:
         else:
             due = any(st.refine_every > 0 and step % st.refine_every == 0 for st in (m.config.refine, m.config.object_refine))
         if not due:
+            self._maybe_filter(step, False)
             return
+        m.__dict__["refine_changed_rows"] = False
         m.refinement_after(self.optimizer, step, generator=self._refine_generator(step), due_only=self.refine_every is None)
+        self._maybe_filter(step, bool(m.__dict__.get("refine_changed_rows")))
         if self.world_size() > 1 and self.check_replicas:
             # replicas must have taken identical decisions: same row count in every sub-model
             rows = torch.tensor([sub.num_points for sub in m.all_models.values()], device=m.device, dtype=torch.int64)
@@ -310,6 +323,20 @@ class TrainStep:
             dist.all_reduce(lo, op=dist.ReduceOp.MIN, group=self.group)
             dist.all_reduce(hi, op=dist.ReduceOp.MAX, group=self.group)
             assert torch.equal(lo, hi), "replicas diverged in a refinement (row counts differ)"
+
+
+    def _maybe_filter(self, step: int, rows_changed: bool) -> None:
+        """Mip-Splatting's schedule for the 3D filter: after a refinement that changed a row count, and every
+        ``filter_3d_every`` steps."""
+        if self.filter_cameras is None:
+            return
+        every = self.model.config.filter_3d_every
+        if rows_changed or (every > 0 and step % every == 0 and self._filter_step != step):
+            self._update_filter(step)
+
+    def _update_filter(self, step: int) -> None:
+        self.model.compute_filter_3d(self.filter_cameras)
+        self._filter_step = step
 
 
 def warm_up_refinement(model: SceneGraphRasterModel, rows: Sequence[int] = (65536, 10000, 10000), step: Optional[int] = None) -> Dict[str, object]:

@@ -27,7 +27,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         actor_range: float = 45.0, pipeline_chunks: int = 0, overlap: bool = False, resident_table: bool = True,
         async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True, sky: bool = False, metrics: bool = False,
         bbox_opt: bool = False, camera_opt: bool = False, sky_view_grad: bool = False, lidar_depth: float = 0.0,
-        semantic: float = 0.0, antialiased: bool = False, scale_reg: bool = False) -> dict:
+        semantic: float = 0.0, antialiased: bool = False, scale_reg: bool = False, filter_3d: bool = False) -> dict:
     """One measurement.  torch.distributed must already be initialised when WORLD_SIZE > 1.  Returns the result dict on
     rank 0 (None elsewhere).  ``sky``: the reference's default learnable sky (use_sky_sphere, a 1024^2 cube map stepped by
     the same Adam launch at the ``sky_sphere`` group's lr 0.005, sgn_config.py:72-75).  ``metrics``: every step also computes
@@ -46,7 +46,8 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     projected with the step's camera.  ``antialiased``: rasterize_mode "antialiased" (the opacity scaled by the blur
     compensation, forward and backward).  ``scale_reg``: nerfstudio's scale regularisation (use_scale_regularization,
     max_gauss_ratio 10, every tenth step); the result then reports the fraction of rows whose max / min scale ratio is above
-    10 before and after the run."""
+    10 before and after the run.  ``filter_3d``: Mip-Splatting's 3D smoothing filter from the 425 rig cameras (SceneGraphConfig
+    .filter_3d), recomputed after every refinement that changed a row count and every 100 steps."""
     import torch
     import torch.distributed as dist
 
@@ -77,7 +78,8 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                            object_refine=RefineSettings(refine_every=refine_every, cull_alpha_thresh=0.005),
                            num_train_data=len(cams), refine_record=True, depth_loss_mult=lidar_depth,
                            semantic_classes=3 if semantic > 0 else 0, semantic_loss_mult=semantic,
-                           rasterize_mode="antialiased" if antialiased else "classic", use_scale_regularization=scale_reg)
+                           rasterize_mode="antialiased" if antialiased else "classic", use_scale_regularization=scale_reg,
+                           filter_3d=filter_3d)
     env_map = None
     if sky:
         from street_gaussians_ns_b200.sky import CubeMapSky
@@ -109,7 +111,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         accumulate = dict(accumulate or {}, semantic=10)
     opt = FusedAdam(model.optimizer_params(), extra=extra, reserve_spare=True, rows=rows)  # no cudaMalloc of moment arenas inside the training loop
     step_fn = TrainStep(model, opt, refine_every=refine_every, pipeline_chunks=pipeline_chunks, overlap=overlap, metrics=metrics,
-                        gradient_accumulation_steps=accumulate)
+                        gradient_accumulation_steps=accumulate, filter_cameras=cams if filter_3d else None)
     g = torch.Generator().manual_seed(5)
     gt = (torch.rand(H, W, 3, generator=g) * 255).to(torch.uint8).to(dev)  # get_loss_dict consumes uint8 directly
     counts0 = [sub.num_points for sub in model.all_models.values()]
@@ -245,6 +247,8 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                       if semantic > 0 else {}),
                    **({"rasterize_mode": "antialiased"} if antialiased else {}),
                    **({"scale_reg": "use_scale_regularization, max_gauss_ratio 10, every tenth step"} if scale_reg else {}),
+                   **({"filter_3d": "Mip-Splatting 3D filter from the 425 rig cameras, variance 0.2, recomputed every 100 steps "
+                                    "and after refinements"} if filter_3d else {}),
                    "loss": "fused kernels" if fused_loss else "torch ops", "metrics": "get_metrics_dict every step" if metrics else "none",
                    "start_step": start_step, "refine_every": refine_every,
                    "refinement_kernels_loaded_before_timing": refine_warm,
@@ -285,6 +289,7 @@ def main():
                     help="> 0: 3-class semantic logits and the cross-entropy term at weight W against synthetic labels")
     ap.add_argument("--antialiased", action="store_true", help="rasterize_mode 'antialiased': opacities scaled by the blur compensation")
     ap.add_argument("--scale-reg", action="store_true", help="nerfstudio's scale regularisation (max_gauss_ratio 10, every tenth step)")
+    ap.add_argument("--filter-3d", action="store_true", help="Mip-Splatting's 3D smoothing filter from the 5 x 85 rig cameras")
     args = ap.parse_args()
     if args.sky_view_grad and not (args.sky and args.camera_opt):
         ap.error("--sky-view-grad needs --sky and --camera-opt")
@@ -301,7 +306,7 @@ def main():
               args.overlap, not args.host_table, ssim_lambda=args.ssim_lambda, fused_loss=not args.torch_loss, sky=args.sky,
               metrics=args.metrics, bbox_opt=args.bbox_opt, camera_opt=args.camera_opt,
               sky_view_grad=args.sky_view_grad, lidar_depth=args.lidar_depth, semantic=args.semantic, antialiased=args.antialiased,
-              scale_reg=args.scale_reg)
+              scale_reg=args.scale_reg, filter_3d=args.filter_3d)
     if res is not None:
         print(json.dumps(res))
     if world > 1:
