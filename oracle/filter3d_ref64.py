@@ -22,6 +22,7 @@ import torch
 
 from oracle import project_aa_ref64 as aa
 from oracle import project_ref64 as ref
+from oracle.oracle_torch import expf_spec
 
 
 def sweep(means: Sequence[np.ndarray], views: Sequence[dict], M: np.ndarray, present: np.ndarray, variance: float = 0.2,
@@ -67,16 +68,31 @@ def sweep(means: Sequence[np.ndarray], views: Sequence[dict], M: np.ndarray, pre
     return dict(sigma=sigma, nu=nus, sampled=sampled, margin=margins, fill=fill, n_sampled=n_sampled)
 
 
+def _axes(ls, sigma):
+    """Per axis (r, v): v = s^2 + sigma^2 and r = s^2 / v, with r = 1 where v == 0 (sigma 0 and s^2 below the dtype's
+    smallest number: the filter is the identity there).  In float64 v is never 0 for the scales the tests use; in float32 a
+    thin axis of exp(-80) reaches v == 0 (sigma 0) or r == 0 (sigma > 0), as the kernels' float32 arithmetic does."""
+    s = expf_spec(ls) if ls.dtype == torch.float32 else torch.exp(ls)  # float32: the kernels' exp sequence
+    s2 = s * s
+    v = s2 + (sigma * sigma)[:, None]
+    pos = v > 0
+    return torch.where(pos, s2 / torch.where(pos, v, torch.ones_like(v)), torch.ones_like(v)), v
+
+
+def _sqrt0(x):
+    """sqrt(x) for x >= 0 whose gradient at 0 is 0 rather than inf * 0 = nan (only float32 evaluations reach 0 here)."""
+    pos = x > 0
+    return torch.where(pos, torch.sqrt(torch.where(pos, x, torch.ones_like(x))), torch.zeros_like(x))
+
+
 def coef(ls, sigma):
     """prod_k sqrt(s_k^2 / (s_k^2 + sigma^2)), s = exp(ls) (torch, differentiable in ls)."""
-    s2 = torch.exp(2.0 * ls)
-    sig2 = (sigma * sigma)[:, None]
-    return torch.sqrt(s2 / (s2 + sig2)).prod(-1)
+    return _sqrt0(_axes(ls, sigma)[0]).prod(-1)
 
 
 def filtered_scales(ls, sigma):
     """s' = sqrt(exp(ls)^2 + sigma^2) (torch, differentiable in ls)."""
-    return torch.sqrt(torch.exp(2.0 * ls) + (sigma * sigma)[:, None])
+    return _sqrt0(_axes(ls, sigma)[1])
 
 
 def forward(frame, st: ref.Settings, sigmas: Sequence, antialiased: bool = False, dtype=torch.float64,

@@ -63,11 +63,13 @@ def metrics(x: torch.Tensor):
     return {"camera_opt_translation": x[:, :3].norm(), "camera_opt_rotation": x[:, 3:].norm()}
 
 
-def record_loss_view(frame, st: ref.Settings, v_records: np.ndarray, view: torch.Tensor):
-    """sum(records * v_records) over the geometry columns of the visible rows, with W | c = view[:12] (float64 leaf)."""
+def record_loss_view(frame, st: ref.Settings, v_records: np.ndarray, view: torch.Tensor, scales=None, opacity=None):
+    """sum(records * v_records) over the geometry columns of the visible rows, with W | c = view[:12] (float64 leaf).
+    ``scales(cat)``: the linear scales of the composed rows in place of exp(log-scales); ``opacity(cat, a, b, c)``: a
+    per-row opacity from the blurred cov2d entries, whose column 5 term then joins the loss (visible rows)."""
     _, cat = pz.compose(frame, pz.pose_leaves(pz.frame_poses(frame)))
     cat = {k: v.detach() for k, v in cat.items()}
-    s = torch.exp(cat["scales"])
+    s = torch.exp(cat["scales"]) if scales is None else scales(cat)
     vis = ref.project_core(cat["means"], cat["quats"], s, frame.camera, st.block_width, st.clip_thresh, F64)["vis"]
     cam = frame.camera
     W = view[:12].reshape(3, 4)
@@ -95,7 +97,10 @@ def record_loss_view(frame, st: ref.Settings, v_records: np.ndarray, view: torch
     rw = 1.0 / (zs + 1e-6)
     xy = torch.stack([p[:, 0] * rw * fx + cam.cx, p[:, 1] * rw * fy + cam.cy], -1)
     v = torch.tensor(np.asarray(v_records, np.float64), dtype=F64)
-    return (((xy * v[:, 0:2]).sum(1) + (conic * v[:, 2:5]).sum(1) + z * v[:, 9]) * vt).sum(), vis
+    loss = (((xy * v[:, 0:2]).sum(1) + (conic * v[:, 2:5]).sum(1) + z * v[:, 9]) * vt).sum()
+    if opacity is not None:
+        loss = loss + (opacity(cat, a, b, c) * vt * v[:, 5]).sum()
+    return loss, vis
 
 
 def v_view_ref(frame, st: ref.Settings, v_records: np.ndarray) -> np.ndarray:

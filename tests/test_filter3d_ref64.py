@@ -256,3 +256,80 @@ def test_export_model_modes(tmp_path):
         ply_io.export_model(m, os.path.join(tmp_path, "z"), filter_3d="mip")
     with pytest.raises(ValueError):
         ply_io.export_model(_model(False, with_empty=False), os.path.join(tmp_path, "w"), filter_3d="bake")
+
+
+# ---- the filtered statements of tests/filter3d_cases.py ------------------------------------------------------------------
+def test_filtered_pose_and_view_statements_at_zero_filter():
+    from tests import antialias_cases as ac
+    from tests import camera_cases as cc
+    from tests import filter3d_cases as fc
+    from tests import pose_cases as pz
+    case = pc.get("fov_clamp")  # an unposed and a posed segment, FOV clamps on every side
+    fr, st = case.frame, case.st
+    zeros = fc.zero_filter(case)
+    v = pc.v_records(case, "all")
+    pairs = ((fc.v_pose_ref(fr, st, zeros, v), pz.v_pose_ref(fr, st, v)),
+             (fc.v_pose_ref(fr, st, zeros, v, True), ac.v_pose_ref(fr, st, v)),
+             (fc.v_view_ref(fr, st, zeros, v), cc.v_view_ref(fr, st, v)),
+             (fc.v_view_ref(fr, st, zeros, v, True), ac.v_view_ref(fr, st, v)))
+    for got, want in pairs:
+        assert np.any(want) and np.allclose(got, want, rtol=1e-12, atol=1e-12 * np.abs(want).max())
+
+
+@pytest.mark.parametrize("antialiased", [False, True])
+def test_filtered_pose_and_view_statements_central_differences(antialiased):
+    from tests import filter3d_cases as fc
+    from tests import pose_cases as pz
+    case = _frame(9)
+    fr, st = case.frame, case.st
+    rng = np.random.default_rng(4)
+    sigmas = [np.float32(rng.uniform(0.3, 3.0, s.params.num_points)) * np.exp(s.params.scales.numpy()).max(1)
+              for s in fr.segments]  # about the scales: both the covariance and coef move
+    v = pc.v_records(case, "all")
+    h = 1e-6
+    pose0 = pz.frame_poses(fr).astype(np.float64)
+    got = fc.v_pose_ref(fr, st, sigmas, v, antialiased)
+    fd = np.zeros_like(pose0)
+    for idx in np.ndindex(*pose0.shape):
+        vals = []
+        for sgn in (1, -1):
+            p = pose0.copy()
+            p[idx] += sgn * h
+            vals.append(float(fc.pose_loss(fr, st, sigmas, v, torch.tensor(p), antialiased)))
+        fd[idx] = (vals[0] - vals[1]) / (2 * h)
+    assert np.abs(got - fd).max() <= 1e-5 * np.abs(fd).max()
+    view0 = np.asarray(fr.camera.viewmat(), np.float64).reshape(-1)
+    got = fc.v_view_ref(fr, st, sigmas, v, antialiased)
+    fd = np.zeros(12)
+    for k in range(12):
+        vals = []
+        for sgn in (1, -1):
+            w = view0.copy()
+            w[k] += sgn * h
+            vals.append(float(fc.view_loss(fr, st, sigmas, v, torch.tensor(w), antialiased)[0]))
+        fd[k] = (vals[0] - vals[1]) / (2 * h)
+    assert np.abs(got - fd).max() <= 1e-5 * np.abs(fd).max()
+
+
+def test_settled_cases():
+    """Every filtered case of the directed tests: no filtered decision within the margin, and the families are what they say."""
+    from tests import filter3d_cases as fc
+    for name in fc.CONFIGS:
+        c = fc.get(name)
+        sig = np.concatenate(c.sigmas)
+        fw = f3.forward(c.frame, c.st, c.sigmas)
+        assert fw["margin"].min(initial=np.inf) >= pc.MARGIN, name
+        assert np.all(sig[c.rows("zero")] == 0) and np.all(sig[~c.rows("zero")] >= 0), name
+        idn = c.rows("identity") & c.thin.any(1)
+        und = c.rows("underflow") & c.thin.any(1)
+        assert np.all(sig[idn] == 0) and np.all(sig[und] > 0), name
+        assert np.all(fw["coef"][idn] == 1.0), name
+        f32 = f3.forward(c.frame, c.st, c.sigmas, dtype=torch.float32)
+        assert np.all(f32["coef"][und] == 0), name  # in float32 an underflowed axis has r = 0
+        assert np.all(np.isfinite(f32["records"])), name
+        if name.startswith("comp_edges/") and not name.endswith("needle"):
+            assert (idn | und).sum() == 6, name
+        if name.endswith("/dominant"):
+            assert np.all(fw["coef"][fw["vis"]] < 0.05), name
+    mixed = fc.get("posed40/mixed")
+    assert len(np.unique(mixed.fams)) == len(fc.FAMILIES)

@@ -249,7 +249,9 @@ def test_full_render_matches_baked_parameters():
     frc = _with_filter(to_cuda(fr), sig)
     baked = Frame(fr.camera, [Segment(ply_io.bake_filter_3d(s.params, torch.as_tensor(g)).to("cuda"), s.cls, s.rot, s.center,
                                       s.idft, s.name) for s, g in zip(fr.segments, sig)])
-    for mode in ("classic",):
+    # the antialiased mode too: comp of the baked s' is comp of the filtered covariance, and sigmoid(logit(sigmoid x coef))
+    # is sigmoid x coef up to rounding
+    for mode in ("classic", "antialiased"):
         st = raster.RenderSettings(rasterize_mode=mode)
         a, _ = raster.render_frame(frc, st)
         b, _ = raster.render_frame(baked, st)
@@ -257,8 +259,8 @@ def test_full_render_matches_baked_parameters():
         for k in ("rgb", "accumulation", "object_acc", "background_acc"):
             d = (a[k] - b[k]).abs().amax(-1)
             frac = float((d > 1e-4).float().mean())
-            print(f"[filter3d bake] {k}: {frac:.4%} of pixels beyond 1e-4, max {float(d.max()):.2e}")
-            assert frac <= 0.005, (k, frac)
+            print(f"[filter3d bake] {mode} {k}: {frac:.4%} of pixels beyond 1e-4, max {float(d.max()):.2e}")
+            assert frac <= 0.005, (mode, k, frac)
 
 
 def test_zoom_property():
