@@ -726,6 +726,25 @@ size_t sgn_sizeof_filter_xform(void);
 int sgn_filter3d(const sgn_filter_sub* subs_dev, int nsub, int num_chunks, const sgn_filter_view* views_dev, int V,
                  const sgn_filter_xform* xforms_dev, double variance, double near, int32_t* stats, void* stream);
 
+/* ---- per-image bilateral grids (Wang et al., SIGGRAPH 2024; gsplat's use_bilateral_grid): appearance correction
+ * A grid is [12, L, Hg, Wg] float32 (a 3x4 affine per node, row-major over output channels r, g, b by inputs r, g, b, 1).
+ * Slice of one H x W image rgb [H,W,3] with one grid: pixel (i, j) samples the grid trilinearly (corners clamped) at
+ *   gx = (j + 0.5) / W * (Wg - 1), gy = (i + 0.5) / H * (Hg - 1), gz = clamp(0.299 r + 0.587 g + 0.114 b, 0, 1) * (L - 1)
+ * giving M = [A | t]; out = A c + t (F.grid_sample(align_corners=True, padding_mode="border") followed by the affine).
+ * sgn_bilagrid_slice_bwd writes d_rgb [H,W,3] (A^T d_out plus the guidance term where the gray is strictly inside (0, 1)) and
+ * overwrites d_grid [12,L,Hg,Wg] with the trilinear scatter of d_out (x) (c, 1).  No float atomics: two runs give the same
+ * bits.  L <= 32 in the backward.  scratch: sgn_bilagrid_slice_bwd_scratch_bytes (per-block partials).
+ * Total variation over N grids [N,12,L,Hg,Wg]: tv = (1/N) sum over the axes L, Hg, Wg of mean((forward difference)^2), each
+ * mean over every image and coefficient, an axis of size 1 adding 0; out is a device float, summed in fp64 in a fixed order
+ * (scratch: sgn_bilagrid_tv_scratch_bytes).  sgn_bilagrid_tv_bwd overwrites d_grids with v_out[0] * d tv / d grids. */
+int sgn_bilagrid_slice_fwd(const float* grid, int L, int Hg, int Wg, const float* rgb, int H, int W, float* out, void* stream);
+size_t sgn_bilagrid_slice_bwd_scratch_bytes(int L, int Hg, int Wg, int H, int W);
+int sgn_bilagrid_slice_bwd(const float* grid, int L, int Hg, int Wg, const float* rgb, const float* d_out, int H, int W, float* d_rgb,
+                           float* d_grid, void* scratch, size_t scratch_bytes, void* stream);
+size_t sgn_bilagrid_tv_scratch_bytes(void);
+int sgn_bilagrid_tv_fwd(const float* grids, int N, int L, int Hg, int Wg, float* out, void* scratch, size_t scratch_bytes, void* stream);
+int sgn_bilagrid_tv_bwd(const float* grids, int N, int L, int Hg, int Wg, const float* v_out, float* d_grids, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -36,6 +36,7 @@ SOURCES = {
     "semantic.cu": [],  # IEEE expf / logf / division in the cross-entropy; the carry only copies
     "scale_reg.cu": [],  # IEEE expf; the gradient chain through explicit _rn intrinsics, as torch autograd rounds it
     "filter3d.cu": ["--fmad=false"],  # fp64 sampling tests rounded per operation, as the float64 statement evaluates them
+    "bilagrid.cu": [],  # IEEE division; the grid coordinates and the gray through explicit _rn intrinsics
 }
 
 

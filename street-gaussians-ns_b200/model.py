@@ -12,7 +12,7 @@ parts of ``SplatfactoModel`` it inherits (street_gaussians_ns/sgn_splatfacto.py:
     ``depths, radii, conics, num_tiles_hit, last_size`` on the model and split per sub-model
     (``SplatfactoModel.after_train`` reads ``self.xys.grad`` and ``self.radii``, :513-541);
   * ``get_loss_dict`` (L1 + SSIM + sky accumulation + object-accumulation entropy, + the lidar depth term when
-    ``depth_loss_mult > 0``);
+    ``depth_loss_mult > 0``, + the bilateral grids' total variation with a ``bilateral_grid``);
   * ``get_metrics_dict`` (per-step psnr, Gaussian count, scale / opacity / radii means: one reduction kernel),
     ``get_image_metrics_and_images`` and ``get_outputs_for_camera`` (eval).
 
@@ -389,7 +389,7 @@ class SceneGraphRasterModel(torch.nn.Module):
     def __init__(self, background: GaussianSet, actors: Dict[str, GaussianSet], config: Optional[SceneGraphConfig] = None,
                  poses_at: Optional[Callable[[float], List[ActorPose]]] = None,
                  sky: Optional[Callable[[Camera, bool], torch.Tensor]] = None, bbox_optimizer: Optional[torch.nn.Module] = None,
-                 camera_optimizer: Optional[torch.nn.Module] = None):
+                 camera_optimizer: Optional[torch.nn.Module] = None, bilateral_grid: Optional[torch.nn.Module] = None):
         super().__init__()
         self.config = config or SceneGraphConfig()
         raster.rasterize_mode_flag(self.config.rasterize_mode)  # an unknown mode raises ValueError, as the reference's does
@@ -404,6 +404,9 @@ class SceneGraphRasterModel(torch.nn.Module):
         # trainable corrections of the actor boxes (box_pose.BoxPoseOptimizer; the reference's attribute name, scene graph
         # :91).  None, or one in mode "off": the boxes are rendered as annotated, by the same calls as without it
         self.bbox_optimizer = bbox_optimizer
+        # per-image appearance correction (bilagrid.BilateralGrid, one grid per training image; gsplat's use_bilateral_grid).
+        # None: every image is rendered and trained by the same calls as without it
+        self.bilateral_grid = bilateral_grid
         self.all_models = torch.nn.ModuleDict()
         C = int(self.config.semantic_classes)
         f3 = bool(self.config.filter_3d)
@@ -729,7 +732,7 @@ class SceneGraphRasterModel(torch.nn.Module):
             res["background_acc"] = torch.zeros(H, W, 1, device=dev)
             if extra is not None:
                 res["semantic"] = torch.zeros(H, W, extra.shape[1], device=dev)
-            return res
+            return self._correct_appearance(res, camera)
         if not self.training:
             # eval-only extra renders (scene graph :367-372): per-class rgb
             with torch.no_grad():
@@ -739,6 +742,15 @@ class SceneGraphRasterModel(torch.nn.Module):
                     # without actors the reference's objects-only render returns {'rgb': zeros[H,W,1], 'depth': zeros[H,W,1]}
                     # (scene graph :264-267), which get_outputs publishes as object_rgb AND object_depth (:371-372)
                     out["object_depth"] = torch.zeros(H, W, 1, device=self.device)
+        return self._correct_appearance(out, camera)
+
+    def _correct_appearance(self, out: Dict[str, torch.Tensor], camera: Camera) -> Dict[str, torch.Tensor]:
+        """In training, for a camera with an index: ``out["rgb"]`` (the render with the sky composited) replaced by its slice with
+        that image's bilateral grid, so the losses, the per-step psnr and every other consumer see the corrected image.  In eval,
+        or for a camera without an index (a novel view has no grid of its own), the raw render."""
+        bg = self.bilateral_grid
+        if bg is not None and self.training and camera.index is not None:
+            out["rgb"] = bg.slice(out["rgb"], camera.index)
         return out
 
     def _fused_scale_reg_due(self) -> bool:
@@ -1038,7 +1050,10 @@ class SceneGraphRasterModel(torch.nn.Module):
         With ``use_scale_regularization``, ``scale_reg`` is present on every call, as nerfstudio emits it: at a step that is a
         multiple of 10, 0.1 * mean(max(amax(s) / amin(s), max_gauss_ratio) - max_gauss_ratio) with s = exp(scales) over the rows
         of the visible sub-models (the render computed it, sgn_scale_reg_fwd; torch ops over ``torch.cat`` of their scales
-        with ``fused_loss=False``), and a zero without gradient on the other steps."""
+        with ``fused_loss=False``), and a zero without gradient on the other steps.
+
+        With a ``bilateral_grid``, in training: ``bilagrid_tv`` = 10 * the total variation of all grids
+        (bilagrid.BilateralGrid.tv_loss), every step."""
         c = self.config
         want_sky = "semantic" in batch and c.sky_acc_loss_mult > 0
         want_ent = c.object_acc_entropy_loss_mult > 0.0 and self.step > c.refine.stop_split_at  # background_model.stop_split_at (:386)
@@ -1107,6 +1122,8 @@ class SceneGraphRasterModel(torch.nn.Module):
         if self.training and co is not None and co.mode != "off":
             terms = getattr(self, "_camera_terms", None)
             losses["camera_opt_regularizer"] = terms[0] if terms is not None else co.regularizer()
+        if self.training and self.bilateral_grid is not None:
+            losses["bilagrid_tv"] = 10.0 * self.bilateral_grid.tv_loss()  # gsplat's tv_loss weight
         return losses
 
     def _depth_target(self, batch) -> Optional[torch.Tensor]:

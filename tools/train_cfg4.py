@@ -27,7 +27,8 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         actor_range: float = 45.0, pipeline_chunks: int = 0, overlap: bool = False, resident_table: bool = True,
         async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True, sky: bool = False, metrics: bool = False,
         bbox_opt: bool = False, camera_opt: bool = False, sky_view_grad: bool = False, lidar_depth: float = 0.0,
-        semantic: float = 0.0, antialiased: bool = False, scale_reg: bool = False, filter_3d: bool = False) -> dict:
+        semantic: float = 0.0, antialiased: bool = False, scale_reg: bool = False, filter_3d: bool = False,
+        bilateral_grid: bool = False) -> dict:
     """One measurement.  torch.distributed must already be initialised when WORLD_SIZE > 1.  Returns the result dict on
     rank 0 (None elsewhere).  ``sky``: the reference's default learnable sky (use_sky_sphere, a 1024^2 cube map stepped by
     the same Adam launch at the ``sky_sphere`` group's lr 0.005, sgn_config.py:72-75).  ``metrics``: every step also computes
@@ -47,7 +48,9 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     compensation, forward and backward).  ``scale_reg``: nerfstudio's scale regularisation (use_scale_regularization,
     max_gauss_ratio 10, every tenth step); the result then reports the fraction of rows whose max / min scale ratio is above
     10 before and after the run.  ``filter_3d``: Mip-Splatting's 3D smoothing filter from the 425 rig cameras (SceneGraphConfig
-    .filter_3d), recomputed after every refinement that changed a row count and every 100 steps."""
+    .filter_3d), recomputed after every refinement that changed a row count and every 100 steps.  ``bilateral_grid``: one
+    bilateral grid per rig image (425, bilagrid.BilateralGrid with gsplat's 16 x 16 x 8) corrects every training render, with
+    the grids' total-variation term; stepped by the same Adam launch at gsplat's lr 2e-3."""
     import torch
     import torch.distributed as dist
 
@@ -89,13 +92,18 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         from street_gaussians_ns_b200.box_pose import BoxPoseOptimizer
         boxes = BoxPoseOptimizer(num_frames, [str(k) for k in sc.actors], {f: f for f in range(num_frames)}, mode="simple")
     cam_opt = None
+    if camera_opt or bilateral_grid:  # both look a training image up by its index
+        for i, c in enumerate(cams):
+            c.index = i
     if camera_opt:
         from street_gaussians_ns_b200.camera_pose import CameraPoseOptimizer
         cam_opt = CameraPoseOptimizer(len(cams))
-        for i, c in enumerate(cams):
-            c.index = i
+    bil = None
+    if bilateral_grid:
+        from street_gaussians_ns_b200.bilagrid import BilateralGrid
+        bil = BilateralGrid(len(cams))
     model = SceneGraphRasterModel(sc.background.to(dev), {k: v.to(dev) for k, v in sc.actors.items()}, cfg, poses_at=poses_at,
-                                  sky=env_map, bbox_optimizer=boxes, camera_optimizer=cam_opt).to(dev)
+                                  sky=env_map, bbox_optimizer=boxes, camera_optimizer=cam_opt, bilateral_grid=bil).to(dev)
     model.train()
     extra = {"sky": (model.env_map.base, 0.005)} if sky else {}
     if bbox_opt:
@@ -105,6 +113,8 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     if camera_opt:
         extra["camera_opt.pose_adjustment"] = (cam_opt.pose_adjustment, 1e-3)
         accumulate = {"camera_opt.pose_adjustment": 100}
+    if bilateral_grid:
+        extra["bilateral_grid.grids"] = (bil.grids, 2e-3)
     rows = None
     if semantic > 0:
         rows = {"semantic": (model.semantic_params(), 0.0025)}
@@ -249,6 +259,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                    **({"scale_reg": "use_scale_regularization, max_gauss_ratio 10, every tenth step"} if scale_reg else {}),
                    **({"filter_3d": "Mip-Splatting 3D filter from the 425 rig cameras, variance 0.2, recomputed every 100 steps "
                                     "and after refinements"} if filter_3d else {}),
+                   **({"bilateral_grid": "BilateralGrid(425, 16 x 16 x 8), 10 * total variation, Adam lr 2e-3"} if bilateral_grid else {}),
                    "loss": "fused kernels" if fused_loss else "torch ops", "metrics": "get_metrics_dict every step" if metrics else "none",
                    "start_step": start_step, "refine_every": refine_every,
                    "refinement_kernels_loaded_before_timing": refine_warm,
@@ -290,6 +301,7 @@ def main():
     ap.add_argument("--antialiased", action="store_true", help="rasterize_mode 'antialiased': opacities scaled by the blur compensation")
     ap.add_argument("--scale-reg", action="store_true", help="nerfstudio's scale regularisation (max_gauss_ratio 10, every tenth step)")
     ap.add_argument("--filter-3d", action="store_true", help="Mip-Splatting's 3D smoothing filter from the 5 x 85 rig cameras")
+    ap.add_argument("--bilateral-grid", action="store_true", help="a bilateral grid per rig image (425) corrects each training render")
     args = ap.parse_args()
     if args.sky_view_grad and not (args.sky and args.camera_opt):
         ap.error("--sky-view-grad needs --sky and --camera-opt")
@@ -306,7 +318,7 @@ def main():
               args.overlap, not args.host_table, ssim_lambda=args.ssim_lambda, fused_loss=not args.torch_loss, sky=args.sky,
               metrics=args.metrics, bbox_opt=args.bbox_opt, camera_opt=args.camera_opt,
               sky_view_grad=args.sky_view_grad, lidar_depth=args.lidar_depth, semantic=args.semantic, antialiased=args.antialiased,
-              scale_reg=args.scale_reg, filter_3d=args.filter_3d)
+              scale_reg=args.scale_reg, filter_3d=args.filter_3d, bilateral_grid=args.bilateral_grid)
     if res is not None:
         print(json.dumps(res))
     if world > 1:
