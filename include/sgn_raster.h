@@ -745,6 +745,75 @@ size_t sgn_bilagrid_tv_scratch_bytes(void);
 int sgn_bilagrid_tv_fwd(const float* grids, int N, int L, int Hg, int Wg, float* out, void* scratch, size_t scratch_bytes, void* stream);
 int sgn_bilagrid_tv_bwd(const float* grids, int N, int L, int Hg, int Wg, const float* v_out, float* d_grids, void* stream);
 
+/* ---- densification by MCMC (Kheradmand et al., NeurIPS 2024; gsplat's MCMCStrategy)
+ * Throughout o = sigmoid(logit) and s = exp(log_scale) in fp32.  Random draws come from Philox4x32-10 with key = seed and counter
+ * (index, step, sub, purpose) -- purpose SGN_MCMC_NOISE / _RELOCATE / _ADD, index the row or the draw -- so a call gives the same
+ * bits on every run and for every launch shape.
+ *
+ * sgn_mcmc_noise: for every row of every sub-model (subs_dev[k]: rows [0, count), first 128-row chunk chunk0, first row row0 of
+ * the concatenated index space, Philox sub index, its noise_lr), with eps ~ N(0, I3) from Philox (or normals[row0 + row] when
+ * normals != NULL) and lr the means' learning rate:
+ *   gate = 1 / (1 + exp(-100 ((1 - o) - 0.995))),  Sigma = R(q/|q|) diag(s^2) R^T,  means += Sigma (eps * gate * (lr * noise_lr)).
+ *
+ * sgn_mcmc_sample: weights w_i = o_i (0 for rows with o_i <= min_opacity when exclude_dead), their fp64 inclusive prefix sum P
+ * (summed in a fixed order), then draw j takes the first row with P_i > u_j * P_{n-1}, u_j from Philox (or uniforms[j], in
+ * [0, 1)).  The number of draws is *num_draws_dev when given (device), else max_draws.  counts [n] is overwritten with the
+ * number of draws of each row (integer atomics).  With a zero total no row is drawn and draws[j] = -1.  dead_rows / num_dead
+ * (optional, device): the rows with o_i <= min_opacity in ascending order and their number.  total (optional, device double):
+ * P_{n-1}.  scratch: sgn_mcmc_sample_scratch_bytes(n).  Nothing is read back.
+ *
+ * sgn_mcmc_relocate: for every row i with c = counts[i] > 0 and N = min(c + 1, 51), in fp64, rounded once:
+ *   o' = 1 - (1 - o)^(1/N),  denom = sum_{k=1..N} (-1)^(k-1) C(N,k) o'^k / sqrt(k),
+ *   log_scale = log((o / denom) s),  logit = logit(clamp(o', min_opacity, 1 - 2^-23)),
+ * and zeroes row i of every tensor of `zero` (the Adam moments) when zero != NULL.
+ *
+ * sgn_mcmc_copy_rows: row dst_j <- row src_j in every tensor of `t`, for j < (*num_rows_dev or max_rows), dst_j = dst_rows[j] or
+ * dst_row0 + j, skipping src_j < 0.  Sources and destinations must not overlap.
+ *
+ * sgn_mcmc_reg_fwd / _bwd: over the N rows of the segment table (128-row chunks), out[0] = w_o * mean_i o_i and
+ * out[1] = w_s * mean_{i,k} s_ik (fp64 sums in a fixed order, each mean rounded once to fp32, times w in fp32; bit-identical
+ * run to run).  The backward ADDS v_out[0] * d out[0] + v_out[1] * d out[1] into grads_dev[k].opacities / .scales (v_out:
+ * two device floats, either pointer may be NULL = no cotangent).  Elementwise: deterministic. */
+#define SGN_MCMC_NOISE 0
+#define SGN_MCMC_RELOCATE 1
+#define SGN_MCMC_ADD 2
+#define SGN_MCMC_MAX_TENSORS 16
+typedef struct sgn_mcmc_sub {
+    float* means;             /* [count,3], updated in place */
+    const float* scales;      /* [count,3] log */
+    const float* quats;       /* [count,4] wxyz, un-normalised */
+    const float* opacities;   /* [count,1] logit */
+    int32_t count;
+    int32_t chunk0;
+    int32_t row0;
+    int32_t index;            /* the sub-model's index: part of the Philox counter */
+    float noise_lr;
+    int32_t pad;
+} sgn_mcmc_sub;
+typedef struct sgn_mcmc_tensors {
+    float* data[SGN_MCMC_MAX_TENSORS]; /* row-major [rows, width] */
+    int32_t width[SGN_MCMC_MAX_TENSORS];
+    int32_t count;
+    int32_t pad;
+} sgn_mcmc_tensors;
+size_t sgn_sizeof_mcmc_sub(void);
+size_t sgn_sizeof_mcmc_tensors(void);
+int sgn_mcmc_noise(const sgn_mcmc_sub* subs_dev, int nsub, int num_chunks, float lr, uint64_t seed, int step, const float* normals,
+                   void* stream);
+size_t sgn_mcmc_sample_scratch_bytes(int n);
+int sgn_mcmc_sample(const float* opacities, int n, float min_opacity, int exclude_dead, int max_draws, const int32_t* num_draws_dev,
+                    uint64_t seed, int step, int sub, int purpose, const double* uniforms, int32_t* draws, int32_t* counts,
+                    int32_t* dead_rows, int32_t* num_dead, double* total, void* scratch, size_t scratch_bytes, void* stream);
+int sgn_mcmc_relocate(float* opacities, float* scales, int n, const int32_t* counts, float min_opacity, const sgn_mcmc_tensors* zero,
+                      void* stream);
+int sgn_mcmc_copy_rows(const sgn_mcmc_tensors* t, const int32_t* dst_rows, int dst_row0, const int32_t* src_rows, int max_rows,
+                       const int32_t* num_rows_dev, void* stream);
+size_t sgn_mcmc_reg_scratch_bytes(void);
+int sgn_mcmc_reg_fwd(const sgn_segment* table_dev, int nseg, int N, int num_chunks, float w_opacity, float w_scale, float* out,
+                     void* scratch, size_t scratch_bytes, void* stream);
+int sgn_mcmc_reg_bwd(const sgn_segment* table_dev, const sgn_segment_grads* grads_dev, int nseg, int N, int num_chunks, float w_opacity,
+                     float w_scale, const float* v_opacity, const float* v_scale, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -104,6 +104,21 @@ class RefineTensors(C.Structure):
     ]
 
 
+class MCMCSub(C.Structure):
+    _fields_ = [
+        ("means", C.c_void_p), ("scales", C.c_void_p), ("quats", C.c_void_p), ("opacities", C.c_void_p),
+        ("count", C.c_int32), ("chunk0", C.c_int32), ("row0", C.c_int32), ("index", C.c_int32), ("noise_lr", C.c_float), ("pad", C.c_int32),
+    ]
+
+
+MCMC_MAX_TENSORS = 16  # SGN_MCMC_MAX_TENSORS
+MCMC_NOISE, MCMC_RELOCATE, MCMC_ADD = 0, 1, 2  # SGN_MCMC_*: the purpose word of the Philox counter
+
+
+class MCMCTensors(C.Structure):
+    _fields_ = [("data", C.c_void_p * MCMC_MAX_TENSORS), ("width", C.c_int32 * MCMC_MAX_TENSORS), ("count", C.c_int32), ("pad", C.c_int32)]
+
+
 # flag bits of sgn_refine_decide (csrc/sgn_refine_rules.cuh)
 RF_SPLIT, RF_DUP, RF_KEEP_ORIG, RF_KEEP_SPLIT, RF_KEEP_DUP, RF_HIGH_GRAD, RF_ALPHA, RF_TOOBIG = (1 << i for i in range(8))
 
@@ -157,7 +172,9 @@ EXPORTS = [
     "sgn_semantic_scratch_bytes", "sgn_semantic_loss_fwd", "sgn_semantic_loss_bwd", "sgn_semantic_metrics", "sgn_refine_carry",
     "sgn_scale_reg_scratch_bytes", "sgn_scale_reg_fwd", "sgn_scale_reg_bwd", "sgn_sizeof_filter_xform", "sgn_filter3d",
     "sgn_bilagrid_slice_fwd", "sgn_bilagrid_slice_bwd_scratch_bytes", "sgn_bilagrid_slice_bwd", "sgn_bilagrid_tv_scratch_bytes",
-    "sgn_bilagrid_tv_fwd", "sgn_bilagrid_tv_bwd",
+    "sgn_bilagrid_tv_fwd", "sgn_bilagrid_tv_bwd", "sgn_sizeof_mcmc_sub", "sgn_sizeof_mcmc_tensors", "sgn_mcmc_noise",
+    "sgn_mcmc_sample_scratch_bytes", "sgn_mcmc_sample", "sgn_mcmc_relocate", "sgn_mcmc_copy_rows", "sgn_mcmc_reg_scratch_bytes",
+    "sgn_mcmc_reg_fwd", "sgn_mcmc_reg_bwd",
 ]
 VIEW_FLOATS = 12  # SGN_VIEW_FLOATS: the view's cotangent, viewmat[12] row-major; the device view itself is 12 + 3 (cam_pos) floats
 POSE_FLOATS = 16  # SGN_POSE_FLOATS: a segment's pose (and its cotangent) as R[9] row-major, t[3], q[4]
@@ -312,6 +329,19 @@ def load():
     L.sgn_bilagrid_tv_bwd.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp]
     for f in ("sgn_bilagrid_slice_fwd", "sgn_bilagrid_slice_bwd", "sgn_bilagrid_tv_fwd", "sgn_bilagrid_tv_bwd"):
         getattr(L, f).restype = C.c_int
+    u64 = C.c_uint64
+    L.sgn_sizeof_mcmc_sub.restype = L.sgn_sizeof_mcmc_tensors.restype = sz
+    L.sgn_mcmc_noise.argtypes = [vp, i32, i32, fl, u64, i32, vp, vp]
+    L.sgn_mcmc_sample_scratch_bytes.argtypes = [i32]
+    L.sgn_mcmc_sample_scratch_bytes.restype = sz
+    L.sgn_mcmc_sample.argtypes = [vp, i32, fl, i32, i32, vp, u64, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, sz, vp]
+    L.sgn_mcmc_relocate.argtypes = [vp, vp, i32, vp, fl, C.POINTER(MCMCTensors), vp]
+    L.sgn_mcmc_copy_rows.argtypes = [C.POINTER(MCMCTensors), vp, i32, vp, i32, vp, vp]
+    L.sgn_mcmc_reg_scratch_bytes.restype = sz
+    L.sgn_mcmc_reg_fwd.argtypes = [vp, i32, i32, i32, fl, fl, vp, vp, sz, vp]
+    L.sgn_mcmc_reg_bwd.argtypes = [vp, vp, i32, i32, i32, fl, fl, vp, vp, vp]
+    for f in ("sgn_mcmc_noise", "sgn_mcmc_sample", "sgn_mcmc_relocate", "sgn_mcmc_copy_rows", "sgn_mcmc_reg_fwd", "sgn_mcmc_reg_bwd"):
+        getattr(L, f).restype = C.c_int
     L.sgn_sizeof_adam_tensor.restype = sz
     L.sgn_adam_chunk_elems.restype = C.c_int
     L.sgn_adam_step.argtypes = [vp, i32, i32, vp, vp, vp, vp]
@@ -328,6 +358,8 @@ def load():
     assert L.sgn_sizeof_segment() == C.sizeof(Segment), "sgn_segment layout mismatch between header and ctypes"
     assert L.sgn_sizeof_segment_grads() == C.sizeof(SegmentGrads)
     assert L.sgn_sizeof_camera() == C.sizeof(CameraStruct), "sgn_camera layout mismatch"
+    assert L.sgn_sizeof_mcmc_sub() == C.sizeof(MCMCSub), "sgn_mcmc_sub layout mismatch"
+    assert L.sgn_sizeof_mcmc_tensors() == C.sizeof(MCMCTensors), "sgn_mcmc_tensors layout mismatch"
     _lib = L
     return L
 

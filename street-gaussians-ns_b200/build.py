@@ -37,6 +37,7 @@ SOURCES = {
     "scale_reg.cu": [],  # IEEE expf; the gradient chain through explicit _rn intrinsics, as torch autograd rounds it
     "filter3d.cu": ["--fmad=false"],  # fp64 sampling tests rounded per operation, as the float64 statement evaluates them
     "bilagrid.cu": [],  # IEEE division; the grid coordinates and the gray through explicit _rn intrinsics
+    "mcmc.cu": ["--fmad=false"],  # the fp64 update rule and the fp32 noise rounded per operation, as their statements evaluate them
 }
 
 

@@ -29,7 +29,8 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
-from . import raster, refine
+from . import mcmc, raster, refine
+from .mcmc import MCMCSettings
 from .refine import RefineSettings
 from .scene import PARAM_NAMES, CLS_BACKGROUND, CLS_OBJECT, Camera, Frame, GaussianSet, Segment, fourier_time, idft_basis
 
@@ -102,6 +103,17 @@ class SceneGraphConfig:
     filter_3d_variance: float = 0.2
     filter_3d_near: float = 0.2
     filter_3d_every: int = 100
+    # densification strategy: "default" is the reference's split / duplicate / cull / opacity reset (refine, object_refine);
+    # "mcmc" is gsplat's MCMCStrategy (mcmc.py): dead rows relocated onto live ones, growth by 5 % per refinement up to a
+    # per-sub-model cap, position noise every step (TrainStep), and two regularisers in the loss, every training step:
+    # mcmc_opacity_reg = mcmc_opacity_reg * mean(sigmoid(opacities)), mcmc_scale_reg = mcmc_scale_reg * mean(exp(scales)), over the
+    # visible sub-models' rows (gsplat averages over all rows).  The weights are those of gsplat's MCMC preset.  The actors' cap of
+    # 100 000 is a placeholder that no measurement backs: set it from the actors' sizes in the data
+    strategy: str = "default"
+    mcmc: MCMCSettings = field(default_factory=MCMCSettings)
+    object_mcmc: MCMCSettings = field(default_factory=lambda: MCMCSettings(cap_max=100_000))
+    mcmc_opacity_reg: float = 0.01
+    mcmc_scale_reg: float = 0.01
 
     # ``stop_split_at`` of the BACKGROUND sub-model: what the reference's entropy gate reads
     # (``config.background_model.stop_split_at``, scene graph :386).  One source: ``refine.stop_split_at``.
@@ -393,6 +405,8 @@ class SceneGraphRasterModel(torch.nn.Module):
         super().__init__()
         self.config = config or SceneGraphConfig()
         raster.rasterize_mode_flag(self.config.rasterize_mode)  # an unknown mode raises ValueError, as the reference's does
+        if self.config.strategy not in ("default", "mcmc"):
+            raise ValueError(f"unknown densification strategy {self.config.strategy!r}: expected 'default' or 'mcmc'")
         # trainable camera poses (camera_pose.CameraPoseOptimizer, nerfstudio's attribute name).  None, or one in mode "off":
         # every camera is rendered as given, by the same calls as without it
         if camera_optimizer is not None and camera_optimizer.mode != "off" and sky is not None:
@@ -427,6 +441,7 @@ class SceneGraphRasterModel(torch.nn.Module):
         self.__dict__["_serial"] = next(_MODEL_SERIAL)  # names this model in raster's static segment-table cache (ids are recycled)
         self._grad_sink = _FullArenaSink() if self.config.full_gradient_arena else _GradSink()
         self._anchor = None
+        self._noise_table = mcmc.NoiseTable()
         # eval's LPIPS (torchmetrics LearnedPerceptualImagePatchSimilarity(normalize=True), sgn_splatfacto.py:331): its AlexNet
         # weights are not part of this library; an integration that has them sets a callable (gt, rgb) -> score here
         self.lpips = None
@@ -708,12 +723,18 @@ class SceneGraphRasterModel(torch.nn.Module):
         self.__dict__["_scale_reg"] = None
         if self._fused_scale_reg_due():
             kw["scale_reg"] = self.config.max_gauss_ratio
+        # likewise MCMC's regularisers, every training step
+        self.__dict__["_mcmc_reg"] = None
+        if self._fused_mcmc_reg_due():
+            kw["terms"] = (raster.MCMCRegTerm(self.config.mcmc_opacity_reg, self.config.mcmc_scale_reg),)
         out, holder = raster.render_frame(frame, self._settings(class_streams=True), sky=sky, grad_sink=sink, anchor=anchor,
                                           pose=pose, view=view, **kw)
         if extra is not None:
             out["semantic"] = out.pop("extra")
         if "scale_reg" in kw:
             self.__dict__["_scale_reg"] = out.pop("scale_reg")
+        if "terms" in kw:
+            self.__dict__["_mcmc_reg"] = {k: out.pop(k) for k in raster.MCMCRegTerm.names}
         self._holder = holder
         self._publish_side_effects(frame, holder)
         if isinstance(holder.M, raster.LazyCount):
@@ -782,6 +803,31 @@ class SceneGraphRasterModel(torch.nn.Module):
                                   torch.tensor(c.max_gauss_ratio, device=scales.device)) - c.max_gauss_ratio
         return 0.1 * scale_reg.mean()
 
+    def _fused_mcmc_reg_due(self) -> bool:
+        """Whether this step's MCMC regularisers come out of the render: the MCMC strategy, the fused loss path and a training
+        render that records gradients."""
+        c = self.config
+        return c.strategy == "mcmc" and c.fused_loss and self.training and torch.is_grad_enabled()
+
+    def _mcmc_reg_losses(self, fused: bool) -> Dict[str, torch.Tensor]:
+        """losses["mcmc_opacity_reg"] and losses["mcmc_scale_reg"] over the visible sub-models' rows: from the render (fused), from
+        the last frame's rows without a gradient (eval / no_grad), or with torch ops over ``torch.cat`` of their parameters."""
+        c = self.config
+        if fused:
+            reg = self.__dict__.get("_mcmc_reg")
+            if reg is not None:
+                return dict(reg)
+            h = self._holder
+            if (self.training and torch.is_grad_enabled()) or h is None or h.table is None:
+                raise RuntimeError("the MCMC regularisers of this step were not rendered: call get_outputs before get_loss_dict")
+            out = raster.mcmc_reg_fwd(h.table, c.mcmc_opacity_reg, c.mcmc_scale_reg)
+            return {"mcmc_opacity_reg": out[0], "mcmc_scale_reg": out[1]}
+        mods = self.all_models._modules
+        opac = torch.cat([mods[n].gauss_params["opacities"] for n in self.visible_model_names])
+        scales = torch.cat([mods[n].gauss_params["scales"] for n in self.visible_model_names])
+        return {"mcmc_opacity_reg": c.mcmc_opacity_reg * torch.sigmoid(opac).mean(),
+                "mcmc_scale_reg": c.mcmc_scale_reg * torch.exp(scales).mean()}
+
     def _semantic_rows(self, frame: Frame) -> Optional[torch.Tensor]:
         """The frame's semantic logits [N, C] in its row order (the visible sub-models' ``semantic_logits``, concatenated in
         segment order), or None without semantic classes.  The logits are static per Gaussian: actors carry no time
@@ -833,7 +879,7 @@ class SceneGraphRasterModel(torch.nn.Module):
         running ||xys.grad|| sums, visibility counts and the max screen-space radius ratio, per sub-model."""
         assert step == self.step
         h = self._holder
-        if h is None or h.v_records is None:
+        if h is None or h.v_records is None or self.config.strategy == "mcmc":  # MCMC keeps no densification statistics
             return
         import ctypes as C
         from . import _lib
@@ -861,7 +907,7 @@ class SceneGraphRasterModel(torch.nn.Module):
 
     # ------------------------------------------------------------------------------------------
     def refinement_after(self, optimizers, step: int, generator: Optional[torch.Generator] = None, sync_stats: bool = True,
-                         due_only: bool = False) -> None:
+                         due_only: bool = False, seed: int = 0) -> None:
         """The ``refinement_after`` callbacks of all sub-models (sgn_splatfacto.py:550-646; the scene graph registers one
         per sub-model, :127-137): split / duplicate / cull / opacity reset, with the optimizer state carried along
         (dup_in_optim / remove_from_optim, :459-511).  ``optimizers`` is a ``FusedAdam`` built over
@@ -874,11 +920,16 @@ class SceneGraphRasterModel(torch.nn.Module):
 
         ``due_only``: nerfstudio runs each sub-model's callback every ITS OWN ``refine_every`` steps
         (``update_every_num_iters=self.config.refine_every``, sgn_splatfacto.py:773-781); with ``due_only`` a sub-model
-        whose ``refine_every`` does not divide ``step`` is left alone (callers that run on a global cadence pass False)."""
+        whose ``refine_every`` does not divide ``step`` is left alone (callers that run on a global cadence pass False).
+
+        With ``strategy="mcmc"`` the sub-models are refined by MCMC instead (``_mcmc_refinement``, draws keyed by ``seed``)."""
         assert step == self.step
         names = list(self.all_models._modules)
         subs = [self.all_models[n] for n in names]
         adapter = _optimizer_adapter(optimizers, len(subs))
+        if self.config.strategy == "mcmc":
+            self._mcmc_refinement(adapter, step, seed, due_only)
+            return
         if sync_stats:
             self._sync_densification_stats(subs)
         # phase 1: every sub-model's decision pass is launched, then ALL totals come back with one read-back
@@ -953,6 +1004,99 @@ class SceneGraphRasterModel(torch.nn.Module):
         if records:  # the logged counters of all sub-models: one read-back, after everything else has been enqueued
             for (sub, plan, _), counts in zip(records, torch.stack([r[2] for r in records]).tolist()):
                 sub.__dict__["refine_record_dict"] = plan.record_from(counts)
+
+    def _mcmc_settings_of(self, name: str) -> MCMCSettings:
+        return self.config.mcmc if name == "background" else self.config.object_mcmc
+
+    def _mcmc_refinement(self, adapter, step: int, seed: int, due_only: bool) -> None:
+        """gsplat's MCMCStrategy._refine per sub-model inside its window (mcmc.py): relocate the dead rows, then draw the added
+        rows; then ONE relayout of the optimizer for the sub-models that grew, whose new rows copy the drawn ones in draw order
+        with zero moments (the semantic logits and the 3D filter sizes ride along).  No opacity reset.  Nothing is read back but
+        the relocation counts with ``refine_record``."""
+        names = list(self.all_models._modules)
+        subs = [self.all_models[n] for n in names]
+        sem = self.config.semantic_classes > 0
+        relocated, added = [], []
+        for i, (name, sub) in enumerate(zip(names, subs)):
+            st = self._mcmc_settings_of(name)
+            if not mcmc.in_window(st, step) or (due_only and (st.refine_every <= 0 or step % st.refine_every != 0)):
+                relocated.append(None)
+                added.append(None)
+                continue
+            sub.__dict__["refine_record_dict"] = {}
+            params = [sub.gauss_params[k].data for k in PARAM_NAMES]
+            carried = ([sub.semantic_logits.data] if sem else []) + ([sub.filter_3d] if sub.filter_3d is not None else [])
+            relocated.append(mcmc.relocate(params, carried, mcmc.moment_tensors(adapter.moments(i)), st, seed, step, i))
+            A = mcmc.num_added(sub.num_points, st)
+            added.append((A, mcmc.draw_added(params, A, st, seed, step, i)) if A > 0 else None)
+        grow = [a is not None for a in added]
+        if any(grow):
+            old = [[sub.gauss_params[k].data for k in PARAM_NAMES] for sub in subs]
+            new = [o if a is None else [torch.empty((o[0].shape[0] + a[0],) + tuple(t.shape[1:]), device=t.device, dtype=t.dtype) for t in o]
+                   for o, a in zip(old, added)]
+            old_sem = [sub.semantic_logits.data for sub in subs] if sem else None
+            new_sem = [o if a is None else torch.empty((o.shape[0] + a[0],) + tuple(o.shape[1:]), device=o.device, dtype=o.dtype)
+                       for o, a in zip(old_sem, added)] if sem else None
+            src_m, dst_m = adapter.relayout(new, grow, {"semantic": new_sem} if sem else None)
+            for i, a in enumerate(added):
+                if a is None:
+                    continue
+                n = old[i][0].shape[0]
+                pairs = [(old[i], new[i])]
+                moments = list(zip(src_m[i] or [], dst_m[i] or []))
+                if sem:
+                    pairs.append(([old_sem[i]], [new_sem[i]]))
+                    ms, md = adapter.row_moments("semantic", i)
+                    if md is not None:
+                        moments.append((ms, md))
+                sub = subs[i]
+                f_new = None
+                if sub.filter_3d is not None:
+                    f_new = torch.empty(n + a[0], device=self.device, dtype=torch.float32)
+                    pairs.append(([sub.filter_3d], [f_new]))
+                for src, dst in pairs:
+                    for s_, d_ in zip(src, dst):
+                        d_[:n].copy_(s_)
+                for src, dst in moments:  # the old rows keep their moments, the appended rows start from zero
+                    for s_, d_ in zip(src, dst):
+                        d_[:n].copy_(s_)
+                        d_[n:].zero_()
+                rows = [d_ for _, dst in pairs for d_ in dst]
+                mcmc.copy_rows(rows, a[1], a[0], dst_row0=n)
+                for k, t in zip(PARAM_NAMES, new[i]):
+                    sub.gauss_params[k] = torch.nn.Parameter(t)
+                if sem:
+                    sub.semantic_logits = torch.nn.Parameter(new_sem[i])
+                if f_new is not None:
+                    sub.filter_3d = f_new
+            adapter.commit([[sub.gauss_params[k] for k in PARAM_NAMES] for sub in subs], grow,
+                           {"semantic": [sub.semantic_logits for sub in subs]} if sem else None)
+            self.invalidate_frames()
+        self.__dict__["refine_changed_rows"] = any(grow)
+        if self.config.refine_record:
+            done = [i for i, r in enumerate(relocated) if r is not None]
+            counts = torch.stack([relocated[i] for i in done]).tolist() if done else []
+            for i, c in zip(done, counts):
+                subs[i].__dict__["refine_record_dict"] = {"mcmc_relocated": int(c), "mcmc_added": added[i][0] if added[i] else 0}
+
+    def inject_noise(self, step: int, lr: float, seed: int = 0, normals: Optional[torch.Tensor] = None) -> None:
+        """gsplat's ``inject_noise_to_position`` on every row of every sub-model, one launch (actors in object coordinates):
+        means += Sigma (eps * gate(1 - opacity) * lr * noise_lr), with the sub-model's noise_lr and ``lr`` the means' learning
+        rate at this step.  eps ~ N(0, I) from Philox keyed by (seed, step, sub-model, row), or ``normals`` [rows, 3] (the
+        sub-models' rows back to back, all_models order)."""
+        d = self.__dict__
+        # the sub-model list and its device table change only with the parameter tensors (invalidate_frames): this runs every
+        # step, and rebuilding them costs more host time than the rest of the step's MCMC work
+        key = (d.get("_param_epoch", 0), self.all_models._modules["background"].gauss_params._parameters["means"].data_ptr())
+        if d.get("_noise_key") != key:
+            subs = []
+            for name, sub in self.all_models._modules.items():
+                g = sub.gauss_params
+                subs.append((g["means"].data, g["scales"].data, g["quats"].data, g["opacities"].data,
+                             self._mcmc_settings_of(name).noise_lr))
+            d["_noise_subs"], d["_noise_key"] = subs, key
+            self._noise_table.get(subs, self.device)
+        mcmc.inject_noise(self._noise_table, d["_noise_subs"], lr, seed, step, normals, rebuild=False)
 
     def _sync_densification_stats(self, subs) -> None:
         """Replicas rendered different cameras: identical split / cull decisions need identical statistics (SURVEY.md 8e).
@@ -1053,7 +1197,11 @@ class SceneGraphRasterModel(torch.nn.Module):
         with ``fused_loss=False``), and a zero without gradient on the other steps.
 
         With a ``bilateral_grid``, in training: ``bilagrid_tv`` = 10 * the total variation of all grids
-        (bilagrid.BilateralGrid.tv_loss), every step."""
+        (bilagrid.BilateralGrid.tv_loss), every step.
+
+        With ``strategy="mcmc"``: ``mcmc_opacity_reg`` = mcmc_opacity_reg * mean(sigmoid(opacities)) and ``mcmc_scale_reg`` =
+        mcmc_scale_reg * mean(exp(scales)) over the rows of the visible sub-models, every call (the render computed them,
+        sgn_mcmc_reg_fwd; torch ops with ``fused_loss=False``)."""
         c = self.config
         want_sky = "semantic" in batch and c.sky_acc_loss_mult > 0
         want_ent = c.object_acc_entropy_loss_mult > 0.0 and self.step > c.refine.stop_split_at  # background_model.stop_split_at (:386)
@@ -1118,6 +1266,8 @@ class SceneGraphRasterModel(torch.nn.Module):
             losses["semantic_loss"] = term(outputs["semantic"], batch["semantic"], batch.get("mask"), c.semantic_loss_mult)
         if c.use_scale_regularization:
             losses["scale_reg"] = self._scale_reg_loss(fused)
+        if c.strategy == "mcmc":
+            losses.update(self._mcmc_reg_losses(fused))
         co = self.camera_optimizer
         if self.training and co is not None and co.mode != "off":
             terms = getattr(self, "_camera_terms", None)
@@ -1256,6 +1406,10 @@ class _NoOptimizer:
     def zero_moments(self, sub: int, k: int):
         pass
 
+    def moments(self, sub: int):
+        """The (exp_avg, exp_avg_sq) pairs of sub-model ``sub``'s six tensors and of its per-row groups, those that exist."""
+        return []
+
 
 class _FusedAdamAdapter(_NoOptimizer):
     """Moments live in two flat arenas: ``relayout`` allocates the arenas of the new layout, hands out views of the old
@@ -1314,6 +1468,9 @@ class _FusedAdamAdapter(_NoOptimizer):
         m, v = self.opt.moment_views(6 * sub + k)
         m.zero_()
         v.zero_()
+
+    def moments(self, sub: int):
+        return [self.opt.moment_views(6 * sub + k) for k in range(6)] + [self.opt.row_moment_views(n, sub) for n in self.opt.row_index]
 
 
 class _TorchAdamGroupsAdapter(_NoOptimizer):
@@ -1393,6 +1550,13 @@ class _TorchAdamGroupsAdapter(_NoOptimizer):
         if "exp_avg" in st:
             st["exp_avg"] = torch.zeros_like(st["exp_avg"])
             st["exp_avg_sq"] = torch.zeros_like(st["exp_avg_sq"])
+
+    def moments(self, sub: int):
+        states = [self._state(k, sub)[1] for k in range(6)]
+        if "semantic" in self.groups:
+            opt = self.groups["semantic"]
+            states.append(opt.state.get(opt.param_groups[0]["params"][sub], {}))
+        return [(st["exp_avg"], st["exp_avg_sq"]) for st in states if "exp_avg" in st]
 
 
 def _optimizer_adapter(optimizers, num_submodels: int):

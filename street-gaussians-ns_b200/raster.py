@@ -15,7 +15,7 @@ import copy
 import ctypes as C
 import os
 from dataclasses import dataclass
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -707,6 +707,97 @@ def scale_reg_bwd(table: SegmentTable, arena: torch.Tensor, max_ratio: float, v_
                                        _stream()), "sgn_scale_reg_bwd")
 
 
+def mcmc_reg_fwd(table: SegmentTable, w_opacity: float, w_scale: float) -> torch.Tensor:
+    """MCMC's regularisers over the frame's rows, [w_opacity * mean(sigmoid(opacities)), w_scale * mean(exp(scales))]: a float32
+    pair on the device, no read-back (sgn_mcmc_reg_fwd)."""
+    L = _lib.load()
+    device = table.dev.device
+    out = torch.empty(2, device=device, dtype=torch.float32)
+    sb = L.sgn_mcmc_reg_scratch_bytes()
+    scratch = torch.empty(sb, device=device, dtype=torch.uint8)
+    with _timed("mcmc_reg_fwd"):
+        _lib.check(L.sgn_mcmc_reg_fwd(_ptr(table.dev), table.nseg, table.N, table.num_chunks, float(w_opacity), float(w_scale), _ptr(out),
+                                      _ptr(scratch), sb, _stream()), "sgn_mcmc_reg_fwd")
+    return out
+
+
+def mcmc_reg_bwd(table: SegmentTable, arena: torch.Tensor, w_opacity: float, w_scale: float, v_opacity: Optional[torch.Tensor],
+                 v_scale: Optional[torch.Tensor], out_offsets: Optional[np.ndarray] = None) -> None:
+    """ADDS the gradients of the two MCMC regularisers times their cotangents (float32 device scalars, None = no cotangent) into
+    the opacities and scales slices of the gradient arena (laid out as project_bwd's); sgn_mcmc_reg_bwd."""
+    L = _lib.load()
+    vo = None if v_opacity is None else v_opacity.detach().reshape(()).to(torch.float32).contiguous()
+    vs = None if v_scale is None else v_scale.detach().reshape(()).to(torch.float32).contiguous()
+    gt = _arena_grads_table(arena, table.static, arena.device, out_offsets)
+    with _timed("mcmc_reg_bwd"):
+        _lib.check(L.sgn_mcmc_reg_bwd(_ptr(table.dev), _ptr(gt), table.nseg, table.N, table.num_chunks, float(w_opacity), float(w_scale),
+                                      _ptr(vo), _ptr(vs), _stream()), "sgn_mcmc_reg_bwd")
+
+
+class ParamTerm:
+    """A loss term of the Gaussian parameters alone, evaluated over the frame's rows through its segment table, as outputs of the
+    render node (``render_frame(terms=...)``).  It is an output of the node rather than a function of its own because project_bwd
+    OVERWRITES the gradient arena: as an output, the render's backward waits for the term's cotangents and adds its gradient into
+    the arena after project_bwd, before the arena is handed on.  ``names``: the outputs, in order; ``kinds``: the PARAM_NAMES
+    positions its gradient reaches."""
+
+    names: Tuple[str, ...] = ()
+    kinds: Tuple[int, ...] = ()
+
+    def forward(self, table: SegmentTable) -> List[torch.Tensor]:
+        raise NotImplementedError
+
+    def backward(self, table: SegmentTable, arena: torch.Tensor, v: Sequence[Optional[torch.Tensor]],
+                 out_offsets: Optional[np.ndarray] = None) -> None:
+        raise NotImplementedError
+
+
+class ScaleRegTerm(ParamTerm):
+    """nerfstudio's scale regularisation (scale_reg_fwd / scale_reg_bwd)."""
+
+    names, kinds = ("scale_reg",), (1,)
+
+    def __init__(self, max_ratio: float):
+        self.max_ratio = max_ratio
+
+    def forward(self, table):
+        return [scale_reg_fwd(table, self.max_ratio)]
+
+    def backward(self, table, arena, v, out_offsets=None):
+        scale_reg_bwd(table, arena, self.max_ratio, v[0], out_offsets)
+
+
+class MCMCRegTerm(ParamTerm):
+    """MCMC's opacity and scale regularisers (mcmc_reg_fwd / mcmc_reg_bwd), two scalar outputs."""
+
+    names, kinds = ("mcmc_opacity_reg", "mcmc_scale_reg"), (1, 5)
+
+    def __init__(self, w_opacity: float, w_scale: float):
+        self.w_opacity, self.w_scale = w_opacity, w_scale
+
+    def forward(self, table):
+        out = mcmc_reg_fwd(table, self.w_opacity, self.w_scale)
+        return [out[0], out[1]]
+
+    def backward(self, table, arena, v, out_offsets=None):
+        mcmc_reg_bwd(table, arena, self.w_opacity, self.w_scale, v[0], v[1], out_offsets)
+
+
+_TERM_NAMES = ScaleRegTerm.names + MCMCRegTerm.names
+
+
+def _terms_of(scale_reg: Optional[float], terms: Sequence[ParamTerm]) -> Tuple[ParamTerm, ...]:
+    return tuple(terms) + ((ScaleRegTerm(scale_reg),) if scale_reg is not None else ())
+
+
+def _split_term_cotangents(terms: Sequence[ParamTerm], v: Sequence[Optional[torch.Tensor]]) -> List[List[Optional[torch.Tensor]]]:
+    out, i = [], 0
+    for t in terms:
+        out.append(list(v[i:i + len(t.names)]))
+        i += len(t.names)
+    return out
+
+
 def _zero_arena(static: dict, device, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """The gradient arena of a backward with no image-space cotangent: ``out`` zeroed (all of it, also the slices of sub-models
     outside the frame when ``out`` has the layout of the whole model), or a new zero arena in the frame's layout."""
@@ -803,15 +894,16 @@ class _Holder:
         # model path: an object with target(static) -> arena-or-None and publish(arena, static); the parameter
         # gradients are then delivered through it instead of through 6 x segments autograd leaves
         self.grad_sink = None
-        # the last backward had no image-space cotangent (only the scale regularisation's): the blend and projection were
-        # skipped, and the arena holds zeros but for the scales
+        # the last backward had no image-space cotangent (only parameter terms', e.g. the scale regularisation's): the blend and
+        # projection were skipped, and the arena holds zeros but for the tensors ``term_kinds`` names (PARAM_NAMES positions)
         self.params_only = False
+        self.term_kinds: List[int] = []
 
 
 class _SceneGraphRasterize(torch.autograd.Function):
     @staticmethod
     def forward(ctx, frame: Frame, settings: RenderSettings, holder: _Holder, sky: Optional[torch.Tensor],
-                extra: Optional[torch.Tensor], pose: Optional[torch.Tensor], view: Optional[torch.Tensor], scale_reg: Optional[float],
+                extra: Optional[torch.Tensor], pose: Optional[torch.Tensor], view: Optional[torch.Tensor], terms: Tuple[ParamTerm, ...],
                 *flat):
         # unused outputs must reach backward as None, not as zero tensors: the kernels specialise on
         # which cotangents exist (depth / background_acc have none in training)
@@ -868,23 +960,25 @@ class _SceneGraphRasterize(torch.autograd.Function):
             extra = extra.contiguous()
             ctx.extra = extra.detach()
             outs.append(blend_extra_fwd(cs, bo, records, sorted_ids, tile_bins, out["final_T"], out["final_idx"], ctx.extra))
-        ctx.scale_reg = scale_reg
-        if scale_reg is not None:  # the scale regularisation: a term of the parameters alone, from the frame's table
-            outs.append(scale_reg_fwd(table, scale_reg))
+        ctx.terms = terms
+        for t in terms:  # terms of the parameters alone (the scale regularisation, ...), from the frame's table
+            outs += t.forward(table)
         return tuple(outs)
 
     @staticmethod
     def backward(ctx, *v):
-        v_scale_reg = v_extra_img = None
-        if ctx.scale_reg is not None:
-            v, v_scale_reg = v[:-1], v[-1]
+        v_extra_img = None
+        n_terms = sum(len(t.names) for t in ctx.terms)
+        v_terms = _split_term_cotangents(ctx.terms, v[len(v) - n_terms:])
+        v = v[:len(v) - n_terms]
+        due = [(t, vt) for t, vt in zip(ctx.terms, v_terms) if any(x is not None for x in vt)]
         if ctx.extra is not None:
             v, v_extra_img = v[:-1], v[-1]
         names = ["rgb", "accumulation", "depth", "object_acc", "background_acc"][: len(v)]
         vd = {k: t for k, t in zip(names, v)}
-        # only the scale regularisation has a cotangent (nothing in view, or a backward of that term alone): every image-space
-        # gradient is zero, so the blend and the projection are skipped and the arena starts from zeros
-        params_only = ctx.scale_reg is not None and v_extra_img is None and all(t is None for t in vd.values())
+        # only parameter terms have a cotangent (nothing in view, or a backward of the terms alone): every image-space gradient is
+        # zero, so the blend and the projection are skipped and the arena starts from zeros
+        params_only = bool(ctx.terms) and v_extra_img is None and all(t is None for t in vd.values())
         v_extra = v_sky = None
         if params_only:
             v_records = torch.zeros_like(ctx.records)
@@ -918,8 +1012,8 @@ class _SceneGraphRasterize(torch.autograd.Function):
                 _, arena = project_bwd(ctx.table, ctx.params, ctx.cs, ctx.records, ctx.radii, v_records, make_views=False,
                                        out=target, out_offsets=offsets, chunk_ranges=chunk_ranges, after_range=after_range,
                                        v_pose=v_pose, view=view, v_view=v_view)
-            if v_scale_reg is not None:  # project_bwd overwrote the arena: the term's gradient is added after it
-                scale_reg_bwd(ctx.table, arena, ctx.scale_reg, v_scale_reg, offsets)
+            for t, vt in due:  # project_bwd overwrote the arena: the terms' gradients are added after it
+                t.backward(ctx.table, arena, vt, offsets)
             sink.publish(arena, ctx.table.static)
             flat = (None,)
         else:
@@ -929,11 +1023,12 @@ class _SceneGraphRasterize(torch.autograd.Function):
             else:
                 flat, arena = project_bwd(ctx.table, ctx.params, ctx.cs, ctx.records, ctx.radii, v_records, v_pose=v_pose, view=view,
                                           v_view=v_view)
-            if v_scale_reg is not None:
-                scale_reg_bwd(ctx.table, arena, ctx.scale_reg, v_scale_reg)
+            for t, vt in due:
+                t.backward(ctx.table, arena, vt)
         if params_only:  # no image term reached the poses or the view
             v_pose = v_view = None
         h.params_only = params_only
+        h.term_kinds = sorted({k for t, _ in due for k in t.kinds})
         h.v_records, h.grad_arena, h.v_pose, h.v_view = v_records, arena, v_pose, v_view
         if v_pose is not None:
             g_pose = v_pose[posed_rows(ctx.table)[0]]
@@ -947,13 +1042,14 @@ class _SceneGraphRasterize(torch.autograd.Function):
 
 def forward_backward(frame: Frame, settings: RenderSettings, cotangents: Dict[str, Optional[torch.Tensor]],
                      sky: Optional[torch.Tensor] = None, want_param_grads: bool = False, grad_out: Optional[torch.Tensor] = None,
-                     chunk_ranges=None, after_range=None, after_project=None, scale_reg: Optional[float] = None):
+                     chunk_ranges=None, after_range=None, after_project=None, scale_reg: Optional[float] = None,
+                     terms: Sequence[ParamTerm] = ()):
     """One frame, forward AND backward, straight through the C-ABI stages (no autograd graph).
 
     ``cotangents`` maps output names (rgb, accumulation, depth, object_acc, background_acc, and scale_reg with ``scale_reg``) to
     their cotangent tensors (missing / None = no gradient from that output).  ``scale_reg`` (max_ratio, None = off): the outputs
     also hold the scale regularisation (see ``render_frame``); its cotangent, a device scalar, adds the term's gradient to the
-    arena after project_bwd.  Returns (outputs, holder);
+    arena after project_bwd.  ``terms`` (raster.ParamTerm): further terms of the parameters alone, likewise.  Returns (outputs, holder);
     ``holder.grad_arena`` is the flat dense gradient arena (what the data-parallel all-reduce and a
     fused optimizer consume), ``holder.v_records[:, 0:2]`` the pixel-space mean gradients the
     densification statistics read.  With ``want_param_grads`` the per-parameter views are returned in
@@ -976,13 +1072,16 @@ def forward_backward(frame: Frame, settings: RenderSettings, cotangents: Dict[st
     if settings.class_streams:
         cls_ids, cls_bins = class_lists(cs, M, sorted_ids, tile_bins)
     out = blend_fwd(cs, bo, records, sorted_ids, tile_bins, sky, cls_ids, cls_bins)
-    reg = scale_reg_fwd(table, scale_reg) if scale_reg is not None else None
+    terms = _terms_of(scale_reg, terms)
+    regs = [t.forward(table) for t in terms]
     v = {k: cotangents.get(k) for k in ("rgb", "accumulation", "depth", "object_acc", "background_acc")}
-    v_scale_reg = cotangents.get("scale_reg")
-    assert v_scale_reg is None or scale_reg is not None, "a scale_reg cotangent needs scale_reg (max_ratio)"
-    # the term's gradient is added after project_bwd: with ranges, the exchange of a range may already be reading it
-    assert scale_reg is None or (chunk_ranges is None and after_range is None), "scale_reg does not combine with ranged exchange"
-    if scale_reg is not None and all(t is None for t in v.values()):  # as the render's backward: nothing image-space to propagate
+    v_terms = [[cotangents.get(n) for n in t.names] for t in terms]
+    named = {n for t in terms for n in t.names}
+    for n in _TERM_NAMES:
+        assert cotangents.get(n) is None or n in named, f"a {n} cotangent needs its term (scale_reg= / terms=)"
+    # the terms' gradients are added after project_bwd: with ranges, the exchange of a range may already be reading it
+    assert not terms or (chunk_ranges is None and after_range is None), "parameter terms do not combine with ranged exchange"
+    if terms and all(t is None for t in v.values()):  # as the render's backward: nothing image-space to propagate
         v_records, v_sky = torch.zeros_like(records), None
         arena = _zero_arena(table.static, device, grad_out)
         flat = arena_views(arena, table.static) if want_param_grads else None
@@ -991,8 +1090,9 @@ def forward_backward(frame: Frame, settings: RenderSettings, cotangents: Dict[st
                                      deterministic=settings.deterministic)
         flat, arena = project_bwd(table, params, cs, records, radii, v_records, make_views=want_param_grads, out=grad_out,
                                   chunk_ranges=chunk_ranges, after_range=after_range)
-    if v_scale_reg is not None:
-        scale_reg_bwd(table, arena, scale_reg, v_scale_reg)
+    for t, vt in zip(terms, v_terms):
+        if any(x is not None for x in vt):
+            t.backward(table, arena, vt)
     holder = _Holder()
     holder.records, holder.radii, holder.num_tiles_hit, holder.M = records, radii, tiles_hit, M
     holder.xys, holder.conics, holder.depths = records[:, 0:2], records[:, 2:5], records[:, 9]
@@ -1001,8 +1101,8 @@ def forward_backward(frame: Frame, settings: RenderSettings, cotangents: Dict[st
     holder.param_grads = flat
     holder.tile_bins, holder.tile_depth = tile_bins, out["tile_depth"]  # diagnostics (tools/depth_stats.py)
     res = {k: out[k] for k in ("rgb", "accumulation", "depth", "object_acc", "background_acc") if k in out}
-    if scale_reg is not None:
-        res["scale_reg"] = reg
+    for t, r in zip(terms, regs):
+        res.update(zip(t.names, r))
     return res, holder
 
 
@@ -1044,7 +1144,8 @@ def blend_extra_bwd(cs, bo, records, sorted_ids, tile_bins, final_T, final_idx, 
 
 def render_frame(frame: Frame, settings: Optional[RenderSettings] = None, sky: Optional[torch.Tensor] = None,
                  grad_sink=None, anchor: Optional[torch.Tensor] = None, extra: Optional[torch.Tensor] = None,
-                 pose: Optional[torch.Tensor] = None, view: Optional[torch.Tensor] = None, scale_reg: Optional[float] = None):
+                 pose: Optional[torch.Tensor] = None, view: Optional[torch.Tensor] = None, scale_reg: Optional[float] = None,
+                 terms: Sequence[ParamTerm] = ()):
     """Render one camera.  Returns (outputs dict, holder).  Segment parameters must be CUDA tensors.
 
     ``scale_reg`` (max_ratio; None = off, and the call sequence is unchanged): ``out["scale_reg"]`` is nerfstudio's scale
@@ -1054,6 +1155,9 @@ def render_frame(frame: Frame, settings: Optional[RenderSettings] = None, sky: O
     its gradient (sgn_scale_reg_bwd) into the arena after project_bwd, before the arena is handed on.  When the term is the
     only output with a cotangent (nothing in view, or a backward of the term alone) the blend and projection backward are
     skipped and the arena holds zeros plus the term's gradient.
+
+    ``terms`` (raster.ParamTerm, e.g. ``MCMCRegTerm``): further terms of the parameters alone, computed and differentiated the
+    same way; ``out`` holds each term's outputs under its names.  Without terms and ``scale_reg`` the call sequence is unchanged.
 
     ``view`` [15] (float32, on the device): the world->camera view to project with -- viewmat 3x4 row-major, then cam_pos
     (the SH view directions' origin) -- in place of the one ``frame.camera`` gives; intrinsics and image size still come
@@ -1081,10 +1185,11 @@ def render_frame(frame: Frame, settings: Optional[RenderSettings] = None, sky: O
     holder = _Holder()
     holder.grad_sink = grad_sink
     flat = [anchor] if grad_sink is not None else [t for seg in frame.segments for t in seg.params.tensors()]
-    outs = _SceneGraphRasterize.apply(frame, settings, holder, sky, extra, pose, view, scale_reg, *flat)
-    reg = None
-    if scale_reg is not None:
-        outs, reg = outs[:-1], outs[-1]
+    terms = _terms_of(scale_reg, terms)
+    outs = _SceneGraphRasterize.apply(frame, settings, holder, sky, extra, pose, view, terms, *flat)
+    n_terms = sum(len(t.names) for t in terms)
+    regs = outs[len(outs) - n_terms:]
+    outs = outs[:len(outs) - n_terms]
     extra_img = None
     if extra is not None:
         outs, extra_img = outs[:-1], outs[-1]
@@ -1092,8 +1197,7 @@ def render_frame(frame: Frame, settings: Optional[RenderSettings] = None, sky: O
     out = {k: t for k, t in zip(names, outs)}
     if extra_img is not None:
         out["extra"] = extra_img
-    if reg is not None:
-        out["scale_reg"] = reg
+    out.update(zip([n for t in terms for n in t.names], regs))
     if sky is not None:
         out["sky"] = sky
     return out, holder

@@ -21,10 +21,10 @@ from typing import Dict, List, Optional, Sequence
 import torch
 import torch.distributed as dist
 
-from . import dp
+from . import dp, mcmc
 from .model import SceneGraphRasterModel, _FullArenaSink
 from .optim import FusedAdam
-from .scene import PARAM_NAMES, Camera
+from .scene import Camera
 
 
 class TrainStep:
@@ -105,6 +105,10 @@ class TrainStep:
             # would normalise by its own visible row count
             raise NotImplementedError("data-parallel training does not exchange the gradient of the scale regularisation: the "
                                       "replicas would diverge")
+        if world > 1 and m.config.strategy == "mcmc":
+            # the relocation and growth would be exchanged as densification statistics are, and the regularisers' gradients reach
+            # rows no replica saw
+            raise NotImplementedError("data-parallel training does not support strategy='mcmc': the replicas would diverge")
         if world > 1:
             self._ensure_exchange()
         m.step = step                                     # step_cb (sgn_splatfacto.py:754-755)
@@ -149,8 +153,8 @@ class TrainStep:
                 kinds = None if len(got) == 6 else got
             elif h is not None and h.grad_arena is not None:
                 arena = h.grad_arena
-                if getattr(h, "params_only", False):  # only the scale regularisation reached the render (nothing in view): only the scales step
-                    kinds = [PARAM_NAMES.index("scales")]
+                if getattr(h, "params_only", False):  # only parameter terms reached the render (nothing in view): only their tensors step
+                    kinds = list(h.term_kinds)
             # with nothing in view a loss term of another tensor (the camera regulariser) can still carry a gradient
             rendered = outside or (h is not None and h.grad_arena is not None)
         if not rendered:
@@ -168,6 +172,7 @@ class TrainStep:
                 if base is not None:
                     opt.step(base, present=[], full_layout=True, extra_grads=due or None, row_grads=due_rows or None)
                 self._maybe_refine(step)
+                self._inject_noise(step)
                 return losses
             arena = m.zero_gradient_arena()
         # the further tensors of the optimizer (the sky cube map, sky.CubeMapSky.base) step with the gradient autograd left
@@ -197,6 +202,7 @@ class TrainStep:
         if rendered and not (type(M) is int and M == 0):
             m.after_train(step)                           # AFTER_TRAIN_ITERATION callbacks, in the reference's order
         self._maybe_refine(step)
+        self._inject_noise(step)
         return losses
 
     def _due_extra_grads(self, step: int, extras: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
@@ -304,17 +310,29 @@ class TrainStep:
         self._gen.manual_seed((self.refine_seed * 1_000_003 + step) & 0x7FFFFFFFFFFFFFFF)
         return self._gen
 
+    def _inject_noise(self, step: int) -> None:
+        """MCMC's position noise, every step after the optimizer step and any refinement (gsplat's MCMCStrategy.step_post_backward),
+        with the means' learning rate of this step."""
+        if self.model.config.strategy == "mcmc":
+            self.model.inject_noise(step, self.optimizer.lrs["means"], seed=self.refine_seed)
+
     def _maybe_refine(self, step: int) -> None:
         m = self.model
+        mc = m.config.strategy == "mcmc"
         if self.refine_every is not None:
             due = self.refine_every > 0 and step % self.refine_every == 0
+        elif mc:
+            due = any(mcmc.due(st, step) for st in (m.config.mcmc, m.config.object_mcmc))
         else:
             due = any(st.refine_every > 0 and step % st.refine_every == 0 for st in (m.config.refine, m.config.object_refine))
         if not due:
             self._maybe_filter(step, False)
             return
         m.__dict__["refine_changed_rows"] = False
-        m.refinement_after(self.optimizer, step, generator=self._refine_generator(step), due_only=self.refine_every is None)
+        if mc:
+            m.refinement_after(self.optimizer, step, due_only=self.refine_every is None, seed=self.refine_seed)
+        else:
+            m.refinement_after(self.optimizer, step, generator=self._refine_generator(step), due_only=self.refine_every is None)
         self._maybe_filter(step, bool(m.__dict__.get("refine_changed_rows")))
         if self.world_size() > 1 and self.check_replicas:
             # replicas must have taken identical decisions: same row count in every sub-model
@@ -347,7 +365,8 @@ def warm_up_refinement(model: SceneGraphRasterModel, rows: Sequence[int] = (6553
     Why: CUDA loads a kernel's module at its first launch.  The first refinement of a process is the first launch of ~20
     kernels nothing else on the training step uses (the decide / apply kernels, scans, reductions, the normal sampler,
     bitwise and comparison kernels, ...), which cost tens of milliseconds of host time in the middle of training.  Calling this once after the
-    model is built moves that one-time cost out of the loop, like the warm-up steps of a benchmark."""
+    model is built moves that one-time cost out of the loop, like the warm-up steps of a benchmark.  With ``strategy="mcmc"`` the
+    refinement is the MCMC one (at its first due step unless ``step`` is given), followed by one position-noise launch."""
     from dataclasses import replace
 
     from .scene import GaussianSet
@@ -363,12 +382,26 @@ def warm_up_refinement(model: SceneGraphRasterModel, rows: Sequence[int] = (6553
     for n, like in zip(rows, widths):
         F, R = int(like.gauss_params["features_dc"].shape[1]), int(like.gauss_params["features_rest"].shape[1])
         sets.append(GaussianSet(rand(n, 3) * 5, rand(n, 3) * 1.5 - 4.0, rand(n, 4), rand(n, F, 3), rand(n, R, 3), rand(n, 1) * 2.5 - 1.0))
-    st = model.config.refine
-    step = step if step is not None else st.warmup_length + st.refine_every * max(1, -(-(model.config.num_train_data + st.refine_every + 1) // st.refine_every))
+    mc = model.config.strategy == "mcmc"
+    if mc:
+        ms = model.config.mcmc
+        step = step if step is not None else (ms.refine_start // ms.refine_every + 1) * ms.refine_every
+    else:
+        st = model.config.refine
+        step = step if step is not None else st.warmup_length + st.refine_every * max(1, -(-(model.config.num_train_data + st.refine_every + 1) // st.refine_every))
     cfg = replace(model.config, full_gradient_arena=False, refine_record=True)
     tmp = SceneGraphRasterModel(sets[0], {str(i): s for i, s in enumerate(sets[1:])}, cfg).to(dev)
     tmp.train()
     tmp.step = step
+    if mc:  # a few per cent of the random opacity logits are below logit(min_opacity): every kernel of both phases runs
+        opt = FusedAdam(tmp.optimizer_params())
+        tmp.refinement_after(opt, step, seed=12345)
+        tmp.inject_noise(step, opt.lrs["means"], seed=12345)
+        if dev.type == "cuda":
+            torch.cuda.synchronize(dev)
+        return {"step": step, "rows_before": [int(n) for n in rows[:len(sets)]],
+                "rows_after": [s.num_points for s in tmp.all_models.values()],
+                "records": [dict(s.refine_record_dict) for s in tmp.all_models.values()]}
     for sub in tmp.all_models.values():
         n, d = sub.num_points, sub.__dict__
         vis = torch.randint(1, 9, (n,), device=dev, generator=g).float()

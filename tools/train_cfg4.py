@@ -28,7 +28,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True, sky: bool = False, metrics: bool = False,
         bbox_opt: bool = False, camera_opt: bool = False, sky_view_grad: bool = False, lidar_depth: float = 0.0,
         semantic: float = 0.0, antialiased: bool = False, scale_reg: bool = False, filter_3d: bool = False,
-        bilateral_grid: bool = False) -> dict:
+        bilateral_grid: bool = False, mcmc: bool = False) -> dict:
     """One measurement.  torch.distributed must already be initialised when WORLD_SIZE > 1.  Returns the result dict on
     rank 0 (None elsewhere).  ``sky``: the reference's default learnable sky (use_sky_sphere, a 1024^2 cube map stepped by
     the same Adam launch at the ``sky_sphere`` group's lr 0.005, sgn_config.py:72-75).  ``metrics``: every step also computes
@@ -50,7 +50,9 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     10 before and after the run.  ``filter_3d``: Mip-Splatting's 3D smoothing filter from the 425 rig cameras (SceneGraphConfig
     .filter_3d), recomputed after every refinement that changed a row count and every 100 steps.  ``bilateral_grid``: one
     bilateral grid per rig image (425, bilagrid.BilateralGrid with gsplat's 16 x 16 x 8) corrects every training render, with
-    the grids' total-variation term; stepped by the same Adam launch at gsplat's lr 2e-3."""
+    the grids' total-variation term; stepped by the same Adam launch at gsplat's lr 2e-3.  ``mcmc``: densification by MCMC
+    (SceneGraphConfig(strategy="mcmc"), gsplat's defaults with the actors' 100 k cap): no densification statistics, relocation
+    and 5 % growth at every refinement, position noise every step, the opacity and scale regularisers in the loss."""
     import torch
     import torch.distributed as dist
 
@@ -82,7 +84,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                            num_train_data=len(cams), refine_record=True, depth_loss_mult=lidar_depth,
                            semantic_classes=3 if semantic > 0 else 0, semantic_loss_mult=semantic,
                            rasterize_mode="antialiased" if antialiased else "classic", use_scale_regularization=scale_reg,
-                           filter_3d=filter_3d)
+                           filter_3d=filter_3d, strategy="mcmc" if mcmc else "default")
     env_map = None
     if sky:
         from street_gaussians_ns_b200.sky import CubeMapSky
@@ -260,6 +262,8 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                    **({"filter_3d": "Mip-Splatting 3D filter from the 425 rig cameras, variance 0.2, recomputed every 100 steps "
                                     "and after refinements"} if filter_3d else {}),
                    **({"bilateral_grid": "BilateralGrid(425, 16 x 16 x 8), 10 * total variation, Adam lr 2e-3"} if bilateral_grid else {}),
+                   **({"strategy": "mcmc: relocation + 5 % growth per refinement (caps 1 M / 100 k), noise every step, "
+                                   "opacity and scale regularisers 0.01"} if mcmc else {}),
                    "loss": "fused kernels" if fused_loss else "torch ops", "metrics": "get_metrics_dict every step" if metrics else "none",
                    "start_step": start_step, "refine_every": refine_every,
                    "refinement_kernels_loaded_before_timing": refine_warm,
@@ -302,6 +306,7 @@ def main():
     ap.add_argument("--scale-reg", action="store_true", help="nerfstudio's scale regularisation (max_gauss_ratio 10, every tenth step)")
     ap.add_argument("--filter-3d", action="store_true", help="Mip-Splatting's 3D smoothing filter from the 5 x 85 rig cameras")
     ap.add_argument("--bilateral-grid", action="store_true", help="a bilateral grid per rig image (425) corrects each training render")
+    ap.add_argument("--mcmc", action="store_true", help="densification by MCMC (SceneGraphConfig(strategy='mcmc'))")
     args = ap.parse_args()
     if args.sky_view_grad and not (args.sky and args.camera_opt):
         ap.error("--sky-view-grad needs --sky and --camera-opt")
@@ -318,7 +323,7 @@ def main():
               args.overlap, not args.host_table, ssim_lambda=args.ssim_lambda, fused_loss=not args.torch_loss, sky=args.sky,
               metrics=args.metrics, bbox_opt=args.bbox_opt, camera_opt=args.camera_opt,
               sky_view_grad=args.sky_view_grad, lidar_depth=args.lidar_depth, semantic=args.semantic, antialiased=args.antialiased,
-              scale_reg=args.scale_reg, filter_3d=args.filter_3d, bilateral_grid=args.bilateral_grid)
+              scale_reg=args.scale_reg, filter_3d=args.filter_3d, bilateral_grid=args.bilateral_grid, mcmc=args.mcmc)
     if res is not None:
         print(json.dumps(res))
     if world > 1:
