@@ -367,6 +367,20 @@ int sgn_blend_bwd(const sgn_camera* cam, const sgn_blend_opts* opts, const float
                   const int32_t* cls_ids /*[2,M] or NULL*/, const int32_t* cls_bins /*[2,tiles,2] or NULL*/,
                   const sgn_blend_bwd_in* in, float* v_records, void* stream);
 
+/* sgn_blend_bwd that also accumulates the absolute screen-space gradient (AbsGS, Ye et al. 2024; gsplat's absgrad):
+ *   v_absxy[k] = (sum_p |g_x(k,p)|, sum_p |g_y(k,p)|)
+ * with g(k,p) the gradient of pixel p's MAIN-stream outputs (rgb, accumulation, depth) with respect to row k's screen-space
+ * mean: the per-pixel terms whose sum over p is v_records[k, 0:2].  The objects-only stream (v_object_acc), the
+ * background-only stream and the extra channels add nothing to it.  v_records and v_sky are those sgn_blend_bwd produces
+ * (bit-identical in deterministic mode).  v_absxy [N,2], 8-byte aligned: ZERO on entry in float mode (accumulated into),
+ * written in deterministic mode.  fixed_absxy [N,2] int64, ZERO on entry: deterministic mode (in->v_fixed) only, else NULL.
+ * v_background_acc must be NULL.  A bad argument returns SGN_ERR_INVALID and launches nothing. */
+int sgn_blend_bwd_absgrad(const sgn_camera* cam, const sgn_blend_opts* opts, const float* records,
+                          const int32_t* sorted_ids, const int32_t* tile_bins, int64_t M,
+                          const int32_t* cls_ids /*[2,M] or NULL*/, const int32_t* cls_bins /*[2,tiles,2] or NULL*/,
+                          const sgn_blend_bwd_in* in, float* v_records, float* v_absxy /*[N,2]*/,
+                          int64_t* fixed_absxy /*[N,2], zero on entry; deterministic mode only, else NULL*/, void* stream);
+
 /* Generic per-Gaussian channels (the north-star's per-Gaussian semantic logits; the reference's dormant consumer:
  * scripts/render.py:188,231-236): extra[N,C] is composited with the weights of the main render -- out[p,c] = sum_k
  * extra[k,c] alpha_k T_k over the entries the main pass blended (final_T / final_idx slot 0 of sgn_blend_fwd) -- 8 channels per
@@ -519,6 +533,10 @@ typedef struct sgn_densify_segment {
 size_t sgn_sizeof_densify_segment(void);
 int sgn_densify_stats(const sgn_densify_segment* table_dev, int nseg, int N, const float* v_records /*[N,12]*/,
                       const int32_t* radii /*[N]*/, int height, int width, void* stream);
+/* The same statistics from the absolute screen-space gradient of sgn_blend_bwd_absgrad: ||v_absxy[g]|| in place of
+ * ||v_records[g, 0:2]||.  v_absxy 8-byte aligned. */
+int sgn_densify_stats_abs(const sgn_densify_segment* table_dev, int nseg, int N, const float* v_absxy /*[N,2]*/,
+                          const int32_t* radii /*[N]*/, int height, int width, void* stream);
 
 /* ---- fused multi-tensor Adam (SURVEY.md 8f rank 1) ------------------------------------------------------
  * torch.optim.Adam semantics (betas, eps, no weight decay, no amsgrad) for every Gaussian parameter tensor in

@@ -156,11 +156,11 @@ EXPORTS = [
     "sgn_last_error", "sgn_abi_version", "sgn_launch_count", "sgn_sizeof_segment", "sgn_sizeof_segment_grads", "sgn_sizeof_camera",
     "sgn_upload", "sgn_bin_count", "sgn_project_fwd", "sgn_project_bwd", "sgn_l1_project_fwd", "sgn_l1_project_bwd", "sgn_l1_project_bwd_comp", "sgn_l1_sh", "sgn_bin_scan_scratch_bytes", "sgn_bin_scan",
     "sgn_bin_sort_scratch_bytes", "sgn_bin_sort", "sgn_bin_class_scratch_bytes", "sgn_bin_class_lists", "sgn_blend_sched_ints",
-    "sgn_blend_fwd", "sgn_blend_bwd", "sgn_sizeof_adam_tensor", "sgn_adam_chunk_elems", "sgn_adam_step",
+    "sgn_blend_fwd", "sgn_blend_bwd", "sgn_blend_bwd_absgrad", "sgn_sizeof_adam_tensor", "sgn_adam_chunk_elems", "sgn_adam_step",
     "sgn_loss_scratch_bytes", "sgn_loss_fwd", "sgn_loss_bwd", "sgn_ssim_workspace_bytes", "sgn_ssim_fwd", "sgn_ssim_bwd",
     "sgn_metrics_scratch_bytes", "sgn_metrics", "sgn_sky_fwd", "sgn_sky_bwd", "sgn_cube_texture_fwd", "sgn_cube_texture_bwd",
     "sgn_sky_det_scratch_bytes", "sgn_sky_bwd_det", "sgn_cube_texture_bwd_det",
-    "sgn_sizeof_densify_segment", "sgn_densify_stats",
+    "sgn_sizeof_densify_segment", "sgn_densify_stats", "sgn_densify_stats_abs",
     "sgn_sizeof_refine_config", "sgn_sizeof_refine_tensors", "sgn_refine_decide", "sgn_refine_apply",
     "sgn_bin_local_cap", "sgn_bin_local_scratch_bytes", "sgn_bin_local_count", "sgn_bin_local_sort",
     "sgn_project_bwd_range", "sgn_allreduce_sym", "sgn_blend_extra_fwd", "sgn_blend_extra_bwd", "sgn_blend_extra_bwd_det",
@@ -258,12 +258,16 @@ def load():
                                 C.POINTER(BlendFwdOut), vp]
     L.sgn_blend_bwd.argtypes = [C.POINTER(CameraStruct), C.POINTER(BlendOpts), vp, vp, vp, i64, vp, vp,
                                 C.POINTER(BlendBwdIn), vp, vp]
+    L.sgn_blend_bwd_absgrad.argtypes = [C.POINTER(CameraStruct), C.POINTER(BlendOpts), vp, vp, vp, i64, vp, vp,
+                                        C.POINTER(BlendBwdIn), vp, vp, vp, vp]
     for f in ("sgn_upload", "sgn_project_fwd", "sgn_project_bwd", "sgn_bin_scan", "sgn_bin_sort", "sgn_bin_class_lists",
-              "sgn_blend_fwd", "sgn_blend_bwd"):
+              "sgn_blend_fwd", "sgn_blend_bwd", "sgn_blend_bwd_absgrad"):
         getattr(L, f).restype = C.c_int
     L.sgn_sizeof_densify_segment.restype = sz
     L.sgn_densify_stats.argtypes = [vp, i32, i32, vp, vp, i32, i32, vp]
     L.sgn_densify_stats.restype = C.c_int
+    L.sgn_densify_stats_abs.argtypes = [vp, i32, i32, vp, vp, i32, i32, vp]
+    L.sgn_densify_stats_abs.restype = C.c_int
     L.sgn_loss_scratch_bytes.restype = sz
     L.sgn_loss_fwd.argtypes = [i32, i32, C.POINTER(LossIn), vp, vp, sz, vp]
     L.sgn_loss_fwd.restype = C.c_int

@@ -974,6 +974,17 @@ struct BlendBwdParams {
     long long* v_fixed;        // deterministic mode: [N,12] fixed-point accumulators instead of float atomics (or null)
     const float* fixed_scale;  // device scalar: fixed-point units per unit of gradient
 };
+// the absgrad instantiations' own arguments (sgn_blend_bwd_absgrad): a separate kernel parameter type, so that every other
+// kernel keeps its parameter layout (and its code) unchanged
+struct BlendBwdAbsParams {
+    BlendBwdParams p;
+    float* v_absxy;       // [N,2] absolute screen-space gradient (float mode: accumulated into)
+    long long* fx_absxy;  // deterministic mode: [N,2] fixed-point accumulators on the xy grid (or null)
+};
+template <bool ABS>
+using BlendBwdArgs = typename std::conditional<ABS, BlendBwdAbsParams, BlendBwdParams>::type;
+__host__ __device__ __forceinline__ const BlendBwdParams& bwd_base(const BlendBwdParams& p) { return p; }
+__host__ __device__ __forceinline__ const BlendBwdParams& bwd_base(const BlendBwdAbsParams& q) { return q.p; }
 
 // Deterministic mode: how many binary places the fixed-point grid of record component idx (= row * 12 + component) gives
 // up, from the Gaussian's own record.  A conic gradient is a sum of 1/2 dx^2 v_sigma (dx dy, 1/2 dy^2) over the pixels the
@@ -1010,6 +1021,24 @@ __device__ __forceinline__ void accumulate_grad(const BlendBwdParams& p, float f
         atomicAdd(reinterpret_cast<unsigned long long*>(p.v_fixed) + idx, (unsigned long long)__float2ll_rn(m));
     } else {
         atomicAdd(p.v_records + idx, v);
+    }
+}
+
+// Absolute screen-space gradient (sgn_blend_bwd_absgrad): absgrad[k] = (sum_p |g_x(k,p)|, sum_p |g_y(k,p)|), g(k,p) the
+// gradient of pixel p's main-stream outputs (rgb, accumulation, depth) with respect to row k's screen-space mean -- the
+// per-pixel terms whose signed sum is v_records[k, 0:2].  Deterministic mode puts it on the xy components' grid (shift 0,
+// the same fixed_scale): each addend is the absolute value of an addend whose signed form v_records' xy accumulation
+// already takes on that grid, so the terms need no more room than v_xy's do; only their cancellation is gone.  The total
+// is at most (pixels covered) x (largest term): a term is |vs| |J| with |J| <= sqrt(2 ln 255) / sigma_min <= 6.2 px^-1
+// (valid pixels lie within Mahalanobis distance^2 2 ln 255, and the projection's 0.3 px^2 blur keeps sigma_min >= 0.55
+// px) and |vs| <= |v_alpha|, a few max|cotangent| (colours <= 1, T <= 1).  One row covering a whole 1920 x 1280 image
+// therefore sums to below 2^27 max|cotangent| = 2^59 grid units, under the 2^63 of int64.
+template <bool DET>
+__device__ __forceinline__ void accumulate_abs(const BlendBwdAbsParams& q, float fscale, size_t idx, float v) {
+    if constexpr (DET) {
+        atomicAdd(reinterpret_cast<unsigned long long*>(q.fx_absxy) + idx, (unsigned long long)__float2ll_rn(v * fscale));
+    } else {
+        atomicAdd(q.v_absxy + idx, v);
     }
 }
 
@@ -1102,12 +1131,14 @@ __device__ __forceinline__ void acc_bwd_traverse(const BlendBwdParams& p, const 
 }
 
 // DEPTHG: the depth output has a cotangent.  OBJ: object_acc has one; its gradient is folded into the main traversal
-// (see below).
+// (see below).  ABS: the absolute screen-space gradient as well (accumulate_abs), from the main stream's share of each
+// slot's d/d sigma, taken before the objects-only fold.
 // (Measured and dropped: software-pipelining the reduction of entry t-1 under the arithmetic of entry t -- it
 // has to run unconditionally, which costs more than the overlap gains: 0.87 vs 0.82 ms on cfg3.)
-template <int PPL, bool DEPTHG, bool PACK, bool OBJ, bool DET>
-__device__ __forceinline__ void blend_bwd_strip(const BlendBwdParams& p, int tile, int strip, const int2 range,
+template <int PPL, bool DEPTHG, bool PACK, bool OBJ, bool DET, bool ABS>
+__device__ __forceinline__ void blend_bwd_strip(const BlendBwdArgs<ABS>& args, int tile, int strip, const int2 range,
                                                 float4 (*sA)[32], float4 (*sB)[32], float4 (*sC)[32]) {
+    const BlendBwdParams& p = bwd_base(args);
     const int tx = tile % p.tiles_x, ty = tile / p.tiles_x;
     const int lane = threadIdx.x;
     const int j = tx * SGN_TILE + (lane & 15);
@@ -1204,6 +1235,7 @@ __device__ __forceinline__ void blend_bwd_strip(const BlendBwdParams& p, int til
     int buf = 0;
     constexpr int NV = DEPTHG ? 10 : 9;
     const int my_comp = multi_reduce_slot<NV>(lane);
+    const int abs_comp = ABS ? multi_reduce_slot<2>(lane) : -1;
     const float clampb = in_register(p.clamp_bwd), nclamp = -clampb;
     const float fscale = DET ? __ldg(p.fixed_scale) : 0.f;
     constexpr bool PK = PACK && PPL >= 2;
@@ -1235,6 +1267,7 @@ __device__ __forceinline__ void blend_bwd_strip(const BlendBwdParams& p, int til
             const float o = Cc.w;
             float S0 = 0.f, Sy = 0.f, Syy = 0.f, cr = 0.f, cg = 0.f, cb = 0.f, cd = 0.f;
             float activity = 0.f;  // sum of alpha*T over the valid slots: non-zero iff some pixel of this lane took the entry
+            float gax = 0.f, gay = 0.f;  // ABS: sum over this lane's slots of |g_x|, |g_y|
             // OE (warp-uniform): an object entry, whose objects-only gradient is added here as well
             auto entry = [&](auto obj_tag) {
                 constexpr bool OE = decltype(obj_tag)::value;
@@ -1246,6 +1279,7 @@ __device__ __forceinline__ void blend_bwd_strip(const BlendBwdParams& p, int til
                     // (OE: a slot valid for the objects-only stream only masks the main terms with selects.)
                     f2 S0p = dup2(0.f), Syp = dup2(0.f), Syyp = dup2(0.f);
                     f2 ncr = dup2(0.f), ncg = dup2(0.f), ncb = dup2(0.f), ncd = dup2(0.f), nact = dup2(0.f);
+                    f2 gx2 = dup2(0.f), gy2 = dup2(0.f);
                     const f2 dyb = f2{dy0, dy0 - 2.f};
 #pragma unroll
                     for (int q = 0; q < NP; ++q) {
@@ -1275,8 +1309,15 @@ __device__ __forceinline__ void blend_bwd_strip(const BlendBwdParams& p, int til
                         }
                         f2 v_alpha = fma2(Tk, dotc, mul2(ram, d2[q]));
                         d2[q] = fma2(nfac, dotc, d2[q]);
+                        if (OE) v_alpha = f2{v0 ? v_alpha.x : 0.f, v1 ? v_alpha.y : 0.f};
+                        if constexpr (ABS) {  // |vs_main| |a dx + b dy|, |vs_main| |b dx + c dy|
+                            const f2 avs = f2{fabsf(nraw.x * v_alpha.x), fabsf(nraw.y * v_alpha.y)};
+                            const f2 jx = fma2(dup2(A.w * LN2), dy, dup2(A.z * (2.f * LN2) * dx));
+                            const f2 jy = fma2(dup2(B.x * (2.f * LN2)), dy, dup2(A.w * LN2 * dx));
+                            gx2 = fma2(avs, f2{fabsf(jx.x), fabsf(jx.y)}, gx2);
+                            gy2 = fma2(avs, f2{fabsf(jy.x), fabsf(jy.y)}, gy2);
+                        }
                         if (OE) {
-                            v_alpha = f2{v0 ? v_alpha.x : 0.f, v1 ? v_alpha.y : 0.f};
                             v_alpha = fma2(ra, f2{o0 ? tfo[2 * q] : 0.f, o1 ? tfo[2 * q + 1] : 0.f}, v_alpha);
                             nact = add2(nact, f2{o0 ? nal.x : 0.f, o1 ? nal.y : 0.f});
                         }
@@ -1290,6 +1331,7 @@ __device__ __forceinline__ void blend_bwd_strip(const BlendBwdParams& p, int til
                     cr = -(ncr.x + ncr.y); cg = -(ncg.x + ncg.y); cb = -(ncb.x + ncb.y);
                     if (DEPTHG) cd = -(ncd.x + ncd.y);
                     activity = nact.x + nact.y;
+                    if constexpr (ABS) { gax = gx2.x + gx2.y; gay = gy2.x + gy2.y; }
                 } else {
                 // straight-line, predicated (see the forward)
 #pragma unroll
@@ -1316,8 +1358,13 @@ __device__ __forceinline__ void blend_bwd_strip(const BlendBwdParams& p, int til
                     }
                     float v_alpha = __fmaf_rn(Tk, dotc, ra * (tfv[s] - bv[s]));
                     bv[s] = __fmaf_rn(fac, dotc, bv[s]);
+                    if (OE) v_alpha = valid ? v_alpha : 0.f;
+                    if constexpr (ABS) {  // |vs_main| |a dx + b dy|, |vs_main| |b dx + c dy|
+                        const float avs = valid ? fabsf(raw * v_alpha) : 0.f;
+                        gax = __fmaf_rn(avs, fabsf(__fmaf_rn(A.w * LN2, dy, A.z * (2.f * LN2) * dx)), gax);
+                        gay = __fmaf_rn(avs, fabsf(__fmaf_rn(B.x * (2.f * LN2), dy, A.w * LN2 * dx)), gay);
+                    }
                     if (OE) {
-                        v_alpha = valid ? v_alpha : 0.f;
                         v_alpha = ov ? __fmaf_rn(ra, tfo[s], v_alpha) : v_alpha;
                         activity += ov ? alpha : 0.f;
                     }
@@ -1350,6 +1397,11 @@ __device__ __forceinline__ void blend_bwd_strip(const BlendBwdParams& p, int til
             const size_t dst = (size_t)(__float_as_int(Cc.z) & ID_MASK) * SGN_RECORD_FLOATS + (my_comp >= 0 ? my_comp : 0);
             const float mine = warp_multi_reduce<NV>(comps, lane);
             if (my_comp >= 0) accumulate_grad<DET>(p, fscale, dst, mine);
+            if constexpr (ABS) {  // a reduction of its own: the NV-component one (and so v_records' bits) stays as it is
+                float ab[2] = {gax, gay};
+                const float amine = warp_multi_reduce<2>(ab, lane);
+                if (abs_comp >= 0) accumulate_abs<DET>(args, fscale, (size_t)(__float_as_int(Cc.z) & ID_MASK) * 2 + abs_comp, amine);
+            }
         }
         buf ^= 1;
     }
@@ -1366,8 +1418,9 @@ __device__ __forceinline__ void blend_bwd_strip(const BlendBwdParams& p, int til
 // the prologue (v_sky, cotangent chain) must run for every pixel, so strips are always launched for the
 // whole tile: W strips of 16/W rows.  OBJ: the strips are sized from the main depth plus how far the objects-only
 // streams run past it (tile_depth[object], see blend_fwd_strip).
-template <bool DEPTHG, bool PACK, bool OBJ, bool DET>
-__global__ void __launch_bounds__(32, BLEND_BWD_MIN_BLOCKS) blend_bwd_kernel(const BlendBwdParams p) {
+template <bool DEPTHG, bool PACK, bool OBJ, bool DET, bool ABS>
+__global__ void __launch_bounds__(32, BLEND_BWD_MIN_BLOCKS) blend_bwd_kernel(const BlendBwdArgs<ABS> args) {
+    const BlendBwdParams& p = bwd_base(args);
     __shared__ float4 sA[2][32];
     __shared__ float4 sB[2][32];
     __shared__ float4 sC[2][32];
@@ -1377,10 +1430,10 @@ __global__ void __launch_bounds__(32, BLEND_BWD_MIN_BLOCKS) blend_bwd_kernel(con
     const int W = strips_for(p.tile_depth[tile] + (OBJ ? p.tile_depth[(size_t)SLOT_OBJ * p.tiles + tile] : 0), p.split_main);
     if (strip >= W) return;
     switch (W) {
-        case 1: blend_bwd_strip<8, DEPTHG, PACK, OBJ, DET>(p, tile, strip, range, sA, sB, sC); break;
-        case 2: blend_bwd_strip<4, DEPTHG, PACK, OBJ, DET>(p, tile, strip, range, sA, sB, sC); break;
-        case 4: blend_bwd_strip<2, DEPTHG, PACK, OBJ, DET>(p, tile, strip, range, sA, sB, sC); break;
-        default: blend_bwd_strip<1, DEPTHG, PACK, OBJ, DET>(p, tile, strip, range, sA, sB, sC); break;
+        case 1: blend_bwd_strip<8, DEPTHG, PACK, OBJ, DET, ABS>(args, tile, strip, range, sA, sB, sC); break;
+        case 2: blend_bwd_strip<4, DEPTHG, PACK, OBJ, DET, ABS>(args, tile, strip, range, sA, sB, sC); break;
+        case 4: blend_bwd_strip<2, DEPTHG, PACK, OBJ, DET, ABS>(args, tile, strip, range, sA, sB, sC); break;
+        default: blend_bwd_strip<1, DEPTHG, PACK, OBJ, DET, ABS>(args, tile, strip, range, sA, sB, sC); break;
     }
 }
 
@@ -1440,9 +1493,16 @@ fixed_to_float_kernel(const long long* __restrict__ fx, const float* __restrict_
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = (float)(ldexp((double)fx[i], fixed_shift(records, (size_t)i)) / (double)scale[0]);
 }
+// the absgrad accumulators [N,2]: the xy grid, shift 0
+__global__ void __launch_bounds__(256)
+absxy_fixed_to_float_kernel(const long long* __restrict__ fx, const float* __restrict__ scale, float* __restrict__ out, long long n) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = (float)((double)fx[i] / (double)scale[0]);
+}
 
-template <bool DET>
-static int launch_blend_bwd(const BlendBwdParams& p, int tuning, cudaStream_t side, cudaStream_t stream) {
+template <bool DET, bool ABS>
+static int launch_blend_bwd(const BlendBwdArgs<ABS>& args, int tuning, cudaStream_t side, cudaStream_t stream) {
+    const BlendBwdParams& p = bwd_base(args);
     const unsigned acc_grid = p.tiles * 8;
     if (p.v_bg) {
         if (!(tuning & SGN_TUNE_ACC_NO_ROW_SKIP)) acc_bwd_kernel<true, DET><<<acc_grid, 32, 0, side>>>(p, 0);
@@ -1452,24 +1512,23 @@ static int launch_blend_bwd(const BlendBwdParams& p, int tuning, cudaStream_t si
     const bool pack = (tuning & SGN_TUNE_BWD_PACKED) != 0;
     const dim3 grid(p.tiles * 8), block(32);
     switch ((p.v_obj ? 4 : 0) | (p.v_depth ? 2 : 0) | (pack ? 1 : 0)) {
-        case 0: blend_bwd_kernel<false, false, false, DET><<<grid, block, 0, stream>>>(p); break;
-        case 1: blend_bwd_kernel<false, true, false, DET><<<grid, block, 0, stream>>>(p); break;
-        case 2: blend_bwd_kernel<true, false, false, DET><<<grid, block, 0, stream>>>(p); break;
-        case 3: blend_bwd_kernel<true, true, false, DET><<<grid, block, 0, stream>>>(p); break;
-        case 4: blend_bwd_kernel<false, false, true, DET><<<grid, block, 0, stream>>>(p); break;
-        case 5: blend_bwd_kernel<false, true, true, DET><<<grid, block, 0, stream>>>(p); break;
-        case 6: blend_bwd_kernel<true, false, true, DET><<<grid, block, 0, stream>>>(p); break;
-        default: blend_bwd_kernel<true, true, true, DET><<<grid, block, 0, stream>>>(p); break;
+        case 0: blend_bwd_kernel<false, false, false, DET, ABS><<<grid, block, 0, stream>>>(args); break;
+        case 1: blend_bwd_kernel<false, true, false, DET, ABS><<<grid, block, 0, stream>>>(args); break;
+        case 2: blend_bwd_kernel<true, false, false, DET, ABS><<<grid, block, 0, stream>>>(args); break;
+        case 3: blend_bwd_kernel<true, true, false, DET, ABS><<<grid, block, 0, stream>>>(args); break;
+        case 4: blend_bwd_kernel<false, false, true, DET, ABS><<<grid, block, 0, stream>>>(args); break;
+        case 5: blend_bwd_kernel<false, true, true, DET, ABS><<<grid, block, 0, stream>>>(args); break;
+        case 6: blend_bwd_kernel<true, false, true, DET, ABS><<<grid, block, 0, stream>>>(args); break;
+        default: blend_bwd_kernel<true, true, true, DET, ABS><<<grid, block, 0, stream>>>(args); break;
     }
     SGN_CHECK_LAUNCH("blend_bwd_kernel");
     return SGN_OK;
 }
 
-extern "C" int sgn_blend_bwd(const sgn_camera* cam, const sgn_blend_opts* opts, const float* records,
-                             const int32_t* sorted_ids, const int32_t* tile_bins, int64_t M, const int32_t* cls_ids,
-                             const int32_t* cls_bins, const sgn_blend_bwd_in* in, float* v_records, void* stream_) {
-    SGN_RANGE("sgn_blend_bwd");
-    cudaStream_t stream = (cudaStream_t)stream_;
+// sgn_blend_bwd, and sgn_blend_bwd_absgrad when v_absxy is set (its arguments checked by the caller)
+static int blend_bwd(const sgn_camera* cam, const sgn_blend_opts* opts, const float* records, const int32_t* sorted_ids,
+                     const int32_t* tile_bins, int64_t M, const int32_t* cls_ids, const int32_t* cls_bins, const sgn_blend_bwd_in* in,
+                     float* v_records, float* v_absxy, int64_t* fixed_absxy, cudaStream_t stream) {
     if (int rc = check_cam(cam)) return rc;
     SGN_REQUIRE(opts && records && tile_bins && in && v_records, "sgn_blend_bwd: null pointer");
     SGN_REQUIRE(in->raw && in->final_T && in->final_idx, "sgn_blend_bwd: saved forward state missing");
@@ -1527,8 +1586,15 @@ extern "C" int sgn_blend_bwd(const sgn_camera* cam, const sgn_blend_opts* opts, 
     {
         // all three kernels only accumulate (RED) into v_records: they may run concurrently
         ForkJoin fj(stream);
-        const int rc = in->v_fixed ? launch_blend_bwd<true>(p, opts->tuning, fj.side(), stream)
-                                   : launch_blend_bwd<false>(p, opts->tuning, fj.side(), stream);
+        int rc;
+        if (v_absxy) {
+            const BlendBwdAbsParams q{p, v_absxy, reinterpret_cast<long long*>(fixed_absxy)};
+            rc = in->v_fixed ? launch_blend_bwd<true, true>(q, opts->tuning, fj.side(), stream)
+                             : launch_blend_bwd<false, true>(q, opts->tuning, fj.side(), stream);
+        } else {
+            rc = in->v_fixed ? launch_blend_bwd<true, false>(p, opts->tuning, fj.side(), stream)
+                             : launch_blend_bwd<false, false>(p, opts->tuning, fj.side(), stream);
+        }
         fj.finish();
         if (rc) return rc;
     }
@@ -1537,8 +1603,38 @@ extern "C" int sgn_blend_bwd(const sgn_camera* cam, const sgn_blend_opts* opts, 
         fixed_to_float_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const long long*>(in->v_fixed), in->fixed_scale,
                                                                                 records, v_records, n);
         SGN_CHECK_LAUNCH("fixed_to_float_kernel");
+        if (fixed_absxy) {
+            const long long na = (long long)in->num_gaussians * 2;
+            absxy_fixed_to_float_kernel<<<(unsigned)((na + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const long long*>(fixed_absxy),
+                                                                                        in->fixed_scale, v_absxy, na);
+            SGN_CHECK_LAUNCH("absxy_fixed_to_float_kernel");
+        }
     }
     return SGN_OK;
+}
+
+extern "C" int sgn_blend_bwd(const sgn_camera* cam, const sgn_blend_opts* opts, const float* records,
+                             const int32_t* sorted_ids, const int32_t* tile_bins, int64_t M, const int32_t* cls_ids,
+                             const int32_t* cls_bins, const sgn_blend_bwd_in* in, float* v_records, void* stream) {
+    SGN_RANGE("sgn_blend_bwd");
+    return blend_bwd(cam, opts, records, sorted_ids, tile_bins, M, cls_ids, cls_bins, in, v_records, nullptr, nullptr,
+                     (cudaStream_t)stream);
+}
+
+extern "C" int sgn_blend_bwd_absgrad(const sgn_camera* cam, const sgn_blend_opts* opts, const float* records,
+                                     const int32_t* sorted_ids, const int32_t* tile_bins, int64_t M, const int32_t* cls_ids,
+                                     const int32_t* cls_bins, const sgn_blend_bwd_in* in, float* v_records, float* v_absxy,
+                                     int64_t* fixed_absxy, void* stream) {
+    SGN_RANGE("sgn_blend_bwd_absgrad");
+    SGN_REQUIRE(in, "sgn_blend_bwd_absgrad: null pointer");
+    SGN_REQUIRE(v_absxy && (reinterpret_cast<uintptr_t>(v_absxy) & 7u) == 0,
+                "sgn_blend_bwd_absgrad: v_absxy must be a non-null, 8-byte aligned [N,2] float array");
+    SGN_REQUIRE((fixed_absxy != nullptr) == (in->v_fixed != nullptr),
+                "sgn_blend_bwd_absgrad: fixed_absxy goes with v_fixed (deterministic mode), and only with it");
+    // the prologue folds v_background_acc into the main stream for the pixels whose background stream is the main one
+    SGN_REQUIRE(!in->v_background_acc, "sgn_blend_bwd_absgrad: v_background_acc must be null");
+    return blend_bwd(cam, opts, records, sorted_ids, tile_bins, M, cls_ids, cls_bins, in, v_records, v_absxy, fixed_absxy,
+                     (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -114,6 +114,12 @@ class SceneGraphConfig:
     object_mcmc: MCMCSettings = field(default_factory=lambda: MCMCSettings(cap_max=100_000))
     mcmc_opacity_reg: float = 0.01
     mcmc_scale_reg: float = 0.01
+    # gsplat's DefaultStrategy(absgrad=True) (AbsGS, Ye et al. 2024): the split / duplicate decision reads the norm of the
+    # absolute screen-space gradient, sum over pixels of |d out_p / d xy| (raster.RenderSettings.absgrad), against
+    # refine.densify_absgrad_thresh, instead of the norm of the signed sum against densify_grad_thresh.  A large Gaussian over
+    # texture, whose per-pixel gradients cancel in the signed sum, is then split.  Only the main stream's outputs (rgb,
+    # accumulation, depth) count.  strategy="default" only: MCMC keeps no densification statistics
+    absgrad: bool = False
 
     # ``stop_split_at`` of the BACKGROUND sub-model: what the reference's entropy gate reads
     # (``config.background_model.stop_split_at``, scene graph :386).  One source: ``refine.stop_split_at``.
@@ -154,6 +160,8 @@ class _FrameSlice:
         t = getattr(holder, self.name)[sl]
         if self.name == "xys" and holder.v_records is not None:  # after backward: the reference reads ``self.xys.grad``
             t.grad = holder.v_records[:, 0:2][sl]
+            if holder.v_absxy is not None:  # gsplat 1.x's means2d.absgrad
+                t.absgrad = holder.v_absxy[sl]
         if cache is None:
             cache = d["_fs_cache"] = {}
         cache[self.name] = t
@@ -407,6 +415,8 @@ class SceneGraphRasterModel(torch.nn.Module):
         raster.rasterize_mode_flag(self.config.rasterize_mode)  # an unknown mode raises ValueError, as the reference's does
         if self.config.strategy not in ("default", "mcmc"):
             raise ValueError(f"unknown densification strategy {self.config.strategy!r}: expected 'default' or 'mcmc'")
+        if self.config.absgrad and self.config.strategy != "default":
+            raise ValueError("absgrad needs strategy='default': the MCMC strategy keeps no densification statistics")
         # trainable camera poses (camera_pose.CameraPoseOptimizer, nerfstudio's attribute name).  None, or one in mode "off":
         # every camera is rendered as given, by the same calls as without it
         if camera_optimizer is not None and camera_optimizer.mode != "off" and sky is not None:
@@ -727,8 +737,10 @@ class SceneGraphRasterModel(torch.nn.Module):
         self.__dict__["_mcmc_reg"] = None
         if self._fused_mcmc_reg_due():
             kw["terms"] = (raster.MCMCRegTerm(self.config.mcmc_opacity_reg, self.config.mcmc_scale_reg),)
-        out, holder = raster.render_frame(frame, self._settings(class_streams=True), sky=sky, grad_sink=sink, anchor=anchor,
-                                          pose=pose, view=view, **kw)
+        settings = self._settings(class_streams=True)
+        # the absolute screen-space gradient for the densification statistics (after_train), in training renders only
+        settings.absgrad = self.config.absgrad and self.training and torch.is_grad_enabled()
+        out, holder = raster.render_frame(frame, settings, sky=sky, grad_sink=sink, anchor=anchor, pose=pose, view=view, **kw)
         if extra is not None:
             out["semantic"] = out.pop("extra")
         if "scale_reg" in kw:
@@ -876,7 +888,8 @@ class SceneGraphRasterModel(torch.nn.Module):
     def after_train(self, step: int) -> None:
         """The ``after_train`` callbacks of all visible sub-models (sgn_splatfacto.py:513-541; the scene graph
         registers one per sub-model, :127-137) as one launch of ``sgn_densify_stats`` over the frame's rows:
-        running ||xys.grad|| sums, visibility counts and the max screen-space radius ratio, per sub-model."""
+        running ||xys.grad|| sums, visibility counts and the max screen-space radius ratio, per sub-model.  With
+        ``absgrad`` (the render left ``holder.v_absxy``) ``sgn_densify_stats_abs`` sums ||xys.absgrad|| instead."""
         assert step == self.step
         h = self._holder
         if h is None or h.v_records is None or self.config.strategy == "mcmc":  # MCMC keeps no densification statistics
@@ -902,6 +915,10 @@ class SceneGraphRasterModel(torch.nn.Module):
             tab[j].max_2Dsize = sub.max_2Dsize.data_ptr()
         raw = torch.frombuffer(bytearray(bytes(tab)), dtype=torch.uint8).to(dev, non_blocking=True)
         H, W = self.last_size
+        if h.v_absxy is not None:
+            _lib.check(L.sgn_densify_stats_abs(raster._ptr(raw), len(slices), h.v_absxy.shape[0], raster._ptr(h.v_absxy),
+                                               raster._ptr(h.radii), H, W, raster._stream()), "sgn_densify_stats_abs")
+            return
         _lib.check(L.sgn_densify_stats(raster._ptr(raw), len(slices), h.v_records.shape[0], raster._ptr(h.v_records),
                                        raster._ptr(h.radii), H, W, raster._stream()), "sgn_densify_stats")
 
@@ -949,7 +966,7 @@ class SceneGraphRasterModel(torch.nn.Module):
             entry = None
             if densify or cull_only:
                 size = sub.last_size or self.last_size
-                cfg = refine.make_config(st, step, size, densify)
+                cfg = refine.make_config(st, step, size, densify, absgrad=self.config.absgrad)
                 g = sub.gauss_params
                 flags, scan = refine.decide_submodel(g["scales"].data, g["opacities"].data, sub.xys_grad_norm if densify else None,
                                                      sub.vis_counts if densify else None,
@@ -1171,6 +1188,8 @@ class SceneGraphRasterModel(torch.nn.Module):
                     if t is not None:
                         v_xy = h.v_records[:, 0:2] if v_xy is None else v_xy
                         t.grad = v_xy[sl]
+                        if h.v_absxy is not None:
+                            t.absgrad = h.v_absxy[sl]
         return hook
 
     # ------------------------------------------------------------------------------------------

@@ -48,6 +48,10 @@ class RenderSettings:
     # projection does not inflate sub-pixel Gaussians -- gsplat's antialiased mode.  Every stream that blends the records
     # (rgb, accumulation, depth, the class streams, the extra channels, the sky composite) follows, forward and backward
     rasterize_mode: str = "classic"
+    # gsplat's absgrad (AbsGS): the backward also accumulates the absolute screen-space gradient, sum over pixels of
+    # |d out_p / d xy| per row (sgn_blend_bwd_absgrad), into ``holder.v_absxy`` [N,2], from the main stream's outputs
+    # (rgb, accumulation, depth) only.  A background_acc cotangent is then refused.  Off: holder.v_absxy is None
+    absgrad: bool = False
 
 
 class StageTimer:
@@ -615,21 +619,29 @@ DETERMINISTIC = os.environ.get("SGN_DETERMINISTIC", "0") == "1"
 
 
 def blend_bwd(cs, bo, records, sorted_ids, tile_bins, saved: Dict[str, torch.Tensor], sky, v: Dict[str, Optional[torch.Tensor]],
-              want_v_sky: bool, obj_ids=None, obj_bins=None, deterministic: Optional[bool] = None):
-    """Returns (v_records[N,12], v_sky or None)."""
+              want_v_sky: bool, obj_ids=None, obj_bins=None, deterministic: Optional[bool] = None, absgrad: bool = False):
+    """Returns (v_records[N,12], v_sky or None); with ``absgrad``, (v_records, v_sky, v_absxy[N,2]) from
+    sgn_blend_bwd_absgrad (the same v_records and v_sky, plus the main stream's absolute screen-space gradient)."""
     L = _lib.load()
     device = records.device
     bi = _lib.BlendBwdIn()
     det = DETERMINISTIC if deterministic is None else deterministic
+    N = records.shape[0]
+    fixed_absxy = None
     if det:  # fixed-point accumulators (zeroed) + one float of scratch; v_records is then written, not accumulated into
         v_records = torch.empty_like(records)
-        v_fixed = torch.zeros(records.shape[0], _lib.RECORD_FLOATS, device=device, dtype=torch.int64)
+        v_fixed = torch.zeros(N, _lib.RECORD_FLOATS, device=device, dtype=torch.int64)
         fixed_scale = torch.empty(1, device=device, dtype=torch.float32)
-        bi.v_fixed, bi.fixed_scale, bi.num_gaussians = v_fixed.data_ptr(), fixed_scale.data_ptr(), records.shape[0]
+        bi.v_fixed, bi.fixed_scale, bi.num_gaussians = v_fixed.data_ptr(), fixed_scale.data_ptr(), N
+        if absgrad:
+            v_absxy = torch.empty(N, 2, device=device, dtype=torch.float32)
+            fixed_absxy = torch.zeros(N, 2, device=device, dtype=torch.int64)
     else:
         v_records = torch.zeros_like(records)
         bi.v_fixed = bi.fixed_scale = None
-        bi.num_gaussians = records.shape[0]
+        bi.num_gaussians = N
+        if absgrad:
+            v_absxy = torch.zeros(N, 2, device=device, dtype=torch.float32)
 
     def c(t):
         return None if t is None else t.contiguous()
@@ -646,6 +658,12 @@ def blend_bwd(cs, bo, records, sorted_ids, tile_bins, saved: Dict[str, torch.Ten
     bi.sky = sky.data_ptr() if sky is not None else None
     v_sky = torch.zeros(cs.height, cs.width, 3, device=device) if (want_v_sky and sky is not None) else None
     bi.v_sky = v_sky.data_ptr() if v_sky is not None else None
+    if absgrad:
+        with _timed("blend_bwd"):
+            _lib.check(L.sgn_blend_bwd_absgrad(C.byref(cs), C.byref(bo), _ptr(records), _ptr(sorted_ids), _ptr(tile_bins),
+                                               max(sorted_ids.shape[0], 1), _ptr(obj_ids), _ptr(obj_bins), C.byref(bi), _ptr(v_records),
+                                               _ptr(v_absxy), _ptr(fixed_absxy), _stream()), "sgn_blend_bwd_absgrad")
+        return v_records, v_sky, v_absxy
     with _timed("blend_bwd"):
         _lib.check(L.sgn_blend_bwd(C.byref(cs), C.byref(bo), _ptr(records), _ptr(sorted_ids), _ptr(tile_bins),
                                    max(sorted_ids.shape[0], 1), _ptr(obj_ids), _ptr(obj_bins), C.byref(bi), _ptr(v_records), _stream()),
@@ -882,6 +900,7 @@ class _Holder:
         self.xys = self.depths = self.radii = self.conics = self.num_tiles_hit = None
         self.records = None
         self.v_records = None
+        self.v_absxy = None  # [N,2] absolute screen-space gradient after a backward with RenderSettings.absgrad, else None
         self.grad_arena = None
         self.param_grads = None
         self.v_sky = None
@@ -979,9 +998,15 @@ class _SceneGraphRasterize(torch.autograd.Function):
         # only parameter terms have a cotangent (nothing in view, or a backward of the terms alone): every image-space gradient is
         # zero, so the blend and the projection are skipped and the arena starts from zeros
         params_only = bool(ctx.terms) and v_extra_img is None and all(t is None for t in vd.values())
-        v_extra = v_sky = None
+        v_extra = v_sky = v_absxy = None
         if params_only:
             v_records = torch.zeros_like(ctx.records)
+            if ctx.settings.absgrad:
+                v_absxy = torch.zeros(ctx.records.shape[0], 2, device=ctx.records.device, dtype=torch.float32)
+        elif ctx.settings.absgrad:
+            v_records, v_sky, v_absxy = blend_bwd(ctx.cs, ctx.bo, ctx.records, ctx.sorted_ids, ctx.tile_bins, ctx.saved, ctx.sky, vd,
+                                                  ctx.sky_needs_grad, ctx.obj_ids, ctx.obj_bins,
+                                                  deterministic=ctx.settings.deterministic, absgrad=True)
         else:
             v_records, v_sky = blend_bwd(ctx.cs, ctx.bo, ctx.records, ctx.sorted_ids, ctx.tile_bins, ctx.saved, ctx.sky, vd,
                                          ctx.sky_needs_grad, ctx.obj_ids, ctx.obj_bins, deterministic=ctx.settings.deterministic)
@@ -1030,6 +1055,7 @@ class _SceneGraphRasterize(torch.autograd.Function):
         h.params_only = params_only
         h.term_kinds = sorted({k for t, _ in due for k in t.kinds})
         h.v_records, h.grad_arena, h.v_pose, h.v_view = v_records, arena, v_pose, v_view
+        h.v_absxy = v_absxy
         if v_pose is not None:
             g_pose = v_pose[posed_rows(ctx.table)[0]]
         # the reference reads ``self.xys.grad`` after backward (densification statistics,
@@ -1081,13 +1107,20 @@ def forward_backward(frame: Frame, settings: RenderSettings, cotangents: Dict[st
         assert cotangents.get(n) is None or n in named, f"a {n} cotangent needs its term (scale_reg= / terms=)"
     # the terms' gradients are added after project_bwd: with ranges, the exchange of a range may already be reading it
     assert not terms or (chunk_ranges is None and after_range is None), "parameter terms do not combine with ranged exchange"
+    v_absxy = None
     if terms and all(t is None for t in v.values()):  # as the render's backward: nothing image-space to propagate
         v_records, v_sky = torch.zeros_like(records), None
+        if settings.absgrad:
+            v_absxy = torch.zeros(records.shape[0], 2, device=device, dtype=torch.float32)
         arena = _zero_arena(table.static, device, grad_out)
         flat = arena_views(arena, table.static) if want_param_grads else None
     else:
-        v_records, v_sky = blend_bwd(cs, bo, records, sorted_ids, tile_bins, out, sky, v, sky is not None, cls_ids, cls_bins,
-                                     deterministic=settings.deterministic)
+        if settings.absgrad:
+            v_records, v_sky, v_absxy = blend_bwd(cs, bo, records, sorted_ids, tile_bins, out, sky, v, sky is not None, cls_ids,
+                                                  cls_bins, deterministic=settings.deterministic, absgrad=True)
+        else:
+            v_records, v_sky = blend_bwd(cs, bo, records, sorted_ids, tile_bins, out, sky, v, sky is not None, cls_ids, cls_bins,
+                                         deterministic=settings.deterministic)
         flat, arena = project_bwd(table, params, cs, records, radii, v_records, make_views=want_param_grads, out=grad_out,
                                   chunk_ranges=chunk_ranges, after_range=after_range)
     for t, vt in zip(terms, v_terms):
@@ -1098,6 +1131,7 @@ def forward_backward(frame: Frame, settings: RenderSettings, cotangents: Dict[st
     holder.xys, holder.conics, holder.depths = records[:, 0:2], records[:, 2:5], records[:, 9]
     holder.table = table
     holder.v_records, holder.grad_arena, holder.v_sky = v_records, arena, v_sky
+    holder.v_absxy = v_absxy
     holder.param_grads = flat
     holder.tile_bins, holder.tile_depth = tile_bins, out["tile_depth"]  # diagnostics (tools/depth_stats.py)
     res = {k: out[k] for k in ("rgb", "accumulation", "depth", "object_acc", "background_acc") if k in out}

@@ -42,6 +42,10 @@ class RefineSettings:
     cull_scale_thresh: float = 0.2
     cull_screen_size: float = 0.15
     continue_cull_post_densification: bool = True
+    # the split / duplicate threshold with SceneGraphConfig.absgrad, against the absolute screen-space gradient (normalised
+    # alike, * 0.5 * max(H, W)): AbsGS's published value.  No measurement on street data backs it: tune it on the data (set
+    # it on the instance).  A plain attribute, not a field: the fields are the reference's SplatfactoModelConfig's
+    densify_absgrad_thresh = 0.0008
 
 
 SIZE_FAC = 1.6  # split_gaussians (:694)
@@ -63,14 +67,16 @@ def opacity_reset_logit(s: RefineSettings) -> float:
     return float(torch.logit(torch.tensor(s.cull_alpha_thresh * 2.0)).item())
 
 
-def make_config(s: RefineSettings, step: int, last_size: Tuple[int, int], densify: bool) -> _lib.RefineConfig:
+def make_config(s: RefineSettings, step: int, last_size: Tuple[int, int], densify: bool, absgrad: bool = False) -> _lib.RefineConfig:
+    """``absgrad``: the statistics are absolute screen-space gradients, thresholded at ``densify_absgrad_thresh``."""
     cfg = _lib.RefineConfig()
     cfg.densify = int(densify)
     cfg.n_split_samples = s.n_split_samples
     cfg.use_screen_size = int(step < s.stop_screen_size_at)
     cfg.cull_big = int(step > s.refine_every * s.reset_alpha_every)
     cfg.max_size = float(max(last_size[0], last_size[1]))
-    cfg.densify_grad_thresh, cfg.densify_size_thresh = s.densify_grad_thresh, s.densify_size_thresh
+    cfg.densify_grad_thresh = s.densify_absgrad_thresh if absgrad else s.densify_grad_thresh
+    cfg.densify_size_thresh = s.densify_size_thresh
     cfg.split_screen_size = s.split_screen_size
     cfg.cull_alpha_thresh, cfg.cull_scale_thresh, cfg.cull_screen_size = s.cull_alpha_thresh, s.cull_scale_thresh, s.cull_screen_size
     cfg.inv_size_fac = float(np.float32(1.0) / np.float32(SIZE_FAC))  # ATen: a / scalar == a * (1.f / (float)scalar)

@@ -28,7 +28,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True, sky: bool = False, metrics: bool = False,
         bbox_opt: bool = False, camera_opt: bool = False, sky_view_grad: bool = False, lidar_depth: float = 0.0,
         semantic: float = 0.0, antialiased: bool = False, scale_reg: bool = False, filter_3d: bool = False,
-        bilateral_grid: bool = False, mcmc: bool = False) -> dict:
+        bilateral_grid: bool = False, mcmc: bool = False, absgrad: bool = False) -> dict:
     """One measurement.  torch.distributed must already be initialised when WORLD_SIZE > 1.  Returns the result dict on
     rank 0 (None elsewhere).  ``sky``: the reference's default learnable sky (use_sky_sphere, a 1024^2 cube map stepped by
     the same Adam launch at the ``sky_sphere`` group's lr 0.005, sgn_config.py:72-75).  ``metrics``: every step also computes
@@ -52,7 +52,8 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     bilateral grid per rig image (425, bilagrid.BilateralGrid with gsplat's 16 x 16 x 8) corrects every training render, with
     the grids' total-variation term; stepped by the same Adam launch at gsplat's lr 2e-3.  ``mcmc``: densification by MCMC
     (SceneGraphConfig(strategy="mcmc"), gsplat's defaults with the actors' 100 k cap): no densification statistics, relocation
-    and 5 % growth at every refinement, position noise every step, the opacity and scale regularisers in the loss."""
+    and 5 % growth at every refinement, position noise every step, the opacity and scale regularisers in the loss.  ``absgrad``:
+    the split / duplicate decision reads the absolute screen-space gradient (SceneGraphConfig(absgrad=True))."""
     import torch
     import torch.distributed as dist
 
@@ -84,7 +85,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                            num_train_data=len(cams), refine_record=True, depth_loss_mult=lidar_depth,
                            semantic_classes=3 if semantic > 0 else 0, semantic_loss_mult=semantic,
                            rasterize_mode="antialiased" if antialiased else "classic", use_scale_regularization=scale_reg,
-                           filter_3d=filter_3d, strategy="mcmc" if mcmc else "default")
+                           filter_3d=filter_3d, strategy="mcmc" if mcmc else "default", absgrad=absgrad)
     env_map = None
     if sky:
         from street_gaussians_ns_b200.sky import CubeMapSky
@@ -264,6 +265,8 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                    **({"bilateral_grid": "BilateralGrid(425, 16 x 16 x 8), 10 * total variation, Adam lr 2e-3"} if bilateral_grid else {}),
                    **({"strategy": "mcmc: relocation + 5 % growth per refinement (caps 1 M / 100 k), noise every step, "
                                    "opacity and scale regularisers 0.01"} if mcmc else {}),
+                   **({"absgrad": "split / duplicate on the absolute screen-space gradient, densify_absgrad_thresh 0.0008"}
+                      if absgrad else {}),
                    "loss": "fused kernels" if fused_loss else "torch ops", "metrics": "get_metrics_dict every step" if metrics else "none",
                    "start_step": start_step, "refine_every": refine_every,
                    "refinement_kernels_loaded_before_timing": refine_warm,
@@ -307,6 +310,7 @@ def main():
     ap.add_argument("--filter-3d", action="store_true", help="Mip-Splatting's 3D smoothing filter from the 5 x 85 rig cameras")
     ap.add_argument("--bilateral-grid", action="store_true", help="a bilateral grid per rig image (425) corrects each training render")
     ap.add_argument("--mcmc", action="store_true", help="densification by MCMC (SceneGraphConfig(strategy='mcmc'))")
+    ap.add_argument("--absgrad", action="store_true", help="densify on absolute screen-space gradients (SceneGraphConfig(absgrad=True))")
     args = ap.parse_args()
     if args.sky_view_grad and not (args.sky and args.camera_opt):
         ap.error("--sky-view-grad needs --sky and --camera-opt")
@@ -323,7 +327,8 @@ def main():
               args.overlap, not args.host_table, ssim_lambda=args.ssim_lambda, fused_loss=not args.torch_loss, sky=args.sky,
               metrics=args.metrics, bbox_opt=args.bbox_opt, camera_opt=args.camera_opt,
               sky_view_grad=args.sky_view_grad, lidar_depth=args.lidar_depth, semantic=args.semantic, antialiased=args.antialiased,
-              scale_reg=args.scale_reg, filter_3d=args.filter_3d, bilateral_grid=args.bilateral_grid, mcmc=args.mcmc)
+              scale_reg=args.scale_reg, filter_3d=args.filter_3d, bilateral_grid=args.bilateral_grid, mcmc=args.mcmc,
+              absgrad=args.absgrad)
     if res is not None:
         print(json.dumps(res))
     if world > 1:
