@@ -15,6 +15,7 @@ import copy
 import ctypes as C
 import os
 from dataclasses import dataclass
+from types import SimpleNamespace
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -848,40 +849,34 @@ def project_bwd(table: SegmentTable, params: List[List[torch.Tensor]], cs, recor
         assert out is not None and not make_views
     gt = _arena_grads_table(arena, st, device, out_offsets)
     flat = arena_views(arena, st) if make_views else None
+    if chunk_ranges is None:
+        chunk_ranges = [(0, table.num_chunks)]
     partials = None
     if v_pose is not None:
         assert v_pose.shape == (table.nseg, _lib.POSE_FLOATS) and v_pose.dtype == torch.float32 and v_pose.is_contiguous() and v_pose.device == device
         partials = torch.empty(max(table.num_chunks, 1), _lib.POSE_FLOATS, device=device, dtype=torch.float32)
-        if chunk_ranges is None:
-            chunk_ranges = [(0, table.num_chunks)]
     view_partials = None
     if v_view is not None:
         assert v_view.shape == (_lib.VIEW_FLOATS,) and v_view.dtype == torch.float32 and v_view.is_contiguous() and v_view.device == device
         view_partials = torch.empty(max(table.num_chunks, 1), _lib.VIEW_FLOATS, device=device, dtype=torch.float32)
-        if chunk_ranges is None:
-            chunk_ranges = [(0, table.num_chunks)]
     with _timed("project_bwd"):
-        if chunk_ranges is None:
-            _lib.check(L.sgn_project_bwd(_ptr(table.dev), _ptr(gt), table.nseg, table.N, table.num_chunks, C.byref(cs), _ptr(records),
-                                         _ptr(radii), _ptr(v_records), _stream()), "sgn_project_bwd")
-        else:
-            # range by range (data parallel): ``after_range(k)`` is called once range k's launch is enqueued -- the exchange of
-            # that range's slices starts there and overlaps the production of the next range (dp.SymmetricExchange)
-            for k, (c0, c1) in enumerate(chunk_ranges):
-                if view_partials is not None:
-                    _lib.check(L.sgn_project_bwd_view(_ptr(table.dev), _ptr(gt), table.nseg, table.N, table.num_chunks, C.byref(cs),
-                                                      _ptr(view), _ptr(records), _ptr(radii), _ptr(v_records), int(c0), int(c1),
-                                                      _ptr(partials), _ptr(view_partials), _stream()), "sgn_project_bwd_view")
-                elif partials is not None:
-                    _lib.check(L.sgn_project_bwd_pose(_ptr(table.dev), _ptr(gt), table.nseg, table.N, table.num_chunks, C.byref(cs),
-                                                      _ptr(records), _ptr(radii), _ptr(v_records), int(c0), int(c1), _ptr(partials),
-                                                      _stream()), "sgn_project_bwd_pose")
-                else:
-                    _lib.check(L.sgn_project_bwd_range(_ptr(table.dev), _ptr(gt), table.nseg, table.N, table.num_chunks, C.byref(cs),
-                                                       _ptr(records), _ptr(radii), _ptr(v_records), int(c0), int(c1), _stream()),
-                               "sgn_project_bwd_range")
-                if after_range is not None:
-                    after_range(k)
+        # range by range (data parallel): ``after_range(k)`` is called once range k's launch is enqueued -- the exchange of
+        # that range's slices starts there and overlaps the production of the next range (dp.SymmetricExchange)
+        for k, (c0, c1) in enumerate(chunk_ranges):
+            if view_partials is not None:
+                _lib.check(L.sgn_project_bwd_view(_ptr(table.dev), _ptr(gt), table.nseg, table.N, table.num_chunks, C.byref(cs),
+                                                  _ptr(view), _ptr(records), _ptr(radii), _ptr(v_records), int(c0), int(c1),
+                                                  _ptr(partials), _ptr(view_partials), _stream()), "sgn_project_bwd_view")
+            elif partials is not None:
+                _lib.check(L.sgn_project_bwd_pose(_ptr(table.dev), _ptr(gt), table.nseg, table.N, table.num_chunks, C.byref(cs),
+                                                  _ptr(records), _ptr(radii), _ptr(v_records), int(c0), int(c1), _ptr(partials),
+                                                  _stream()), "sgn_project_bwd_pose")
+            else:
+                _lib.check(L.sgn_project_bwd_range(_ptr(table.dev), _ptr(gt), table.nseg, table.N, table.num_chunks, C.byref(cs),
+                                                   _ptr(records), _ptr(radii), _ptr(v_records), int(c0), int(c1), _stream()),
+                           "sgn_project_bwd_range")
+            if after_range is not None:
+                after_range(k)
         if partials is not None:
             _lib.check(L.sgn_pose_grad_reduce(_ptr(table.dev), table.nseg, table.num_chunks, _ptr(partials), _ptr(v_pose), _stream()),
                        "sgn_pose_grad_reduce")
@@ -919,6 +914,120 @@ class _Holder:
         self.term_kinds: List[int] = []
 
 
+IMAGE_NAMES = ("rgb", "accumulation", "depth", "object_acc", "background_acc")
+
+
+def _output_names(settings: RenderSettings, extra: Optional[torch.Tensor], terms: Sequence[ParamTerm]) -> List[str]:
+    """The names of a frame's outputs in the order the render node returns them: the images (the two class streams only with
+    ``class_streams``), ``extra`` with extra channels, then each term's outputs."""
+    names = list(IMAGE_NAMES if settings.class_streams else IMAGE_NAMES[:3])
+    if extra is not None:
+        names.append("extra")
+    return names + [n for t in terms for n in t.names]
+
+
+class _FramePass(SimpleNamespace):
+    """One frame's forward as its backward reads it: the launch structs (cs, bo), the table and parameters, the projection's
+    records / radii / tiles_hit, the tile lists and class sub-lists, the blend buffers the backward replays (``saved``, not
+    the images), sky, view, extra and terms.  ``outputs``: the forward's outputs in ``_output_names`` order, for the caller
+    to hand out."""
+
+    def fill(self, h: _Holder) -> None:
+        """The side-effect attributes of ``h`` that the forward sets."""
+        h.records, h.radii, h.num_tiles_hit, h.M, h.table = self.records, self.radii, self.tiles_hit, self.M, self.table
+        h.xys, h.conics, h.depths = self.records[:, 0:2], self.records[:, 2:5], self.records[:, 9]
+
+
+def _forward(frame: Frame, settings: RenderSettings, params: List[List[torch.Tensor]], sky: Optional[torch.Tensor],
+             extra: Optional[torch.Tensor], pose: Optional[torch.Tensor], view: Optional[torch.Tensor], terms: Sequence[ParamTerm],
+             after_project=None) -> _FramePass:
+    """The forward of one frame, the one place its stages are called: project, bin, class sub-lists, blend, the extra
+    channels, the terms.  ``after_project(radii)`` runs between the projection and the binning."""
+    device = params[0][0].device
+    K = (settings.sh_degree + 1) ** 2
+    for ps in params:
+        if ps[4].shape[1] != K - 1:
+            raise _lib.SgnError(f"features_rest has {ps[4].shape[1]} coefficients, sh_degree={settings.sh_degree} needs {K - 1}")
+    cs = camera_struct(frame.camera, settings)
+    if sky is not None:
+        sky = sky.contiguous()
+        assert sky.shape == (cs.height, cs.width, 3)
+    bo = blend_opts(settings, sky is not None)
+    table = SegmentTable(frame, params, device)
+    if pose is not None:
+        table = with_poses(table, pose)
+    if view is not None:
+        view = check_view(view, device)
+    proj = project_fwd(table, cs, device, view)
+    records, radii, tiles_hit, _ = proj
+    if after_project is not None:  # data parallel: the rows this replica sees are published early (dp.SymmetricExchange)
+        after_project(radii)
+    M, sorted_ids, tile_bins = bin_and_sort(cs, records, radii, proj=proj, async_binning=settings.async_binning)
+    cls_ids = cls_bins = None
+    if settings.class_streams:
+        cls_ids, cls_bins = class_lists(cs, M, sorted_ids, tile_bins)
+    out = blend_fwd(cs, bo, records, sorted_ids, tile_bins, sky, cls_ids, cls_bins)
+    outputs = [out[k] for k in IMAGE_NAMES if k in out]
+    if extra is not None:  # generic per-Gaussian channels composited with the main render's weights, 8 per traversal
+        assert extra.dim() == 2 and extra.shape[0] == records.shape[0] and extra.dtype == torch.float32 and extra.is_cuda
+        extra = extra.contiguous().detach()
+        outputs.append(blend_extra_fwd(cs, bo, records, sorted_ids, tile_bins, out["final_T"], out["final_idx"], extra))
+    for t in terms:  # terms of the parameters alone (the scale regularisation, ...), from the frame's table
+        outputs += t.forward(table)
+    # "sched", the heavy-first work lists' scratch, is saved too: the backward rebuilds its schedule in it
+    saved = {k: out[k] for k in ("raw", "final_T", "final_idx", "tile_depth", "sched") if k in out}
+    return _FramePass(settings=settings, cs=cs, bo=bo, table=table, params=params, records=records, radii=radii, tiles_hit=tiles_hit,
+                      M=M, sorted_ids=sorted_ids, tile_bins=tile_bins, cls_ids=cls_ids, cls_bins=cls_bins, saved=saved, sky=sky,
+                      view=view, extra=extra, terms=terms, outputs=outputs)
+
+
+def _backward(st: _FramePass, v: Dict[str, Optional[torch.Tensor]], v_extra_img: Optional[torch.Tensor],
+              v_terms: Sequence[Sequence[Optional[torch.Tensor]]], want_v_sky: bool, want_v_pose: bool,
+              out: Optional[torch.Tensor] = None, out_offsets: Optional[np.ndarray] = None, make_views: bool = False,
+              chunk_ranges=None, after_range=None) -> SimpleNamespace:
+    """The backward of one frame, the one place its stages are called: blend, extra channels, projection, then the terms'
+    gradients added into the arena.  ``v``: the image cotangents by name; ``v_terms``: one list per term; the arena
+    arguments are project_bwd's.  Returns v_records, v_sky, v_absxy (with ``settings.absgrad``), v_extra, arena, views (with
+    ``make_views``), v_pose ([nseg, 16] with ``want_v_pose``), v_view (the view's [15] cotangent when the forward had a
+    view), params_only and term_kinds; a params-only backward has no v_pose or v_view."""
+    # the terms' gradients are added after project_bwd: with ranges, the exchange of a range may already be reading the arena
+    assert not st.terms or (chunk_ranges is None and after_range is None), "parameter terms do not combine with ranged exchange"
+    s, table, device = st.settings, st.table, st.records.device
+    due = [(t, vt) for t, vt in zip(st.terms, v_terms) if any(x is not None for x in vt)]
+    # only parameter terms have a cotangent (nothing in view, or a backward of the terms alone): every image-space gradient is
+    # zero, so the blend and the projection are skipped and the arena starts from zeros
+    params_only = bool(st.terms) and v_extra_img is None and all(t is None for t in v.values())
+    v_sky = v_absxy = v_extra = v_pose = v_view = None
+    if params_only:
+        v_records = torch.zeros_like(st.records)
+        if s.absgrad:
+            v_absxy = torch.zeros(st.records.shape[0], 2, device=device, dtype=torch.float32)
+        arena = _zero_arena(table.static, device, out)
+        views = arena_views(arena, table.static) if make_views else None
+    else:
+        res = blend_bwd(st.cs, st.bo, st.records, st.sorted_ids, st.tile_bins, st.saved, st.sky, v, want_v_sky, st.cls_ids,
+                        st.cls_bins, deterministic=s.deterministic, absgrad=s.absgrad)
+        v_records, v_sky = res[:2]
+        if s.absgrad:
+            v_absxy = res[2]
+        if v_extra_img is not None:  # adds the extra channels' share of the geometry gradients to v_records before project_bwd
+            v_extra = blend_extra_bwd(st.cs, st.bo, st.records, st.sorted_ids, st.tile_bins, st.saved["final_T"],
+                                      st.saved["final_idx"], st.extra, v_extra_img, v_records, deterministic=s.deterministic)
+        if want_v_pose:
+            v_pose = torch.empty(table.nseg, _lib.POSE_FLOATS, device=device, dtype=torch.float32)
+        # a render with a device view differentiates with that view and yields its cotangent (cam_pos, detached like the SH
+        # view direction, gets 0)
+        if st.view is not None:
+            v_view = torch.zeros(VIEW_LEN, device=device, dtype=torch.float32)
+        views, arena = project_bwd(table, st.params, st.cs, st.records, st.radii, v_records, make_views=make_views, out=out,
+                                   out_offsets=out_offsets, chunk_ranges=chunk_ranges, after_range=after_range, v_pose=v_pose,
+                                   view=st.view, v_view=None if v_view is None else v_view[:_lib.VIEW_FLOATS])
+    for t, vt in due:  # project_bwd overwrote the arena: the terms' gradients are added after it
+        t.backward(table, arena, vt, out_offsets)
+    return SimpleNamespace(v_records=v_records, v_sky=v_sky, v_absxy=v_absxy, v_extra=v_extra, arena=arena, views=views, v_pose=v_pose,
+                           v_view=v_view, params_only=params_only, term_kinds=sorted({k for t, _ in due for k in t.kinds}))
+
+
 class _SceneGraphRasterize(torch.autograd.Function):
     @staticmethod
     def forward(ctx, frame: Frame, settings: RenderSettings, holder: _Holder, sky: Optional[torch.Tensor],
@@ -934,136 +1043,43 @@ class _SceneGraphRasterize(torch.autograd.Function):
         else:
             assert len(flat) == 6 * nseg
             params = [list(flat[6 * i: 6 * i + 6]) for i in range(nseg)]
-        device = params[0][0].device
-        for seg, ps in zip(frame.segments, params):
-            K = (settings.sh_degree + 1) ** 2
-            if ps[4].shape[1] != K - 1:
-                raise _lib.SgnError(f"features_rest has {ps[4].shape[1]} coefficients, sh_degree={settings.sh_degree} needs {K - 1}")
-        cs = camera_struct(frame.camera, settings)
-        if sky is not None:
-            sky = sky.contiguous()
-            assert sky.shape == (cs.height, cs.width, 3)
-        bo = blend_opts(settings, sky is not None)
-        table = SegmentTable(frame, params, device)
-        if pose is not None:
-            table = with_poses(table, pose)
-        ctx.pose_needs_grad = pose is not None and pose.requires_grad
-        ctx.view_needs_grad = view is not None and view.requires_grad
-        if view is not None:
-            view = check_view(view, device)
-        ctx.view = view
-        proj = project_fwd(table, cs, device, view)
-        records, radii, tiles_hit, bbox = proj
-        M, sorted_ids, tile_bins = bin_and_sort(cs, records, radii, proj=proj, async_binning=settings.async_binning)
-        obj_ids = obj_bins = None
-        if settings.class_streams:
-            obj_ids, obj_bins = class_lists(cs, M, sorted_ids, tile_bins)
-        out = blend_fwd(cs, bo, records, sorted_ids, tile_bins, sky, obj_ids, obj_bins)
-        holder.records, holder.radii, holder.num_tiles_hit, holder.M = records, radii, tiles_hit, M
-        holder.xys, holder.conics, holder.depths = records[:, 0:2], records[:, 2:5], records[:, 9]
-        holder.table = table
-        ctx.frame, ctx.settings, ctx.holder = frame, settings, holder
-        ctx.cs, ctx.bo, ctx.table, ctx.params = cs, bo, table, params
-        ctx.saved = dict(raw=out["raw"], final_T=out["final_T"], final_idx=out["final_idx"], tile_depth=out["tile_depth"])
-        if "sched" in out:  # the heavy-first work lists' scratch: the backward rebuilds its schedule in it
-            ctx.saved["sched"] = out["sched"]
-        ctx.records, ctx.radii, ctx.sorted_ids, ctx.tile_bins, ctx.sky = records, radii, sorted_ids, tile_bins, sky
-        ctx.obj_ids, ctx.obj_bins = obj_ids, obj_bins
-        ctx.sky_needs_grad = sky is not None and sky.requires_grad
-        outs = [out["rgb"], out["accumulation"], out["depth"]]
-        if settings.class_streams:
-            outs += [out["object_acc"], out["background_acc"]]
-        ctx.extra = None
-        if extra is not None:  # generic per-Gaussian channels composited with the main render's weights, 8 per traversal
-            assert extra.dim() == 2 and extra.shape[0] == records.shape[0] and extra.dtype == torch.float32 and extra.is_cuda
-            extra = extra.contiguous()
-            ctx.extra = extra.detach()
-            outs.append(blend_extra_fwd(cs, bo, records, sorted_ids, tile_bins, out["final_T"], out["final_idx"], ctx.extra))
-        ctx.terms = terms
-        for t in terms:  # terms of the parameters alone (the scale regularisation, ...), from the frame's table
-            outs += t.forward(table)
+        st = _forward(frame, settings, params, sky, extra, pose, view, terms)
+        st.fill(holder)
+        outs, st.outputs = st.outputs, None  # until the backward the node keeps the blend buffers, not the images
+        ctx.st, ctx.holder = st, holder
         return tuple(outs)
 
     @staticmethod
     def backward(ctx, *v):
-        v_extra_img = None
-        n_terms = sum(len(t.names) for t in ctx.terms)
-        v_terms = _split_term_cotangents(ctx.terms, v[len(v) - n_terms:])
-        v = v[:len(v) - n_terms]
-        due = [(t, vt) for t, vt in zip(ctx.terms, v_terms) if any(x is not None for x in vt)]
-        if ctx.extra is not None:
-            v, v_extra_img = v[:-1], v[-1]
-        names = ["rgb", "accumulation", "depth", "object_acc", "background_acc"][: len(v)]
-        vd = {k: t for k, t in zip(names, v)}
-        # only parameter terms have a cotangent (nothing in view, or a backward of the terms alone): every image-space gradient is
-        # zero, so the blend and the projection are skipped and the arena starts from zeros
-        params_only = bool(ctx.terms) and v_extra_img is None and all(t is None for t in vd.values())
-        v_extra = v_sky = v_absxy = None
-        if params_only:
-            v_records = torch.zeros_like(ctx.records)
-            if ctx.settings.absgrad:
-                v_absxy = torch.zeros(ctx.records.shape[0], 2, device=ctx.records.device, dtype=torch.float32)
-        elif ctx.settings.absgrad:
-            v_records, v_sky, v_absxy = blend_bwd(ctx.cs, ctx.bo, ctx.records, ctx.sorted_ids, ctx.tile_bins, ctx.saved, ctx.sky, vd,
-                                                  ctx.sky_needs_grad, ctx.obj_ids, ctx.obj_bins,
-                                                  deterministic=ctx.settings.deterministic, absgrad=True)
-        else:
-            v_records, v_sky = blend_bwd(ctx.cs, ctx.bo, ctx.records, ctx.sorted_ids, ctx.tile_bins, ctx.saved, ctx.sky, vd,
-                                         ctx.sky_needs_grad, ctx.obj_ids, ctx.obj_bins, deterministic=ctx.settings.deterministic)
-        if v_extra_img is not None:  # adds the extra channels' share of the geometry gradients to v_records before project_bwd
-            v_extra = blend_extra_bwd(ctx.cs, ctx.bo, ctx.records, ctx.sorted_ids, ctx.tile_bins, ctx.saved["final_T"],
-                                      ctx.saved["final_idx"], ctx.extra, v_extra_img, v_records,
-                                      deterministic=ctx.settings.deterministic)
-        h = ctx.holder
+        st, h = ctx.st, ctx.holder
+        _, _, _, want_v_sky, _, want_v_pose, want_v_view = ctx.needs_input_grad[:7]
+        names = _output_names(st.settings, st.extra, ())
+        vd = dict(zip(names, v))
+        v_extra_img = vd.pop("extra", None)
         sink = h.grad_sink
-        v_pose = g_pose = None
-        if ctx.pose_needs_grad:
-            v_pose = torch.empty(ctx.table.nseg, _lib.POSE_FLOATS, device=v_records.device, dtype=torch.float32)
-        # a render with a device view differentiates with that view and yields its cotangent (cam_pos, detached like the SH
-        # view direction, gets 0)
-        view = ctx.view
-        g_view = torch.zeros(VIEW_LEN, device=v_records.device, dtype=torch.float32) if view is not None else None
-        v_view = g_view[:_lib.VIEW_FLOATS] if g_view is not None else None
+        target = offsets = chunk_ranges = after_range = None
         if sink is not None:
-            target = sink.target(ctx.table.static, v_records.device)
-            offsets = sink.grad_offsets(ctx.table.static) if target is not None else None  # None: the frame's own layout
-            if params_only:
-                arena = _zero_arena(ctx.table.static, v_records.device, target)
-            else:
-                chunk_ranges = after_range = None
+            target = sink.target(st.table.static, st.records.device)
+            if target is not None:
+                offsets = sink.grad_offsets(st.table.static)  # None: the frame's own layout
                 plan = getattr(sink, "exchange_plan", None)  # data parallel: the arena is produced and exchanged range by range
-                if plan is not None and target is not None:
-                    chunk_ranges, after_range = plan(ctx.table)
-                _, arena = project_bwd(ctx.table, ctx.params, ctx.cs, ctx.records, ctx.radii, v_records, make_views=False,
-                                       out=target, out_offsets=offsets, chunk_ranges=chunk_ranges, after_range=after_range,
-                                       v_pose=v_pose, view=view, v_view=v_view)
-            for t, vt in due:  # project_bwd overwrote the arena: the terms' gradients are added after it
-                t.backward(ctx.table, arena, vt, offsets)
-            sink.publish(arena, ctx.table.static)
-            flat = (None,)
-        else:
-            if params_only:
-                arena = _zero_arena(ctx.table.static, v_records.device)
-                flat = arena_views(arena, ctx.table.static)
-            else:
-                flat, arena = project_bwd(ctx.table, ctx.params, ctx.cs, ctx.records, ctx.radii, v_records, v_pose=v_pose, view=view,
-                                          v_view=v_view)
-            for t, vt in due:
-                t.backward(ctx.table, arena, vt)
-        if params_only:  # no image term reached the poses or the view
-            v_pose = v_view = None
-        h.params_only = params_only
-        h.term_kinds = sorted({k for t, _ in due for k in t.kinds})
-        h.v_records, h.grad_arena, h.v_pose, h.v_view = v_records, arena, v_pose, v_view
-        h.v_absxy = v_absxy
-        if v_pose is not None:
-            g_pose = v_pose[posed_rows(ctx.table)[0]]
+                if plan is not None:
+                    chunk_ranges, after_range = plan(st.table)
+        g = _backward(st, vd, v_extra_img, _split_term_cotangents(st.terms, v[len(names):]), want_v_sky, want_v_pose, out=target,
+                      out_offsets=offsets, make_views=sink is None, chunk_ranges=chunk_ranges, after_range=after_range)
+        if sink is not None:
+            sink.publish(g.arena, st.table.static)
+        h.params_only, h.term_kinds = g.params_only, g.term_kinds
+        h.v_records, h.grad_arena, h.v_pose, h.v_absxy = g.v_records, g.arena, g.v_pose, g.v_absxy
+        h.v_view = None if g.v_view is None else g.v_view[:_lib.VIEW_FLOATS]
         # the reference reads ``self.xys.grad`` after backward (densification statistics,
         # sgn_splatfacto.py:520-524): xys is a view of the record array, its gradient a view of v_records
-        h.xys.grad = v_records[:, 0:2]
+        h.xys.grad = g.v_records[:, 0:2]
         if h.post_backward is not None:
             h.post_backward(h)
-        return (None, None, None, v_sky, v_extra, g_pose, g_view if ctx.view_needs_grad and not params_only else None, None, *flat)
+        g_pose = None if g.v_pose is None else g.v_pose[posed_rows(st.table)[0]]
+        flat = (None,) if sink is not None else g.views
+        return (None, None, None, g.v_sky, g.v_extra, g_pose, g.v_view if want_v_view else None, None, *flat)
 
 
 def forward_backward(frame: Frame, settings: RenderSettings, cotangents: Dict[str, Optional[torch.Tensor]],
@@ -1079,65 +1095,23 @@ def forward_backward(frame: Frame, settings: RenderSettings, cotangents: Dict[st
     ``holder.grad_arena`` is the flat dense gradient arena (what the data-parallel all-reduce and a
     fused optimizer consume), ``holder.v_records[:, 0:2]`` the pixel-space mean gradients the
     densification statistics read.  With ``want_param_grads`` the per-parameter views are returned in
-    ``holder.param_grads``.  Same kernels and same arithmetic as ``render_frame`` + ``backward()``.
+    ``holder.param_grads``.  The same forward and backward as ``render_frame`` + ``backward()``, with the sky's gradient
+    (``holder.v_sky``) always computed.
     ``grad_out``: a persistent arena to write into (data parallel: a symmetric allocation); ``chunk_ranges`` / ``after_range``:
-    see ``project_bwd``."""
-    params = [seg.params.tensors() for seg in frame.segments]
-    device = params[0][0].device
-    cs = camera_struct(frame.camera, settings)
-    if sky is not None:
-        sky = sky.contiguous()
-    bo = blend_opts(settings, sky is not None)
-    table = SegmentTable(frame, params, device)
-    proj = project_fwd(table, cs, device)
-    records, radii, tiles_hit, bbox = proj
-    if after_project is not None:  # data parallel: the rows this replica sees are published early (dp.SymmetricExchange)
-        after_project(radii)
-    M, sorted_ids, tile_bins = bin_and_sort(cs, records, radii, proj=proj, async_binning=settings.async_binning)
-    cls_ids = cls_bins = None
-    if settings.class_streams:
-        cls_ids, cls_bins = class_lists(cs, M, sorted_ids, tile_bins)
-    out = blend_fwd(cs, bo, records, sorted_ids, tile_bins, sky, cls_ids, cls_bins)
+    see ``project_bwd``; ``after_project(radii)``: called between the projection and the binning."""
     terms = _terms_of(scale_reg, terms)
-    regs = [t.forward(table) for t in terms]
-    v = {k: cotangents.get(k) for k in ("rgb", "accumulation", "depth", "object_acc", "background_acc")}
-    v_terms = [[cotangents.get(n) for n in t.names] for t in terms]
+    st = _forward(frame, settings, [seg.params.tensors() for seg in frame.segments], sky, None, None, None, terms, after_project)
     named = {n for t in terms for n in t.names}
     for n in _TERM_NAMES:
         assert cotangents.get(n) is None or n in named, f"a {n} cotangent needs its term (scale_reg= / terms=)"
-    # the terms' gradients are added after project_bwd: with ranges, the exchange of a range may already be reading it
-    assert not terms or (chunk_ranges is None and after_range is None), "parameter terms do not combine with ranged exchange"
-    v_absxy = None
-    if terms and all(t is None for t in v.values()):  # as the render's backward: nothing image-space to propagate
-        v_records, v_sky = torch.zeros_like(records), None
-        if settings.absgrad:
-            v_absxy = torch.zeros(records.shape[0], 2, device=device, dtype=torch.float32)
-        arena = _zero_arena(table.static, device, grad_out)
-        flat = arena_views(arena, table.static) if want_param_grads else None
-    else:
-        if settings.absgrad:
-            v_records, v_sky, v_absxy = blend_bwd(cs, bo, records, sorted_ids, tile_bins, out, sky, v, sky is not None, cls_ids,
-                                                  cls_bins, deterministic=settings.deterministic, absgrad=True)
-        else:
-            v_records, v_sky = blend_bwd(cs, bo, records, sorted_ids, tile_bins, out, sky, v, sky is not None, cls_ids, cls_bins,
-                                         deterministic=settings.deterministic)
-        flat, arena = project_bwd(table, params, cs, records, radii, v_records, make_views=want_param_grads, out=grad_out,
-                                  chunk_ranges=chunk_ranges, after_range=after_range)
-    for t, vt in zip(terms, v_terms):
-        if any(x is not None for x in vt):
-            t.backward(table, arena, vt)
+    g = _backward(st, {k: cotangents.get(k) for k in IMAGE_NAMES}, None, [[cotangents.get(n) for n in t.names] for t in terms],
+                  sky is not None, False, out=grad_out, make_views=want_param_grads, chunk_ranges=chunk_ranges, after_range=after_range)
     holder = _Holder()
-    holder.records, holder.radii, holder.num_tiles_hit, holder.M = records, radii, tiles_hit, M
-    holder.xys, holder.conics, holder.depths = records[:, 0:2], records[:, 2:5], records[:, 9]
-    holder.table = table
-    holder.v_records, holder.grad_arena, holder.v_sky = v_records, arena, v_sky
-    holder.v_absxy = v_absxy
-    holder.param_grads = flat
-    holder.tile_bins, holder.tile_depth = tile_bins, out["tile_depth"]  # diagnostics (tools/depth_stats.py)
-    res = {k: out[k] for k in ("rgb", "accumulation", "depth", "object_acc", "background_acc") if k in out}
-    for t, r in zip(terms, regs):
-        res.update(zip(t.names, r))
-    return res, holder
+    st.fill(holder)
+    holder.v_records, holder.grad_arena, holder.v_sky, holder.v_absxy = g.v_records, g.arena, g.v_sky, g.v_absxy
+    holder.param_grads = g.views
+    holder.tile_bins, holder.tile_depth = st.tile_bins, st.saved["tile_depth"]  # diagnostics (tools/depth_stats.py)
+    return dict(zip(_output_names(settings, None, terms), st.outputs)), holder
 
 
 def blend_extra_fwd(cs, bo, records, sorted_ids, tile_bins, final_T, final_idx, extra: torch.Tensor) -> torch.Tensor:
@@ -1221,17 +1195,7 @@ def render_frame(frame: Frame, settings: Optional[RenderSettings] = None, sky: O
     flat = [anchor] if grad_sink is not None else [t for seg in frame.segments for t in seg.params.tensors()]
     terms = _terms_of(scale_reg, terms)
     outs = _SceneGraphRasterize.apply(frame, settings, holder, sky, extra, pose, view, terms, *flat)
-    n_terms = sum(len(t.names) for t in terms)
-    regs = outs[len(outs) - n_terms:]
-    outs = outs[:len(outs) - n_terms]
-    extra_img = None
-    if extra is not None:
-        outs, extra_img = outs[:-1], outs[-1]
-    names = ["rgb", "accumulation", "depth", "object_acc", "background_acc"][: len(outs)]
-    out = {k: t for k, t in zip(names, outs)}
-    if extra_img is not None:
-        out["extra"] = extra_img
-    out.update(zip([n for t in terms for n in t.names], regs))
+    out = dict(zip(_output_names(settings, extra, terms), outs))
     if sky is not None:
         out["sky"] = sky
     return out, holder
