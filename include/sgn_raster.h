@@ -559,6 +559,24 @@ size_t sgn_sizeof_adam_tensor(void);
 int sgn_adam_chunk_elems(void);
 int sgn_adam_step(const sgn_adam_tensor* table_dev, int ntensors, int num_chunks, const float* grad_arena,
                   float* exp_avg, float* exp_avg_sq, void* stream);
+/* Selective Adam (gsplat's visible_adam, Taming 3DGS): sgn_adam_step restricted to the rows a frame saw.  `rows_dev` is a
+ * DEVICE table parallel to `table_dev` (8-byte aligned).  Element e of tensor i belongs to row e / row_width and is stepped
+ * when visible[flag_row0 + e / row_width] != 0; flag_row0 = -1 steps the tensor densely.  A stepped element gets exactly
+ * sgn_adam_step's update; for any other element the parameter and both moments are neither read nor written.  Every tensor
+ * holds fewer than 2^31 elements.  `visible` (uint8, one byte per row, e.g. sgn_visible_flags of the frame's radii) is
+ * required even when every tensor is dense. */
+typedef struct sgn_adam_rows {
+    int64_t flag_row0; /* the byte of the tensor's row 0 in `visible`; -1: dense */
+    int32_t row_width; /* elements per row (numel / rows) */
+    int32_t pad;
+} sgn_adam_rows;
+size_t sgn_sizeof_adam_rows(void);
+int sgn_adam_step_visible(const sgn_adam_tensor* table_dev, const sgn_adam_rows* rows_dev, int ntensors, int num_chunks,
+                          const float* grad_arena, float* exp_avg, float* exp_avg_sq, const uint8_t* visible, void* stream);
+/* seen[segs[s][1] + j] |= flags[segs[s][0] + j] for j < segs[s][2], for the n bytes of `flags`: a frame's visibility bytes
+ * folded into a mask kept across frames, one launch for all segments.  `segs_dev`: DEVICE int64 [nseg][3] (src_row0,
+ * dst_row0, rows), 8-byte aligned, src_row0 non-decreasing; bytes of `flags` behind a segment's rows are ignored. */
+int sgn_visible_or(const int64_t* segs_dev, int nseg, int64_t n, const uint8_t* flags, uint8_t* seen, void* stream);
 
 /* ---- gradient exchange of the camera-sharded data-parallel step (SURVEY.md 8e) ---------------------------------
  * The reference has no distributed code; SURVEY 8e defines the exchange: SUM (or mean) of the flat per-Gaussian gradient

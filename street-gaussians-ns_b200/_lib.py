@@ -81,6 +81,10 @@ class AdamTensor(C.Structure):
     ]
 
 
+class AdamRows(C.Structure):
+    _fields_ = [("flag_row0", C.c_int64), ("row_width", C.c_int32), ("pad", C.c_int32)]
+
+
 class DensifySegment(C.Structure):
     _fields_ = [
         ("row0", C.c_int32), ("count", C.c_int32), ("first", C.c_int32), ("pad", C.c_int32),
@@ -174,7 +178,7 @@ EXPORTS = [
     "sgn_bilagrid_slice_fwd", "sgn_bilagrid_slice_bwd_scratch_bytes", "sgn_bilagrid_slice_bwd", "sgn_bilagrid_tv_scratch_bytes",
     "sgn_bilagrid_tv_fwd", "sgn_bilagrid_tv_bwd", "sgn_sizeof_mcmc_sub", "sgn_sizeof_mcmc_tensors", "sgn_mcmc_noise",
     "sgn_mcmc_sample_scratch_bytes", "sgn_mcmc_sample", "sgn_mcmc_relocate", "sgn_mcmc_copy_rows", "sgn_mcmc_reg_scratch_bytes",
-    "sgn_mcmc_reg_fwd", "sgn_mcmc_reg_bwd",
+    "sgn_mcmc_reg_fwd", "sgn_mcmc_reg_bwd", "sgn_sizeof_adam_rows", "sgn_adam_step_visible", "sgn_visible_or",
 ]
 VIEW_FLOATS = 12  # SGN_VIEW_FLOATS: the view's cotangent, viewmat[12] row-major; the device view itself is 12 + 3 (cam_pos) floats
 POSE_FLOATS = 16  # SGN_POSE_FLOATS: a segment's pose (and its cotangent) as R[9] row-major, t[3], q[4]
@@ -350,6 +354,10 @@ def load():
     L.sgn_adam_chunk_elems.restype = C.c_int
     L.sgn_adam_step.argtypes = [vp, i32, i32, vp, vp, vp, vp]
     L.sgn_adam_step.restype = C.c_int
+    L.sgn_sizeof_adam_rows.restype = sz
+    L.sgn_adam_step_visible.argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, vp]
+    L.sgn_visible_or.argtypes = [vp, i32, i64, vp, vp, vp]
+    L.sgn_adam_step_visible.restype = L.sgn_visible_or.restype = C.c_int
     L.sgn_sizeof_refine_config.restype = sz
     L.sgn_sizeof_refine_tensors.restype = sz
     L.sgn_refine_decide.argtypes = [i32, C.POINTER(RefineConfig), vp, vp, vp, vp, vp, vp, vp, vp]
@@ -359,6 +367,7 @@ def load():
     assert L.sgn_sizeof_refine_config() == C.sizeof(RefineConfig), "sgn_refine_config layout mismatch"
     assert L.sgn_sizeof_refine_tensors() == C.sizeof(RefineTensors), "sgn_refine_tensors layout mismatch"
     assert L.sgn_sizeof_adam_tensor() == C.sizeof(AdamTensor), "sgn_adam_tensor layout mismatch"
+    assert L.sgn_sizeof_adam_rows() == C.sizeof(AdamRows), "sgn_adam_rows layout mismatch"
     assert L.sgn_sizeof_segment() == C.sizeof(Segment), "sgn_segment layout mismatch between header and ctypes"
     assert L.sgn_sizeof_segment_grads() == C.sizeof(SegmentGrads)
     assert L.sgn_sizeof_camera() == C.sizeof(CameraStruct), "sgn_camera layout mismatch"

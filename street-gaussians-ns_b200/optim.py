@@ -35,6 +35,9 @@ ADAM_DTYPE = np.dtype([("param", "<u8"), ("arena_offset", "<i8"), ("grad_offset"
                        ("beta1", "<f4"), ("beta2", "<f4"), ("eps", "<f4"), ("step_size", "<f4"),
                        ("sqrt_bc2", "<f4"), ("one_minus_beta1", "<f4"), ("one_minus_beta2", "<f4")])
 assert ADAM_DTYPE.itemsize == C.sizeof(_lib.AdamTensor) == 64
+# sgn_adam_rows: the row table of the selective step, parallel to the sgn_adam_tensor rows (flag_row0 = -1: dense)
+ADAM_ROWS_DTYPE = np.dtype([("flag_row0", "<i8"), ("row_width", "<i4"), ("pad", "<i4")])
+assert ADAM_ROWS_DTYPE.itemsize == C.sizeof(_lib.AdamRows) == 16
 
 
 def padded(numel: int) -> int:
@@ -140,6 +143,11 @@ class FusedAdam:
         self._extra_ptrs = {t.data_ptr() for t, _ in self._extra.values()}
         self._extra_ptrs |= {t.data_ptr() for ts, _ in self._rows.values() for t in ts}  # addressed relative to the arena too
         self._lr_vec = np.array([self.lrs[k] for k in self.kinds], np.float64)
+        # per tensor, for the selective step: the sub-model whose rows it holds (-1: an extra tensor) and its row width
+        self._sub_of = np.array([i // 6 if i < 6 * len(params) else -1 for i in range(len(flat))], np.int64)
+        for name, i0 in self.row_index.items():
+            self._sub_of[i0:i0 + len(params)] = np.arange(len(params))
+        self._width = np.array([t.numel() // t.shape[0] if t.dim() and t.shape[0] else 1 for t in flat], np.int64)
 
     def extra_tensors(self) -> Dict[str, torch.Tensor]:
         """The further tensors this optimizer steps (``extra``), by name."""
@@ -168,14 +176,22 @@ class FusedAdam:
     def step_table(self, present: Optional[Sequence[int]] = None, full_layout: bool = False, grad_arena: Optional[torch.Tensor] = None,
                    extra_grads: Optional[Dict[str, torch.Tensor]] = None,
                    row_grads: Optional[Dict[str, Sequence[Optional[torch.Tensor]]]] = None,
-                   kinds: Optional[Sequence[int]] = None) -> np.ndarray:
+                   kinds: Optional[Sequence[int]] = None, visible: bool = False,
+                   row_flag_row0: Optional[Dict[str, Sequence[int]]] = None):
         """Advance the step counts of the tensors that have a gradient and return their sgn_adam_tensor rows.
         ``present``: indices of the sub-models that have a gradient this step (None = all).  The gradient arena
         either holds exactly those, back to back in that order (a frame's arena, the default), or has the optimizer's
         own layout with the absent sub-models' slices unused (``full_layout``: the data-parallel arena, model.py).
         ``kinds``: which of a present sub-model's six tensors (PARAM_NAMES positions) have a gradient (None = all six); the
         arena keeps its layout, the other tensors are skipped -- moments, step counts and values untouched, as torch.optim.Adam
-        skips a parameter whose ``grad`` is None."""
+        skips a parameter whose ``grad`` is None.
+
+        ``visible``: return ``(tab, rows)``, with the parallel sgn_adam_rows table of the selective step.  The flags are in the
+        frame's row order -- the present sub-models back to back, in ``present``'s order (None: all, in the optimizer's order)
+        -- so a present sub-model's tensors, and its tensors of the row groups, start at the sum of the row counts of the present
+        sub-models before it; the extra tensors are dense (flag_row0 = -1).  ``row_flag_row0``: name of a row group -> per
+        sub-model the flag byte of its row 0, in place of the frame's (a mask kept across frames, training.py); a row-group
+        tensor with a gradient whose sub-model is not present needs one."""
         extras = []
         if self.extra_index:  # rows of the extra tensors that have a gradient this step
             assert not extra_grads or grad_arena is not None, "extra_grads need grad_arena (their offsets are relative to it)"
@@ -227,18 +243,59 @@ class FusedAdam:
         b1, b2 = self.betas
         tab["step_size"] = self._lr_vec[idx] / (1.0 - b1 ** st)   # lr / bias_correction1, in double like torch
         tab["sqrt_bc2"] = np.sqrt(1.0 - b2 ** st)
-        return tab
+        if not visible:
+            assert row_flag_row0 is None, "row_flag_row0 belongs to the selective step (visible=True)"
+            return tab
+        return tab, self._flag_rows(tab, idx, present, row_flag_row0)
+
+    def _flag_rows(self, tab: np.ndarray, idx, present: Optional[Sequence[int]],
+                   row_flag_row0: Optional[Dict[str, Sequence[int]]]) -> np.ndarray:
+        """The sgn_adam_rows table of ``tab`` (whose rows are the optimizer's tensors ``idx``), see step_table."""
+        tidx = np.arange(len(self._params), dtype=np.int64)[idx]
+        pres = list(range(self.num_segments)) if present is None else list(present)
+        frame_row0 = np.full(self.num_segments, -1, np.int64)
+        if pres:
+            n = np.array([self._params[6 * s].shape[0] for s in pres], np.int64)
+            frame_row0[pres] = np.concatenate([[0], np.cumsum(n)[:-1]])
+        sub = self._sub_of[tidx]
+        f0 = np.where(sub >= 0, frame_row0[np.maximum(sub, 0)], -1)
+        for name, r0s in (row_flag_row0 or {}).items():
+            i0 = self.row_index[name]
+            sel = (tidx >= i0) & (tidx < i0 + self.num_segments)
+            r0s = np.asarray(r0s, np.int64)
+            assert r0s.shape == (self.num_segments,) and np.all(r0s >= 0), (name, r0s)
+            f0[sel] = r0s[tidx[sel] - i0]
+        if np.any((sub >= 0) & (f0 < 0)):
+            raise ValueError("visible: a row-group tensor of a sub-model that is not in the frame needs row_flag_row0")
+        # the kernel indexes a tensor in 32 bits
+        assert int(tab["numel"].max(initial=0)) < 2 ** 31
+        rows = np.zeros(len(tab), ADAM_ROWS_DTYPE)
+        rows["flag_row0"], rows["row_width"] = f0, self._width[tidx]
+        return rows
 
     def step(self, grad_arena: torch.Tensor, present: Optional[Sequence[int]] = None, full_layout: bool = False,
              extra_grads: Optional[Dict[str, torch.Tensor]] = None,
-             row_grads: Optional[Dict[str, Sequence[Optional[torch.Tensor]]]] = None, kinds: Optional[Sequence[int]] = None) -> None:
+             row_grads: Optional[Dict[str, Sequence[Optional[torch.Tensor]]]] = None, kinds: Optional[Sequence[int]] = None,
+             visible: Optional[torch.Tensor] = None, row_flag_row0: Optional[Dict[str, Sequence[int]]] = None) -> None:
+        """``visible``: the selective step (gsplat's visible_adam): uint8 [frame rows], one byte per row of the frame in its
+        row order (``sgn_visible_flags`` of the frame's radii); a present sub-model's rows whose byte is 0 keep their
+        parameters and moments, bit for bit.  The step counts advance as in the dense step.  ``row_flag_row0``: see
+        step_table.  None: the dense step (``sgn_adam_step``)."""
         self.step_count += 1
         # the launch is asynchronous: keep the gradient tensors alive until the next step
         self._keep = extra_grads if row_grads is None else (extra_grads, row_grads)
-        self.launch(self.step_table(present, full_layout, grad_arena, extra_grads, row_grads, kinds), grad_arena)
+        if visible is None:
+            self.launch(self.step_table(present, full_layout, grad_arena, extra_grads, row_grads, kinds), grad_arena)
+            return
+        self._keep = (self._keep, visible)
+        tab, rows = self.step_table(present, full_layout, grad_arena, extra_grads, row_grads, kinds, visible=True,
+                                    row_flag_row0=row_flag_row0)
+        self.launch(tab, grad_arena, rows=rows, visible=visible)
 
-    def launch(self, tab: np.ndarray, grad_arena: torch.Tensor) -> None:
-        """One ``sgn_adam_step`` over the rows of ``tab`` (from step_table, possibly cut by rows_in_range)."""
+    def launch(self, tab: np.ndarray, grad_arena: torch.Tensor, rows: Optional[np.ndarray] = None,
+               visible: Optional[torch.Tensor] = None) -> None:
+        """One ``sgn_adam_step`` over the rows of ``tab`` (from step_table, possibly cut by rows_in_range); with ``rows`` and
+        ``visible`` one ``sgn_adam_step_visible``."""
         assert grad_arena.is_cuda, "FusedAdam runs on the CUDA library only"
         if len(tab) == 0:
             return
@@ -250,9 +307,24 @@ class FusedAdam:
             need = int((inside["grad_offset"] + inside["numel"]).max())
             assert grad_arena.numel() >= need, (grad_arena.numel(), need)
         num_chunks = int(tab["chunk0"][-1] + (int(tab["numel"][-1]) + self._chunk - 1) // self._chunk)
-        dev_tab = torch.from_numpy(np.ascontiguousarray(tab).view(np.uint8).reshape(-1)).to(self.device, non_blocking=True)
         stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
         L = _lib.load()
+        if rows is not None:
+            assert visible is not None and visible.is_cuda and visible.dtype == torch.uint8 and visible.is_contiguous()
+            assert len(rows) == len(tab)
+            masked = rows["flag_row0"] >= 0
+            if masked.any():  # every row of a masked tensor has its byte
+                last = rows["flag_row0"][masked] + (tab["numel"][masked] + rows["row_width"][masked] - 1) // rows["row_width"][masked]
+                assert int(last.max()) <= visible.numel(), (int(last.max()), visible.numel())
+            # one upload: the tensor table, then the row table (16-byte aligned behind it)
+            raw = np.concatenate([np.ascontiguousarray(tab).view(np.uint8).reshape(-1), np.ascontiguousarray(rows).view(np.uint8).reshape(-1)])
+            dev = torch.from_numpy(raw).to(self.device, non_blocking=True)
+            _lib.check(L.sgn_adam_step_visible(C.c_void_p(dev.data_ptr()), C.c_void_p(dev.data_ptr() + tab.nbytes), len(tab), num_chunks,
+                                               C.c_void_p(grad_arena.data_ptr()), C.c_void_p(self.exp_avg.data_ptr()),
+                                               C.c_void_p(self.exp_avg_sq.data_ptr()), C.c_void_p(visible.data_ptr()), stream),
+                       "sgn_adam_step_visible")
+            return
+        dev_tab = torch.from_numpy(np.ascontiguousarray(tab).view(np.uint8).reshape(-1)).to(self.device, non_blocking=True)
         _lib.check(L.sgn_adam_step(C.c_void_p(dev_tab.data_ptr()), len(tab), num_chunks,
                                    C.c_void_p(grad_arena.data_ptr()), C.c_void_p(self.exp_avg.data_ptr()),
                                    C.c_void_p(self.exp_avg_sq.data_ptr()), stream), "sgn_adam_step")

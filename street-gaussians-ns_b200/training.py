@@ -18,6 +18,7 @@ from __future__ import annotations
 
 from typing import Dict, List, Optional, Sequence
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -31,7 +32,8 @@ class TrainStep:
     def __init__(self, model: SceneGraphRasterModel, optimizer: FusedAdam, refine_every: Optional[int] = None,
                  group: Optional[dist.ProcessGroup] = None, pipeline_chunks: int = 0, refine_seed: int = 0,
                  check_replicas: bool = True, overlap: bool = False, exchange: str = "auto", metrics: bool = False,
-                 gradient_accumulation_steps: Optional[Dict[str, int]] = None, filter_cameras: Optional[Sequence[Camera]] = None):
+                 gradient_accumulation_steps: Optional[Dict[str, int]] = None, filter_cameras: Optional[Sequence[Camera]] = None,
+                 visible_adam: bool = False):
         """``pipeline_chunks`` > 0 (data parallel only): all-reduce and Adam are pipelined over that many ranges of the
         arena (dp.allreduce_and_step) instead of running one after the other.  ``metrics``: every step calls
         ``model.get_metrics_dict`` between ``get_outputs`` and ``get_loss_dict`` (nerfstudio's order,
@@ -46,8 +48,19 @@ class TrainStep:
         ``filter_cameras`` (a model with ``SceneGraphConfig.filter_3d``): the training cameras the 3D smoothing filter is
         computed from -- on the first step, right after every refinement that changed a row count, and every
         ``filter_3d_every`` steps otherwise (Mip-Splatting's schedule).  Under data parallelism every replica computes the same
-        filter from the same full list, so nothing is exchanged."""
+        filter from the same full list, so nothing is exchanged.
+        ``visible_adam``: the selective Adam step (gsplat's ``visible_adam``, Taming 3DGS): a Gaussian whose radius is 0 in the
+        frame keeps its parameters and both moments, bit for bit, instead of moving on its decaying first moment.  The
+        visibility bytes are built on the device from the frame's radii (no read-back); a step with nothing in view leaves
+        every Gaussian untouched.  Accumulated row groups (``{"semantic": 10}``) step, at their due step, the rows seen in any
+        frame of their cycle.  Deliberately: the gradients of the regularisers (the scale regularisation, MCMC's terms) on rows
+        the camera did not see are dropped, as in gsplat; the refinement, MCMC's relocation and the moment carrying are
+        unchanged; the update keeps torch's bias correction with per-tensor step counts.  Single GPU only."""
         self.model, self.optimizer, self.group = model, optimizer, group
+        self.visible_adam = visible_adam
+        # the selective step's visibility bytes: the frame's flags at 0, then one per-row "seen" mask per accumulated row
+        # group (all sub-models back to back, in the optimizer's order); see _visible_flags
+        self._vis_buf, self._vis_counts, self._vis_keep = None, None, None
         self.accumulate = dict(gradient_accumulation_steps or {})
         unknown = sorted(set(self.accumulate) - set(optimizer.extra_tensors()) - set(optimizer.row_tensors()))
         if unknown or any(int(n) < 1 for n in self.accumulate.values()):
@@ -109,6 +122,9 @@ class TrainStep:
             # the relocation and growth would be exchanged as densification statistics are, and the regularisers' gradients reach
             # rows no replica saw
             raise NotImplementedError("data-parallel training does not support strategy='mcmc': the replicas would diverge")
+        if world > 1 and self.visible_adam:
+            # the replicas would have to step the union of every replica's rows, actors included
+            raise NotImplementedError("data-parallel training does not support visible_adam: the replicas would diverge")
         if world > 1:
             self._ensure_exchange()
         m.step = step                                     # step_cb (sgn_splatfacto.py:754-755)
@@ -169,8 +185,9 @@ class TrainStep:
                 base = next(iter(due.values()), None)
                 if base is None and due_rows:
                     base = next(g for gs in due_rows.values() for g in gs if g is not None)
+                vis = self._visible_flags(step, [], False) if self.visible_adam else {}
                 if base is not None:
-                    opt.step(base, present=[], full_layout=True, extra_grads=due or None, row_grads=due_rows or None)
+                    opt.step(base, present=[], full_layout=True, extra_grads=due or None, row_grads=due_rows or None, **vis)
                 self._maybe_refine(step)
                 self._inject_noise(step)
                 return losses
@@ -191,6 +208,11 @@ class TrainStep:
             if world > 1:
                 dp.allreduce_gradients(arena, average=True, group=self.group)
             kw = {"kinds": kinds} if kinds is not None else {}
+            if self.visible_adam:  # the flags are in the frame's row order: the present sub-models, in that order
+                h = m._holder
+                seen = rendered and not getattr(h, "params_only", False) and getattr(h, "radii", None) is not None
+                kw.update(self._visible_flags(step, present, seen))
+                everything = False
             if row_grads:
                 opt.step(arena, present=None if everything else present, full_layout=full, extra_grads=extra_grads or None,
                          row_grads=row_grads, **kw)
@@ -223,6 +245,62 @@ class TrainStep:
             if any(g is not None for g in gs):
                 out[name] = gs
         return out
+
+    def _visible_flags(self, step: int, present: Sequence[int], seen: bool) -> Dict[str, object]:
+        """The selective step's arguments of ``FusedAdam.step``: ``visible`` and, for the accumulated row groups, ``row_flag_row0``.
+        ``present``: the frame's sub-models in its row order; ``seen``: the frame was rendered with an image-space gradient, its
+        radii say which rows were seen (otherwise no row was).  The frame's bytes come from ``sgn_visible_flags`` (radii > 0),
+        one launch over its rows.  Each accumulated row group keeps a mask of the rows seen since its cycle started: zeroed where
+        the cycle starts (where its gradient is zeroed), OR-ed with the frame's bytes by one ``sgn_visible_or`` per step, and
+        started over for a sub-model whose tensor a refinement replaced (its accumulated gradient went with the old tensor)."""
+        import ctypes as C
+
+        from . import _lib
+        m, opt = self.model, self.optimizer
+        counts = [sub.num_points for sub in m.all_models.values()]
+        groups = [name for name in opt.row_tensors() if name in self.accumulate]
+        stride = (sum(counts) + 15) // 16 * 16
+        if self._vis_buf is None or self._vis_counts != counts or self._vis_keep is not None:
+            self._vis_relayout(counts, groups, stride)
+        buf, row0 = self._vis_buf, self._vis_row0
+        n = sum(counts[s] for s in present)
+        for k, name in enumerate(groups):
+            if step % self.accumulate[name] == 0:  # a cycle starts here: its gradient was zeroed before this frame
+                buf[stride * (1 + k):stride * (2 + k)].zero_()
+        if seen and n:
+            L, stream = _lib.load(), C.c_void_p(torch.cuda.current_stream().cuda_stream)
+            radii = m._holder.radii
+            assert radii.dtype == torch.int32 and radii.shape[0] == n, (radii.shape, n)
+            _lib.check(L.sgn_visible_flags(C.c_void_p(radii.data_ptr()), n, C.c_void_p(buf.data_ptr()), stream), "sgn_visible_flags")
+            frame0 = np.concatenate([[0], np.cumsum([counts[s] for s in present])[:-1]]).astype(np.int64)
+            for k, name in enumerate(groups):
+                segs = np.stack([frame0, stride * (1 + k) + row0[present], np.asarray([counts[s] for s in present], np.int64)], 1)
+                dev = torch.from_numpy(np.ascontiguousarray(segs)).to(buf.device, non_blocking=True)
+                self._vis_segs = dev  # the launch is asynchronous
+                _lib.check(L.sgn_visible_or(C.c_void_p(dev.data_ptr()), len(present), n, C.c_void_p(buf.data_ptr()),
+                                            C.c_void_p(buf.data_ptr()), stream), "sgn_visible_or")
+        elif n:
+            buf[:n].zero_()
+        out: Dict[str, object] = {"visible": buf}
+        if groups:
+            out["row_flag_row0"] = {name: (stride * (1 + k) + row0).tolist() for k, name in enumerate(groups)}
+        return out
+
+    def _vis_relayout(self, counts: List[int], groups: List[str], stride: int) -> None:
+        """A new flag buffer for the model's row counts; the masks of the sub-models whose row-group tensor was kept carry over."""
+        old, old_counts, old_row0, keep = self._vis_buf, self._vis_counts, getattr(self, "_vis_row0", None), self._vis_keep or set()
+        buf = torch.zeros(stride * (1 + len(groups)), dtype=torch.uint8, device=self.model.device)
+        row0 = np.concatenate([[0], np.cumsum(counts)[:-1]]).astype(np.int64)
+        if old is not None and old_counts is not None and len(old_counts) == len(counts):
+            old_stride = (sum(old_counts) + 15) // 16 * 16
+            for k, name in enumerate(groups):
+                if k >= len(self._vis_groups) or self._vis_groups[k] != name:
+                    continue
+                for s, c in enumerate(counts):
+                    if (name, s) in keep and c == old_counts[s] and c:
+                        a, b = old_stride * (1 + k) + int(old_row0[s]), stride * (1 + k) + int(row0[s])
+                        buf[b:b + c].copy_(old[a:a + c])
+        self._vis_buf, self._vis_counts, self._vis_row0, self._vis_groups, self._vis_keep = buf, list(counts), row0, list(groups), None
 
     def _ensure_exchange(self) -> None:
         """(Re)allocates the symmetric gradient arena when the model's layout changed (first step, after a refinement).
@@ -329,10 +407,14 @@ class TrainStep:
             self._maybe_filter(step, False)
             return
         m.__dict__["refine_changed_rows"] = False
+        before = self.optimizer.row_tensors() if self.visible_adam else {}
         if mc:
             m.refinement_after(self.optimizer, step, due_only=self.refine_every is None, seed=self.refine_seed)
         else:
             m.refinement_after(self.optimizer, step, generator=self._refine_generator(step), due_only=self.refine_every is None)
+        if self.visible_adam:  # the row-group tensors a refinement kept keep their "seen" masks (_visible_flags)
+            after = self.optimizer.row_tensors()
+            self._vis_keep = {(name, s) for name, ts in before.items() for s, t in enumerate(ts) if after[name][s] is t}
         self._maybe_filter(step, bool(m.__dict__.get("refine_changed_rows")))
         if self.world_size() > 1 and self.check_replicas:
             # replicas must have taken identical decisions: same row count in every sub-model

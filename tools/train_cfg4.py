@@ -28,7 +28,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         async_binning: bool = True, ssim_lambda: float = 0.0, fused_loss: bool = True, sky: bool = False, metrics: bool = False,
         bbox_opt: bool = False, camera_opt: bool = False, sky_view_grad: bool = False, lidar_depth: float = 0.0,
         semantic: float = 0.0, antialiased: bool = False, scale_reg: bool = False, filter_3d: bool = False,
-        bilateral_grid: bool = False, mcmc: bool = False, absgrad: bool = False) -> dict:
+        bilateral_grid: bool = False, mcmc: bool = False, absgrad: bool = False, visible_adam: bool = False) -> dict:
     """One measurement.  torch.distributed must already be initialised when WORLD_SIZE > 1.  Returns the result dict on
     rank 0 (None elsewhere).  ``sky``: the reference's default learnable sky (use_sky_sphere, a 1024^2 cube map stepped by
     the same Adam launch at the ``sky_sphere`` group's lr 0.005, sgn_config.py:72-75).  ``metrics``: every step also computes
@@ -53,7 +53,8 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
     the grids' total-variation term; stepped by the same Adam launch at gsplat's lr 2e-3.  ``mcmc``: densification by MCMC
     (SceneGraphConfig(strategy="mcmc"), gsplat's defaults with the actors' 100 k cap): no densification statistics, relocation
     and 5 % growth at every refinement, position noise every step, the opacity and scale regularisers in the loss.  ``absgrad``:
-    the split / duplicate decision reads the absolute screen-space gradient (SceneGraphConfig(absgrad=True))."""
+    the split / duplicate decision reads the absolute screen-space gradient (SceneGraphConfig(absgrad=True)).  ``visible_adam``:
+    the selective Adam step (TrainStep(visible_adam=True)): only the rows the step's camera saw are stepped."""
     import torch
     import torch.distributed as dist
 
@@ -124,7 +125,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
         accumulate = dict(accumulate or {}, semantic=10)
     opt = FusedAdam(model.optimizer_params(), extra=extra, reserve_spare=True, rows=rows)  # no cudaMalloc of moment arenas inside the training loop
     step_fn = TrainStep(model, opt, refine_every=refine_every, pipeline_chunks=pipeline_chunks, overlap=overlap, metrics=metrics,
-                        gradient_accumulation_steps=accumulate, filter_cameras=cams if filter_3d else None)
+                        gradient_accumulation_steps=accumulate, filter_cameras=cams if filter_3d else None, visible_adam=visible_adam)
     g = torch.Generator().manual_seed(5)
     gt = (torch.rand(H, W, 3, generator=g) * 255).to(torch.uint8).to(dev)  # get_loss_dict consumes uint8 directly
     counts0 = [sub.num_points for sub in model.all_models.values()]
@@ -267,6 +268,7 @@ def run(steps: int = 50, warmup: int = 5, scale: float = 1.0, refine_every: int 
                                    "opacity and scale regularisers 0.01"} if mcmc else {}),
                    **({"absgrad": "split / duplicate on the absolute screen-space gradient, densify_absgrad_thresh 0.0008"}
                       if absgrad else {}),
+                   **({"visible_adam": "selective Adam: only the rows with radius > 0 in the step's frame are stepped"} if visible_adam else {}),
                    "loss": "fused kernels" if fused_loss else "torch ops", "metrics": "get_metrics_dict every step" if metrics else "none",
                    "start_step": start_step, "refine_every": refine_every,
                    "refinement_kernels_loaded_before_timing": refine_warm,
@@ -311,6 +313,7 @@ def main():
     ap.add_argument("--bilateral-grid", action="store_true", help="a bilateral grid per rig image (425) corrects each training render")
     ap.add_argument("--mcmc", action="store_true", help="densification by MCMC (SceneGraphConfig(strategy='mcmc'))")
     ap.add_argument("--absgrad", action="store_true", help="densify on absolute screen-space gradients (SceneGraphConfig(absgrad=True))")
+    ap.add_argument("--visible-adam", action="store_true", help="selective Adam: step only the Gaussians the step's camera saw")
     args = ap.parse_args()
     if args.sky_view_grad and not (args.sky and args.camera_opt):
         ap.error("--sky-view-grad needs --sky and --camera-opt")
@@ -328,7 +331,7 @@ def main():
               metrics=args.metrics, bbox_opt=args.bbox_opt, camera_opt=args.camera_opt,
               sky_view_grad=args.sky_view_grad, lidar_depth=args.lidar_depth, semantic=args.semantic, antialiased=args.antialiased,
               scale_reg=args.scale_reg, filter_3d=args.filter_3d, bilateral_grid=args.bilateral_grid, mcmc=args.mcmc,
-              absgrad=args.absgrad)
+              absgrad=args.absgrad, visible_adam=args.visible_adam)
     if res is not None:
         print(json.dumps(res))
     if world > 1:
